@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- megapixels/s of HEIC-grid decode -> RGB on B200 (BASELINE.json metric), one JSON line on stdout.
+"""bench.py -- megapixels/s of HEIC-grid decode -> RGB on H100 (BASELINE.json metric), one JSON line on stdout.
 
 Workload (BASELINE configs[2]): a synthetic 16384x16384 HEIC grid = 256 independent 1024x1024 HEVC-intra tiles
 (8-bit 4:2:0, fixed QP 27, CTB 32, WPP, SAO + deblocking on; seed 0xB200 + tile index; SURVEY.md 8d) decoded to
@@ -16,6 +16,8 @@ interleaved RGB24.  One "step" = the whole grid once.
           holding the very same tiles (oracle/ref_arm.py, oracle/heic_writer.py) -- the whole 256-tile grid per step.
 Multi-GPU (torchrun, one rank per GPU): tile rows are sharded across ranks (strong scaling: the grid is fixed); the only
 collective is the final gather of RGB row bands to rank 0 (NCCL over NVLink) in the device-timed leg.
+--dump-outputs DIR: after the timed steps, writes what the last device-timed step delivered (the interleaved RGB24 picture)
+as float32 .npy files: rgb_tile0.npy = the top-left tile, rgb_sample.npy = a fixed, seeded sample of the whole picture.
 """
 import argparse
 import ctypes
@@ -70,9 +72,9 @@ def make_tiles(indices, tile=TILE, workers=None, log2_ctb=5):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons / power limit sampled DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, gpu_index):
         self.samples = []
@@ -86,7 +88,7 @@ class ClockSampler:
                 r = subprocess.run(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-i", str(self.idx)],
                                    stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=5)
                 f = [x.strip() for x in r.stdout.strip().split(",")]
-                if len(f) >= 7:
+                if len(f) >= 8:
                     self.samples.append(f)
             except Exception:
                 pass
@@ -102,14 +104,18 @@ class ClockSampler:
 
     def summary(self):
         if not self.samples:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["unsampled"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["unsampled"]}
         sm = sorted(int(float(s[0])) for s in self.samples)
         reasons = set()
         for s in self.samples:
             for name, v in zip(["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"], s[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
-        return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": int(float(self.samples[0][1])), "reasons": sorted(reasons), "samples": len(sm)}
+        try:
+            plim = float(self.samples[0][7])
+        except ValueError:
+            plim = None
+        return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": int(float(self.samples[0][1])), "power_limit_w": plim, "reasons": sorted(reasons), "samples": len(sm)}
 
 
 def effective_cores():
@@ -128,11 +134,18 @@ def effective_cores():
     return n
 
 
-def measured_peak():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return json.load(open(p))["hbm_gbs"], "MEASURED_PEAKS.json hbm_gbs (of measured)"
-    return 6650.0, "B200_PROFILING.md fallback 6.65 TB/s (of fallback)"
+HBM_PEAK_GBS = 3350.0    # H100 SXM data sheet: 3.35 TB/s HBM3 (a bound to compare with, never a measured figure)
+
+
+def dump_outputs(d, rgb):
+    """rgb: the (H, W * 3) uint8 picture on the device.  Writes float32 .npy files, 12 MB + at most 16 MB."""
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "rgb_tile0.npy"), rgb[:TILE, :TILE * 3].cpu().numpy().astype(np.float32))
+    flat = rgb.reshape(-1)
+    n = min(1 << 22, flat.numel())
+    idx = np.sort(np.random.default_rng(0x5EED).choice(flat.numel(), size=n, replace=False))
+    import torch
+    np.save(os.path.join(d, "rgb_sample.npy"), flat[torch.from_numpy(idx).to(flat.device)].cpu().numpy().astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------ reference CPU arm
@@ -159,16 +172,6 @@ def reference_arm(side, sub, steps, warmup, cores, dump=None, log2_ctb=5, extra=
     return res, None
 
 
-def load_traffic():
-    """dram__bytes_read + dram__bytes_write per launch of each kernel, from the ncu captures of THIS code committed under
-    profiles/ (profiles/r02_traffic.json names the capture each figure comes from); None when no capture exists."""
-    p = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    try:
-        return json.load(open(p))
-    except Exception:  # noqa: BLE001
-        return {}
-
-
 def main():
     if "B200_BENCH_TILE_CACHE" not in os.environ:
         import atexit
@@ -183,12 +186,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--tiles-side", type=int, default=16, help="grid is tiles-side x tiles-side tiles of 1024x1024 (16 = BASELINE config)")
-    ap.add_argument("--ref-sample-side", type=int, default=16, help="sub-grid the in-run parity check / cpu_baseline decodes with the reference (default: the whole 16 x 16 grid, ~2.4 s per decode on 16 cores)")
+    ap.add_argument("--ref-sample-side", type=int, default=16, help="sub-grid the in-run parity check / cpu_baseline decodes with the reference (default: the whole 16 x 16 grid)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-plugin-leg", action="store_true", help="skip the heif_decode_image + plugin legs (e2e_plugin, e2e_plugin_n2)")
     ap.add_argument("--no-ctb64", action="store_true", help="skip the additional CTB 64 measurement (x265's default CTB size)")
     ap.add_argument("--ctb", type=int, default=5, choices=[4, 5, 6], help="log2 CTB size of the synthetic tiles (5 = the benchmark workload)")
     ap.add_argument("--front-end", default="device", choices=["device", "host"], help="where CABAC runs: GPU (one warp per WPP sub-stream) or host cores")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last device-timed step computed as float32 .npy files into DIR")
     args = ap.parse_args()
     warmup = max(3, args.warmup)
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -293,10 +297,12 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
         for _ in range(args.steps):
-            device_step()
+            last = device_step()
         e1.record(stream)
         barrier()
         dev_ms = max_over_ranks(e0.elapsed_time(e1)) / args.steps
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last)
         # ---- leg B: end to end through the C ABI, host buffers in, page-locked host RGB out (wall clock around a synchronised region)
         barrier()
         t0 = time.perf_counter()
@@ -345,7 +351,7 @@ def main():
     # ---- rank 0: report
     pixels = W * H
     my_px = band_h * W
-    peak, peak_src = measured_peak()
+    props = torch.cuda.get_device_properties(dev)
     C = st0.command_bytes / my_px                                     # measured command-stream bytes per pixel
     bpp = st0.bitstream_bytes / my_px
     # algorithmic B/px (SURVEY.md 8(d), 8-bit): entropy reads the bitstream and writes the command stream once
@@ -357,14 +363,14 @@ def main():
         alg["entropy+recon"] = bpp + 1.5 + C         # bitstream read, planes written; the command stream stays in L2 / HBM in between
     dom = max(kern, key=kern.get)
     ach = alg[dom] * my_px / (kern[dom] * 1e-3) / 1e9
-    tr = load_traffic().get(dom) if (world == 1 and side == 16 and args.ctb == 5) else None      # the captures are of this exact workload
     bins = 2.0 * my_px                               # ~2.0 CABAC bins per pixel on this workload (1.57 context-coded + 0.43 bypass, counted by the host front-end)
     line = {
         "metric": "megapixels/sec HEIC-grid decode->RGB", "value": pixels / 1e6 / (dev_ms / 1e3), "unit": "MP/s", "n_gpus": world,
         "steps": args.steps, "warmup": warmup, "ms_per_step": dev_ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
         "dtype": "u8", "data": "synthetic",
         "config": {"workload": workload, "sharding": f"{world} x contiguous tile-row bands, NCCL gather of RGB bands to rank 0 (device leg); per-rank D2H into one shared page-locked host buffer (e2e leg)" if world > 1 else "single GPU",
-                   "l2": "inputs larger than L2 (command stream + planes > 126 MB per GPU)" if st0.command_bytes + my_px * 1.5 > 126e6 else "flush not needed: see note",
+                   "gpu": props.name, "sms": props.multi_processor_count,
+                   "l2": f"inputs larger than L2 (command stream + planes > {props.L2_cache_size / 1e6:.0f} MB per GPU)" if st0.command_bytes + my_px * 1.5 > props.L2_cache_size else "flush not needed: see note",
                    "bits_per_pixel": 8.0 * st0.bitstream_bytes / my_px, "command_bytes_per_pixel": C, "host_parser_threads": max(1, cores // world), "front_end": args.front_end + (" (CABAC on the GPU, one warp per WPP sub-stream)" if args.front_end == "device" else " (CABAC on the host cores)")},
         "e2e": {"value": pixels / 1e6 / (e2e_ms / 1e3), "unit": "MP/s", "ms_per_step": e2e_ms, "h2d_bytes_per_step": int(stats_e2e.h2d_bytes * (pixels / my_px)),
                 "d2h_bytes_per_step": pixels * 3, "host_parse_ms": stats_e2e.parse_ms, "host_pack_ms": stats_e2e.pack_ms,
@@ -376,9 +382,8 @@ def main():
                      "note": "e2e legs of large grids: the tile rows go through K1 -> K3 -> K4 -> K6 in row bands and the D2H of band c overlaps the kernels of band c + 1; K1 is queued behind the full-occupancy entropy kernel and follows it CTB by CTB in the SM slots its draining wavefronts free (tail overlap), so band_pipeline_ms is what remains after the entropy kernel has ended (kernels_ms below: one launch per kernel for the whole grid, one after the other: B200_CHUNKS=0 B200_TAIL_OVERLAP=0)"},
         "gpu_launches": (stats_e2e.kernel_launches + (stats_e2e.bands if chunked else 1)) * args.steps,   # K0 (+ gate), (K1, K3 x2, K4 luma + chroma) per band as counted by the library, + K6 per band -- of the e2e leg
         "clocks": clk.summary(),
-        "roofline": {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                     "traffic": tr["bytes_per_launch"] if tr else None, "traffic_source": tr["source"] if tr else None,
-                     "peak_source": peak_src, "algorithmic_bytes_per_pixel": alg[dom],
+        "roofline": {"bound": "hbm", "kernel": dom, "achieved": ach, "peak": HBM_PEAK_GBS, "unit": "GB/s", "frac": ach / HBM_PEAK_GBS,
+                     "peak_source": "H100 SXM data sheet, 3.35 TB/s", "algorithmic_bytes_per_pixel": alg[dom],
                      "kernels_ms": kern, "kernels_gb_s": {k: alg[k] * my_px / (v * 1e-3) / 1e9 if v > 0 else None for k, v in kern.items()},
                      "entropy_gbins_per_s": bins / (kern["entropy"] * 1e-3) / 1e9 if kern.get("entropy") else None,
                      "pipeline_A_bytes_per_pixel": 12.0 + C,
@@ -409,7 +414,7 @@ def main():
     if world == 1 and not args.no_plugin_leg and args.front_end == "device":
         for key, extra in (("e2e_plugin", []), ("e2e_plugin_n2", ["--lib", "libheif_ref_b200.so"])):
             dump = f"/dev/shm/b200_bench_plug_{os.getpid()}.rgb"
-            res, why = reference_arm(side, side, 3, 2, side * side, dump=dump, log2_ctb=args.ctb, extra=["--decoder", "b200"] + extra)
+            res, why = reference_arm(side, side, args.steps, 2, side * side, dump=dump, log2_ctb=args.ctb, extra=["--decoder", "b200"] + extra)
             if res:
                 got = np.fromfile(dump, dtype=np.uint8)
                 os.unlink(dump)
@@ -423,12 +428,12 @@ def main():
             t64 = make_tiles(my_idx, workers=max(4, cores), log2_ctb=6)
             dec.decode_grid_to_rgb_host(t64, side, nrows, lb.CHROMA_INTERLEAVED_RGB, out=my_out)
             ts = []
-            for _ in range(3):
+            for _ in range(args.steps):
                 t0 = time.perf_counter(); dec.decode_grid_to_rgb_host(t64, side, nrows, lb.CHROMA_INTERLEAVED_RGB, out=my_out); ts.append(time.perf_counter() - t0)
             s64 = dec.stats()
             line["ctb64"] = {"e2e_mp_s": pixels / 1e6 / (sum(ts) / len(ts)), "e2e_ms_per_step": 1e3 * sum(ts) / len(ts), "entropy_ms": s64.entropy_ms, "recon_ms": s64.recon_ms,
                              "deblock_ms": s64.deblock_ms, "sao_paste_ms": s64.sao_ms, "bits_per_pixel": 8.0 * s64.bitstream_bytes / my_px,
-                             "note": "same pictures, same QP, coded with CTB 64 (x265 default); 3 e2e steps after 1 warm-up"}
+                             "note": f"same pictures, same QP, coded with CTB 64 (x265 default); {args.steps} e2e steps after 1 warm-up"}
         except Exception as e:  # noqa: BLE001
             line["ctb64"] = {"error": str(e)[:200]}
     print(json.dumps(line))

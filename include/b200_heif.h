@@ -1,5 +1,5 @@
 /*
- * b200_heif.h -- C ABI of libb200heif.so: the B200-native replacement for libheif's per-tile decode
+ * b200_heif.h -- C ABI of libb200heif.so: the H100-native replacement for libheif's per-tile decode
  * pixel pipeline (HEVC-intra decoder in the libde265 role + colour-conversion / rotate / mirror / crop /
  * overlay post-stage).  Plain pointers and sizes only; no C++ or torch types.
  *
@@ -195,7 +195,7 @@ void b200_free(void* p);
 
 /* ------------------------------------------------------------------------------------------------
  * HEVC intra decoder: header parsing on the host; CABAC + slice-data syntax, reconstruction, deblocking and SAO as
- * sm_100a kernels (CABAC can be moved to host threads with b200_decoder_set_front_end).
+ * sm_90a kernels (CABAC can be moved to host threads with b200_decoder_set_front_end).
  * Replaces: the libde265 calls of libheif/plugins/decoder_libde265.cc -- de265_new_decoder :181,
  *   de265_push_NAL :360, de265_decode :402, de265_get_next_picture :410, de265_get_image_plane :137,
  *   de265_get_image_{colour_primaries,transfer_characteristics,matrix_coefficients,full_range_flag} :428-446,

@@ -1,7 +1,7 @@
-"""libheif_b200 -- B200-native replacement of libheif's per-tile decode pixel pipeline.
+"""libheif_b200 -- H100-native replacement of libheif's per-tile decode pixel pipeline.
 
 Host-side mirror (Python) of the reference interfaces for this path; all pixel work happens in
-libb200heif.so (hand-written sm_100a CUDA behind the C ABI of include/b200_heif.h).
+libb200heif.so (hand-written sm_90a CUDA behind the C ABI of include/b200_heif.h).
 PyTorch is used only for device memory, streams and torch.distributed plumbing.
 """
 from ._lib import lib, B200Error, SO_PATH  # noqa: F401

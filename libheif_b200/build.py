@@ -1,4 +1,4 @@
-"""Build libb200heif.so in-tree with nvcc for sm_100a (called by __graft_entry__.build() and by `python -m libheif_b200.build`)."""
+"""Build libb200heif.so in-tree with nvcc for sm_90a (H100) (called by __graft_entry__.build() and by `python -m libheif_b200.build`)."""
 import glob
 import os
 import subprocess
@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200heif.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--fmad=false",
          "-Xcompiler", "-fPIC,-ffp-contract=off,-O2,-pthread", "-Xptxas", "-v"]
 
 

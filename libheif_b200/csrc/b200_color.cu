@@ -1,4 +1,4 @@
-// b200_color.cu -- K6: fused colour post-stage for sm_100a.
+// b200_color.cu -- K6: fused colour post-stage for sm_90a.
 //
 // One pass over HBM does what the reference does in 2-4 passes with calloc'ed intermediates
 // (libheif/color-conversion/colorconversion.cc:450-487 runs each op into a fresh image):

@@ -135,9 +135,8 @@ static int check_device_error(b200_decoder* d) {
 // K0 (entropy) and K1 (reconstruction) can run CONCURRENTLY: K1 consumes the command stream CTB by CTB as K0 publishes
 // it.  Both kernels are persistent and ticket-driven, so they need not be fully co-resident (whatever part of either
 // grid is resident finishes the work); the caps below only share the SM's registers between them.
-// Measured (profiles/README.md): the overlap hides K1 completely while the batch is critical-path bound -- up to about
-// one wave of sub-streams (32 tiles: 63 vs 85 ms, 64 tiles: 82 vs 94 ms) -- and LOSES once the GPU is throughput bound
-// (128 tiles: 109 vs 101 ms, 256 tiles: 195 vs 126 ms; the two instruction streams evict each other), so it is chosen
+// The overlap hides K1 completely while the batch is critical-path bound -- up to about one wave of sub-streams -- and
+// LOSES once the GPU is throughput bound (the two instruction streams evict each other), so it is chosen
 // per batch.  B200_OVERLAP=0/1 forces it.
 static int overlap_blocks(const char* env, int dflt) { if (const char* e = getenv(env)) { const int v = atoi(e); if (v >= 1 && v <= 4) return v; } return dflt; }
 // At most ONE overlapped K0/K1 pair is in flight per process: libheif drives many decoder instances from its own threads,
@@ -168,11 +167,9 @@ static bool use_overlap(size_t n_subs) {
 // is queued behind it on the other stream, so K1's CTAs become resident only where K0's persistent CTAs have left -- which
 // they do over the last ~30 % of K0's run time, once every sub-stream has been handed out and the wavefronts of the tiles
 // drain.  K1 (and, with bands, K3 / K4 / K6 / D2H of the first band) then runs in SM slots that would otherwise idle.
-// Measured on the bench grid (256 tiles, profiles/r02_tail_overlap_probe.json): resident step 76.1 -> 71.1 ms (K1 adds 1 - 2 ms
-// to K0 instead of 8.5), end to end 94.0 -> 89.5 ms with two row bands.
 // B200_TAIL_OVERLAP=0 switches it off; 1 (default): with row bands, one live K1 per band (the first band's K1 ends with K0, its
 // filters / K6 / D2H overlap the second band's K1); 2: ONE live K1 over the whole grid, bands only for K3 / K4 / K6 / D2H
-// (measured 3 ms slower end to end: nothing is left to overlap the first band's D2H).
+// (slower end to end: nothing is left to overlap the first band's D2H).
 static int use_tail_overlap() {
   if (const char* e = getenv("B200_TAIL_OVERLAP")) return atoi(e);
   return 1;
@@ -398,7 +395,7 @@ int b200_decoder_decode_grid(b200_decoder* d, int cols, int rows, const uint8_t*
     const char* ce = getenv("B200_CHUNKS");
     if (rows >= 2 && (ce ? atoi(ce) != 0 : (d->chunk_hook && (!devfe || !use_overlap(n_subs))))) {      // B200_CHUNKS=0 / 1: never / always (tests, diagnostics)
       // two bands by default: every K1 launch costs one tile's wavefront latency (~5 ms for 1024x1024), so more bands lose
-      // more than their finer D2H overlap gains (measured: 2 / 4 / 8 / 16 bands, profiles/README.md)
+      // more than their finer D2H overlap gains
       int target = (n + 1) / 2; if (const char* e = getenv("B200_CHUNK_TILES")) { const int v = atoi(e); if (v > 0) target = v; }
       rpc = std::max(1, (target + cols / 2) / cols);
       nch = (rows + rpc - 1) / rpc;

@@ -269,7 +269,7 @@ __global__ void __launch_bounds__(256) sao_kernel(const DeviceBatch b) {
 // its group .. the row below) are requested up front with 8- / 16-byte loads -- six independent loads in flight per thread
 // instead of a dependent chain of three -- and the horizontal neighbours come from the adjacent lanes by shuffle (one warp =
 // 256 consecutive samples of a row; only lanes 0 and 31 load their outer neighbour).  The CTB's parameters, the
-// bypass / PCM cell and the picture descriptor are fetched once per 32 samples.  Measured on the bench grid: see profiles/README.md.
+// bypass / PCM cell and the picture descriptor are fetched once per 32 samples.
 // (The first form above walks one row per thread: its 393 K blocks of 2 KB were bound by block turnover and load latency; walking
 // four rows one after the other in a rolled loop was slower still.)
 template <typename T> struct SaoPack;

@@ -1,4 +1,4 @@
-// b200_hevc_recon.cu -- K1 + K2: scaling, inverse DCT/DST, intra prediction and reconstruction on sm_100a.
+// b200_hevc_recon.cu -- K1 + K2: scaling, inverse DCT/DST, intra prediction and reconstruction on sm_90a.
 //
 // Does the per-sample half of what libde265 does inside de265_decode() (reached from
 // libheif/plugins/decoder_libde265.cc:386-457): H.265 8.6.2-8.6.4 (scaling, transforms), 8.4.4.2 (intra sample

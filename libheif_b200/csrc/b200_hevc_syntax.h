@@ -195,7 +195,7 @@ struct Cabac {
   }
 #ifdef B200_SYN_DEVICE
   // out of line ON PURPOSE: a call inside the refill keeps ptxas from if-converting (predicating) its ~10 instructions into
-  // every bin -- they are needed once per 16 consumed bits (measured: 12 % of K0's issue slots, profiles/README.md)
+  // every bin -- they are needed once per 16 consumed bits
   static __device__ __noinline__ uint32_t fetch16_cold(const uint8_t* d, uint32_t q) { return __byte_perm((uint32_t)__ldg(reinterpret_cast<const unsigned short*>(d + q)), 0, 0x4401); }
 #else
   static inline uint32_t fetch16_cold(const uint8_t* d, uint32_t q) { return ((uint32_t)d[q] << 8) | d[q + 1]; }
@@ -296,7 +296,7 @@ struct SaoRaw { int8_t type[3], band[3], eo[3]; int8_t off[3][4]; };
 // front-end instantiates the decoder twice: CfgRuntime (anything the parser accepts) and CfgCommon, the parameter
 // combination of x265-produced HEIC files (and of libheif/examples/example.heic: 4:2:0 8 bit, min CB 8, TB 4..32, no
 // transform skip, cu_qp_delta + sign data hiding + SAO on, WPP); the kernel's speed is set by its instruction-cache
-// footprint (profiles/README.md), and the constants remove ~5 KB of it.  The host front-end uses CfgRuntime.
+// footprint, and the constants remove ~5 KB of it.  The host front-end uses CfgRuntime.
 struct CfgRuntime { enum : int { chroma = -1, bd = -1, log2_min_cb = -1, log2_min_tb = -1, log2_max_tb = -1, transform_skip = -1, cu_qp_delta = -1, sign_hiding = -1, sao_enabled = -1, wpp = -1, dense = -1, pcm = -1, tq_bypass = -1, tiles = -1 }; };
 struct CfgCommon { enum : int { chroma = 1, bd = 8, log2_min_cb = 3, log2_min_tb = 2, log2_max_tb = 5, transform_skip = 0, cu_qp_delta = 1, sign_hiding = 1, sao_enabled = 1, wpp = 1, dense = 0, pcm = 0, tq_bypass = 0, tiles = 0 }; };
 B200_HD inline bool matches_common(const SeqParams& q) {

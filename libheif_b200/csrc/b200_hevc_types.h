@@ -1,5 +1,5 @@
 // b200_hevc_types.h -- command stream between the entropy stage (K0 on the GPU, b200_hevc_entropy.cu; or the same
-// syntax decoder on the host, b200_hevc_parse.cc) and the sm_100a reconstruction kernels (b200_hevc_recon.cu,
+// syntax decoder on the host, b200_hevc_parse.cc) and the sm_90a reconstruction kernels (b200_hevc_recon.cu,
 // b200_hevc_filters.cu).  Plain PODs, identical on host and device.
 //
 // Division of labour: NAL / parameter-set / slice-header parsing runs on the host (microseconds per tile); everything

@@ -121,7 +121,7 @@ void release_decoder(b200_decoder* d) { std::lock_guard<std::mutex> l(g_pool_mu)
 struct Pending { std::vector<uint8_t> au; uintptr_t user; };
 struct DecInstance { std::deque<Pending> q; std::vector<uint8_t> param_sets; std::vector<uint8_t> data; int strict = 0; const b200h_security_limits* limits = nullptr; };
 
-const char* dec_name() { return "b200 HEVC intra decoder (sm_100a CUDA kernels)"; }
+const char* dec_name() { return "b200 HEVC intra decoder (sm_90a CUDA kernels)"; }
 void dec_init() {}
 void dec_deinit();
 int dec_supports(int format) { return format == B200H_COMPRESSION_HEVC ? 200 : 0; }          // libde265 reports 100, ffmpeg 90

@@ -1,4 +1,4 @@
-"""HEVC intra decoder (host front-end + sm_100a kernels) -- Python mirror of the decoder-plugin call sequence.
+"""HEVC intra decoder (host front-end + sm_90a kernels) -- Python mirror of the decoder-plugin call sequence.
 
 Reference interfaces mirrored:
   heif_decoder_plugin::new_decoder2 / push_data2 / decode_next_image2 / free_decoder   libheif/api/libheif/heif_plugin.h:85-169

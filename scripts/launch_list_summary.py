@@ -1,5 +1,5 @@
 """Per-kernel launch count / mean duration / share of an `ncu --metrics gpu__time_duration.sum --csv` log:
-python scripts/launch_list_summary.py <launches.csv> > profiles/<name>.txt"""
+python scripts/launch_list_summary.py <launches.csv> > <name>.txt"""
 import collections, csv, sys
 rows = [r for r in csv.reader(l for l in open(sys.argv[1]) if l.startswith('"'))]
 hdr = rows[0]; ik, iv, iu = hdr.index("Kernel Name"), hdr.index("Metric Value"), hdr.index("Metric Unit")

@@ -1,4 +1,4 @@
-"""Key numbers of one kernel from an .ncu-rep (ncu --set full): python scripts/ncu_summary.py <rep> > profiles/<name>.txt"""
+"""Key numbers of one kernel from an .ncu-rep (ncu --set full): python scripts/ncu_summary.py <rep> > <name>.txt"""
 import csv, subprocess, sys, io
 rep = sys.argv[1]
 raw = subprocess.run(['ncu', '-i', rep, '--page', 'raw', '--csv'], capture_output=True, text=True).stdout

@@ -1,4 +1,4 @@
-"""Batch-throughput probe (one B200): K pictures (the bench grid, 16 x 16 tiles of 1024x1024) through the asynchronous fused
+"""Batch-throughput probe (one GPU): K pictures (the bench grid, 16 x 16 tiles of 1024x1024) through the asynchronous fused
 entry point, with ONE decoder object (D2H of picture i overlaps the kernels of picture i + 1) and with TWO decoder objects
 taking the pictures alternately (own streams and device buffers each: K0 of picture i + 1 can take the SM slots the draining
 K0 of picture i leaves).  Every step parses, uploads, decodes and delivers its RGB into page-locked host memory."""

@@ -5,11 +5,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import libheif_b200 as lb
 
-peak = 6480.5
-try:
-    peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"]
-except Exception:
-    pass
+peak = 3350.0      # H100 SXM data sheet HBM3 bandwidth
 res = {"peak_gbs": peak}
 w, h = 16384, 8192
 for bpp in (3, 4):

@@ -1,4 +1,4 @@
-"""K0-tail overlap probe (one B200): the bench workload (16 x 16 tiles of 1024x1024) under combinations of
+"""K0-tail overlap probe (one GPU): the bench workload (16 x 16 tiles of 1024x1024) under combinations of
 B200_TAIL_OVERLAP (K1 queued behind a full-occupancy K0, filling the SM slots K0's draining wavefronts leave) and
 B200_CHUNK_TILES (band count of the synchronous fused call).  Prints one JSON object: per configuration the resident step
 (CUDA events), the end-to-end step (one C-ABI call, host bitstreams -> page-locked host RGB), the kernel stats of the last

@@ -1,48 +1,55 @@
-// Compile-time cross-check of include/b200_heif_plugin_abi.h against the reference's own headers
-// (libheif/api/libheif/heif_plugin.h, heif_error.h, heif_library.h).  Built and run by tests/test_plugin_abi.py
-// only where /root/reference exists.
+// Layout of include/b200_heif_plugin_abi.h next to the reference's own headers (libheif/api/libheif/heif_plugin.h,
+// heif_error.h, heif_library.h).  Prints one line per size, offset and constant the mirror depends on, always under the
+// reference's name:
+//   g++ -std=c++17 tests/abi/abi_check.cc                      -> what the mirror has (tests/test_plugin.py)
+//   g++ -std=c++17 -DREFERENCE -I<libheif>/libheif/api -I<dir of heif_version.h> tests/abi/abi_check.cc
+//                                                               -> what libheif has (tests/golden/abi/reference_layout.txt)
+#include <cstddef>
+#include <cstdint>
+#include <cstdio>
+#ifdef REFERENCE
 #include <libheif/heif.h>
 #include <libheif/heif_plugin.h>
-#include <cstddef>
+#define T(mirror, ref) ref
+#else
 #include "../../include/b200_heif_plugin_abi.h"
+#define T(mirror, ref) mirror
+#endif
 
-#define SAME_OFF(A, B, m) static_assert(offsetof(A, m) == offsetof(B, m), "offset of " #m)
-static_assert(sizeof(b200h_error) == sizeof(heif_error), "heif_error");
-static_assert(offsetof(b200h_error, message) == offsetof(heif_error, message), "heif_error.message");
-static_assert(sizeof(b200h_decoder_plugin) == sizeof(heif_decoder_plugin), "decoder plugin size");
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, plugin_api_version); SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, get_plugin_name);
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, does_support_format); SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, new_decoder);
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, push_data); SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, decode_image);
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, set_strict_decoding); SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, id_name);
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, decode_next_image); SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, minimum_required_libheif_version);
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, does_support_format2); SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, new_decoder2);
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, push_data2); SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, flush_data);
-SAME_OFF(b200h_decoder_plugin, heif_decoder_plugin, decode_next_image2);
-static_assert(sizeof(b200h_encoder_plugin) == sizeof(heif_encoder_plugin), "encoder plugin size");
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, compression_format); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, id_name);
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, priority); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, supports_lossless_compression);
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, new_encoder); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, list_parameters);
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, get_parameter_string); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, query_input_colorspace);
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, encode_image); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, get_compressed_data);
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, query_input_colorspace2); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, query_encoded_size);
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, minimum_required_libheif_version); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, start_sequence_encoding);
-SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, get_compressed_data2); SAME_OFF(b200h_encoder_plugin, heif_encoder_plugin, does_indicate_keyframes);
-static_assert(sizeof(b200h_encoder_parameter) == sizeof(heif_encoder_parameter), "encoder parameter size");
-static_assert(offsetof(b200h_encoder_parameter, has_default) == offsetof(heif_encoder_parameter, has_default), "has_default");
-static_assert(sizeof(b200h_decoder_options) == sizeof(heif_decoder_plugin_options), "decoder options");
-static_assert(offsetof(b200h_decoder_options, limits) == offsetof(heif_decoder_plugin_options, limits), "options.limits");
-static_assert(offsetof(b200h_security_limits, max_image_size_pixels) == offsetof(heif_security_limits, max_image_size_pixels), "limits");
-static_assert(sizeof(b200h_plugin_info) == sizeof(heif_plugin_info), "plugin_info");
-static_assert(B200H_ERR_DECODER_PLUGIN == heif_error_Decoder_plugin_error && B200H_ERR_ENCODER_PLUGIN == heif_error_Encoder_plugin_error &&
-              B200H_ERR_UNSUPPORTED_FEATURE == heif_error_Unsupported_feature && B200H_ERR_MEMORY == heif_error_Memory_allocation_error &&
-              B200H_ERR_USAGE == heif_error_Usage_error, "error codes");
-static_assert(B200H_SUBERR_SECURITY_LIMIT == heif_suberror_Security_limit_exceeded && B200H_SUBERR_UNSUPPORTED_CODEC == heif_suberror_Unsupported_codec &&
-              B200H_SUBERR_END_OF_DATA == heif_suberror_End_of_data && B200H_SUBERR_UNSUPPORTED_BIT_DEPTH == heif_suberror_Unsupported_bit_depth, "suberrors");
-static_assert(B200H_COMPRESSION_HEVC == heif_compression_HEVC && B200H_COLORSPACE_YCBCR == heif_colorspace_YCbCr && B200H_COLORSPACE_MONOCHROME == heif_colorspace_monochrome &&
-              B200H_CHANNEL_Y == heif_channel_Y && B200H_CHANNEL_CB == heif_channel_Cb && B200H_CHANNEL_CR == heif_channel_Cr && heif_chroma_420 == 1 &&
-              heif_plugin_type_decoder == 1 && heif_plugin_type_encoder == 0, "enums");
-static_assert(LIBHEIF_MAKE_VERSION(1, 21, 0) == ((1u << 24) | (21u << 16)), "version macro");
 struct NclxPublic { uint8_t version; int color_primaries; int transfer_characteristics; int matrix_coefficients; uint8_t full_range_flag; };
-static_assert(offsetof(NclxPublic, full_range_flag) == offsetof(heif_color_profile_nclx, full_range_flag), "nclx.full_range_flag");
-static_assert(offsetof(NclxPublic, matrix_coefficients) == offsetof(heif_color_profile_nclx, matrix_coefficients), "nclx.matrix");
-int main() { return 0; }
+
+#define SIZE(m, r) printf("sizeof %s %zu\n", #r, sizeof(T(m, r)));
+#define OFF(m, r, f) printf("offsetof %s.%s %zu\n", #r, #f, offsetof(T(m, r), f));
+#define VAL(m, r) printf("value %s %lld\n", #r, (long long)(T(m, r)));
+
+#define D(f) OFF(b200h_decoder_plugin, heif_decoder_plugin, f)
+#define E(f) OFF(b200h_encoder_plugin, heif_encoder_plugin, f)
+
+int main() {
+  SIZE(b200h_error, heif_error) OFF(b200h_error, heif_error, message)
+  SIZE(b200h_decoder_plugin, heif_decoder_plugin)
+  D(plugin_api_version) D(get_plugin_name) D(does_support_format) D(new_decoder) D(push_data) D(decode_image)
+  D(set_strict_decoding) D(id_name) D(decode_next_image) D(minimum_required_libheif_version) D(does_support_format2)
+  D(new_decoder2) D(push_data2) D(flush_data) D(decode_next_image2)
+  SIZE(b200h_encoder_plugin, heif_encoder_plugin)
+  E(compression_format) E(id_name) E(priority) E(supports_lossless_compression) E(new_encoder) E(list_parameters)
+  E(get_parameter_string) E(query_input_colorspace) E(encode_image) E(get_compressed_data) E(query_input_colorspace2)
+  E(query_encoded_size) E(minimum_required_libheif_version) E(start_sequence_encoding) E(get_compressed_data2)
+  E(does_indicate_keyframes)
+  SIZE(b200h_encoder_parameter, heif_encoder_parameter) OFF(b200h_encoder_parameter, heif_encoder_parameter, has_default)
+  SIZE(b200h_decoder_options, heif_decoder_plugin_options) OFF(b200h_decoder_options, heif_decoder_plugin_options, limits)
+  OFF(b200h_security_limits, heif_security_limits, max_image_size_pixels)
+  SIZE(b200h_plugin_info, heif_plugin_info)
+  VAL(B200H_ERR_DECODER_PLUGIN, heif_error_Decoder_plugin_error) VAL(B200H_ERR_ENCODER_PLUGIN, heif_error_Encoder_plugin_error)
+  VAL(B200H_ERR_UNSUPPORTED_FEATURE, heif_error_Unsupported_feature) VAL(B200H_ERR_MEMORY, heif_error_Memory_allocation_error)
+  VAL(B200H_ERR_USAGE, heif_error_Usage_error)
+  VAL(B200H_SUBERR_SECURITY_LIMIT, heif_suberror_Security_limit_exceeded) VAL(B200H_SUBERR_UNSUPPORTED_CODEC, heif_suberror_Unsupported_codec)
+  VAL(B200H_SUBERR_END_OF_DATA, heif_suberror_End_of_data) VAL(B200H_SUBERR_UNSUPPORTED_BIT_DEPTH, heif_suberror_Unsupported_bit_depth)
+  VAL(B200H_COMPRESSION_HEVC, heif_compression_HEVC) VAL(B200H_COLORSPACE_YCBCR, heif_colorspace_YCbCr)
+  VAL(B200H_COLORSPACE_MONOCHROME, heif_colorspace_monochrome)
+  VAL(B200H_CHANNEL_Y, heif_channel_Y) VAL(B200H_CHANNEL_CB, heif_channel_Cb) VAL(B200H_CHANNEL_CR, heif_channel_Cr)
+  VAL(1, heif_chroma_420) VAL(1, heif_plugin_type_decoder) VAL(0, heif_plugin_type_encoder)   // what b200_plugin.cc passes
+  VAL(((1u << 24) | (21u << 16)), LIBHEIF_MAKE_VERSION(1, 21, 0))
+  OFF(NclxPublic, heif_color_profile_nclx, full_range_flag) OFF(NclxPublic, heif_color_profile_nclx, matrix_coefficients)
+  return 0;
+}

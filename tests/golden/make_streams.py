@@ -1,5 +1,5 @@
-"""Regenerates tests/golden/streams/*.au from the reference's own fixture files (run in the build container, where
-/root/reference and oracle/_ref exist):
+"""Regenerates tests/golden/streams/*.au from the reference's own fixture files (needs the reference source tree and the
+oracle/_ref build):
 
     python tests/golden/make_streams.py [--check]
 
@@ -7,8 +7,9 @@ Each .au is byte-for-byte what the UNMODIFIED reference libheif pushes into a de
 (Decoder::get_compressed_data, libheif/codecs/decoder.cc:275-308: hvcC parameter-set NALs followed by the item's NALs,
 each with a 4-byte big-endian length).  They are captured by the CPU oracle plugin (oracle/ref_plugin.cc,
 B200_ORACLE_DUMP_DIR) while heif_decode_image decodes the file -- run in a child process per file, because the reference
-library must be loaded RTLD_GLOBAL (see oracle/refheif.py).  With --check nothing is written; the script fails if a
-regenerated stream differs from the committed one.
+library must be loaded RTLD_GLOBAL (see oracle/refheif.py).  With --check nothing is written and only the fixture files
+stored under tests/golden/fixtures/ are decoded (all but examples/example.heic); the script fails if a regenerated stream
+differs from the committed one.
 """
 import hashlib
 import os
@@ -19,6 +20,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 REF = "/root/reference"
 OUT = os.path.join(ROOT, "tests", "golden", "streams")
+STORED = os.path.join(ROOT, "tests", "golden", "fixtures")
 
 # (reference fixture, [names of the access units in the order the reference pushes them])
 FIXTURES = [
@@ -49,7 +51,13 @@ def main():
     check = "--check" in sys.argv
     bad = 0
     for rel, names in FIXTURES:
-        dumps = capture(os.path.join(REF, rel))
+        if check:
+            path = os.path.join(STORED, os.path.basename(rel))
+            if not os.path.exists(path):
+                continue
+        else:
+            path = os.path.join(REF, rel)
+        dumps = capture(path)
         # one dump per decoder instance / pushed item, in decoding order; the primary item's stream may be pushed once per
         # decode pass, so keep the first occurrence of every distinct stream
         seen, uniq = set(), []

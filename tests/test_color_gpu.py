@@ -1,4 +1,4 @@
-"""GPU parity: the fused sm_100a colour kernel (K6) through the C ABI vs the C restatement of the reference
+"""GPU parity: the fused sm_90a colour kernel (K6) through the C ABI vs the C restatement of the reference
 (oracle/color_oracle.c, itself pinned on the unmodified reference by test_color_oracle.py). Bit-exact."""
 import hashlib
 

@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a HEVC intra decoder (host front-end + reconstruction / deblocking / SAO kernels, through the
+"""GPU parity: the sm_90a HEVC intra decoder (host front-end + reconstruction / deblocking / SAO kernels, through the
 C ABI) vs the C restatement (oracle/hevc_oracle.c, pinned on FFmpeg) -- bit-exact on every plane, every stream,
 including the intermediate stages (before deblocking, after deblocking) to localise mismatches."""
 import hashlib
