@@ -119,7 +119,7 @@ const b200h_decoder_plugin* b200_get_decoder_plugin(void);
 const b200h_encoder_plugin* b200_get_encoder_plugin(void);
 int b200_plugin_bind_libheif(void* dl_handle);
 /* Submission queue of the decoder plugin (concurrent decode_next_image2 calls are decoded as one batch, see b200_plugin.cc):
-   out3 = {batches decoded, pictures decoded, largest batch}.  Environment: B200_PLUGIN_BATCH=0 decodes every call on its own. */
+   out3 = {batches decoded, pictures decoded, largest batch}. */
 void b200_plugin_queue_stats(uint64_t out3[3]);
 
 #ifdef __cplusplus

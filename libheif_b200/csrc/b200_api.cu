@@ -158,6 +158,7 @@ struct HostXfer {
 };
 HostXfer g_xfer;
 constexpr size_t kBounceSlot = (size_t)32 << 20;
+constexpr unsigned kMaxCopyThreads = 16;           // host threads that fill / drain the bounce buffer: the online cores, at most this
 
 bool host_page_locked(const void* p) {
   cudaPointerAttributes a;
@@ -165,7 +166,7 @@ bool host_page_locked(const void* p) {
   return a.type == cudaMemoryTypeHost;
 }
 int xfer_threads() {
-  static const int n = [] { unsigned h = std::thread::hardware_concurrency(); if (const char* e = getenv("B200_COPY_THREADS")) { const int v = atoi(e); if (v >= 1 && v <= 64) return v; } return (int)(h < 1 ? 1 : (h > 16 ? 16 : h)); }();
+  static const int n = [] { unsigned h = std::thread::hardware_concurrency(); return (int)(h < 1 ? 1 : (h > kMaxCopyThreads ? kMaxCopyThreads : h)); }();
   return n;
 }
 template <class F>
@@ -230,7 +231,6 @@ cudaError_t download_plane(HostXfer& X, void* dst, size_t dstride, const char* s
 int b200_color_convert_host(const b200_planes* in, const b200_geometry* geom, const b200_color_options* opt, void* out,
                             void* out_g, void* out_b, size_t out_stride, int* pipeline) {
   if (!in || !geom || !opt || !out) return set_error(B200_E_INVALID, "null argument");
-  if (getenv("B200_COLOR_HOST_SIMPLE")) return color_convert_host_simple(in, geom, opt, out, out_g, out_b, out_stride, pipeline);
   const int bps = in->bit_depth > 8 ? 2 : 1;
   const int sh = (in->chroma == B200_CHROMA_420 || in->chroma == B200_CHROMA_422) ? 1 : 0;
   const int sv = in->chroma == B200_CHROMA_420 ? 1 : 0;

@@ -11,6 +11,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -50,8 +51,12 @@ class Pool {
 };
 
 template <typename T>
-struct DevBuf {   // grow-only device buffer with optional pinned host staging of the same capacity
+struct DevBuf {   // grow-only device buffer with optional pinned host staging of the same capacity; owns both (move-only)
   T* d = nullptr; T* h = nullptr; size_t cap = 0, hcap = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : d(o.d), h(o.h), cap(o.cap), hcap(o.hcap) { o.d = o.h = nullptr; o.cap = o.hcap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(d, o.d); std::swap(h, o.h); std::swap(cap, o.cap); std::swap(hcap, o.hcap); return *this; }
+  ~DevBuf() { if (d) cudaFree(d); if (h) cudaFreeHost(h); }
   int reserve(size_t n, bool host = true) {
     if (n > cap) {
       const size_t nc = n + n / 4 + 1024;
@@ -68,77 +73,171 @@ struct DevBuf {   // grow-only device buffer with optional pinned host staging o
     }
     return B200_OK;
   }
-  void release() { if (d) cudaFree(d); if (h) cudaFreeHost(h); d = nullptr; h = nullptr; cap = hcap = 0; }
 };
+
+// owning handle of a stream, an event or a page-locked block
+template <typename H, cudaError_t (*Destroy)(H)>
+struct Owned {
+  H h = nullptr;
+  Owned() = default;
+  Owned(const Owned&) = delete;
+  Owned& operator=(const Owned&) = delete;
+  ~Owned() { if (h) Destroy(h); }
+  operator H() const { return h; }
+};
+cudaError_t free_pinned(unsigned* p) { return cudaFreeHost(p); }
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using PinnedFlags = Owned<unsigned*, free_pinned>;
+
+// The counters and queues the kernels share, one batch-wide array each.  Their offsets follow from the batch's CTB rows and
+// sub-streams alone; sizing, clearing and the kernels' batch descriptors all go through this one layout.
+struct ScratchLayout {
+  size_t n_rows = 0, n_subs = 0;
+  // sync (K1 .. K4): [0] unused, [1] error flag, three progress counters per CTB row, then one work ticket per band
+  static constexpr size_t error_flag = 1, progress = 2;
+  size_t tickets() const { return progress + 3 * n_rows; }
+  size_t sync_size() const { return tickets() + MAX_CHUNKS; }
+  // esync (K0): [0] unused, one progress counter per CTB row, then one entry per sub-stream (EntropyBatch::sub_done)
+  static constexpr size_t entropy_progress = 1;
+  size_t sub_done() const { return entropy_progress + n_rows; }
+  size_t esync_size() const { return sub_done() + n_subs; }
+  // equeue (K0's ready queue): [0] pop cursor, [1] push cursor, one queue slot per sub-stream, then its dependency count
+  static constexpr size_t qhead = 0, qtail = 1, queue = 2;
+  size_t deps() const { return queue + n_subs; }
+  size_t equeue_size() const { return deps() + n_subs; }
+};
+
+// Overrides of the launch schedule from the environment (tests, bench.py, diagnostics).  Read at the start of every
+// decode_grid and rerun_device call, since callers change them between calls.
+struct Overrides {
+  enum Force { AUTO, OFF, ON };
+  Force bands = AUTO;          // B200_CHUNKS=0 / 1: never / always run the tile rows in bands
+  int band_tiles = 0;          // B200_CHUNK_TILES=n: tiles per band (default: half the grid)
+  Force overlap = AUTO;        // B200_OVERLAP=0 / 1: K0 and K1 back to back / concurrently
+  bool tail = true;            // B200_TAIL_OVERLAP=0: no tail overlap
+  bool tail_force = false;     // B200_TAIL_FORCE: tail overlap for batches of at most one K0 wave too
+  static Overrides read() {
+    auto force = [](const char* name) { const char* e = getenv(name); return !e ? AUTO : (atoi(e) != 0 ? ON : OFF); };
+    Overrides o;
+    o.bands = force("B200_CHUNKS"); o.overlap = force("B200_OVERLAP");
+    if (const char* e = getenv("B200_CHUNK_TILES")) o.band_tiles = std::max(0, atoi(e));
+    if (const char* e = getenv("B200_TAIL_OVERLAP")) o.tail = atoi(e) != 0;
+    o.tail_force = getenv("B200_TAIL_FORCE") != nullptr;
+    return o;
+  }
+};
+
+struct BatchShape {            // what the launch schedule depends on in a batch
+  int cols = 1, rows = 1;      // grid of pictures
+  bool device_front_end = false;
+  size_t n_subs = 0;           // CABAC sub-streams (device front-end)
+  bool any_tiles = false;      // a picture uses HEVC tiles
+  bool all_common = false;     // every picture has the syn::CfgCommon parameter combination
+  int bands = 0;               // row bands the row list is laid out in (0: not laid out yet)
+};
+
+enum { OVERLAP_K0_BLOCKS_PER_SM = 3, OVERLAP_K1_BLOCKS_PER_SM = 2 };   // resident CTAs per SM while K0 and K1 share the SMs
+
+struct LaunchPlan {
+  int bands = 1, rows_per_band = 1;   // row bands of whole tile rows (rows_per_band: when the plan lays them out)
+  bool banded = false;                // K1 -> K3 -> K4 (-> the caller's band hook) run band by band
+  bool overlap = false;               // K0 on the side stream, K1 following it CTB by CTB (if the process-wide slot is free)
+  bool tail = false;                  // ... with K0 at full occupancy and K1 queued behind it
+  int k0_blocks_per_sm = 0, k1_blocks_per_sm = 0;   // CTA caps of an overlapped run (0: none)
+  bool common_k0 = false;             // the entropy kernel specialised for syn::CfgCommon
+};
+
+int sm_count() { int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); return sms; }
+
+// The launch schedule of one run, from the batch, whether the caller takes the result band by band (`hook`), and the
+// overrides.
+// Bands: only a caller that takes the bands one by one (the synchronous fused entry point: the D2H of band c overlaps the
+// kernels of band c + 1) gets them, and only when the batch is larger than what K0 and K1 overlap CTB by CTB.  Two bands by
+// default: every K1 launch costs one tile's wavefront latency (~5 ms for 1024x1024), so more bands lose more than their
+// finer D2H overlap gains.  Everything else -- the composition API, rerun_device, the asynchronous entry point whose D2H
+// already overlaps the next picture -- runs one launch per kernel (the band-major row list is a valid ticket order for that).
+// Overlap: K0 and K1 are persistent and ticket-driven, so they need not be fully co-resident (whatever part of either grid
+// is resident finishes the work); the CTA caps only share the SM's registers between them.  Running them concurrently hides
+// K1 completely while the batch is critical-path bound -- up to about one wave of sub-streams -- and LOSES once the GPU is
+// throughput bound (the two instruction streams evict each other).
+// Tail overlap, for batches of more than one wave: K0 keeps the whole GPU (4 CTAs per SM, launched first) and the live K1 is
+// queued behind it on the other stream, so K1's CTAs become resident only where K0's persistent CTAs have left -- which they
+// do over the last ~30 % of K0's run time, once every sub-stream has been handed out and the wavefronts of the tiles drain.
+// K1 (and, with bands, K3 / K4 / K6 / D2H of the first band; one K1 per band) then runs in SM slots that would otherwise idle.
+// K1 follows K0 through per-row progress counters in raster order; sub-streams of HEVC tiles produce CTBs tile by tile, so
+// a batch with tiles never overlaps.
+LaunchPlan plan_launches(const BatchShape& b, bool hook, const Overrides& env) {
+  LaunchPlan p;
+  const bool devfe = b.device_front_end;
+  const bool one_wave = devfe && (env.overlap == Overrides::AUTO ? b.n_subs <= (size_t)sm_count() * 16       // 4 CTAs x 4 warps of K0 per SM
+                                                                  : env.overlap == Overrides::ON);
+  p.bands = b.bands;
+  if (!p.bands) {
+    p.bands = 1; p.rows_per_band = b.rows;
+    if (b.rows >= 2 && (env.bands != Overrides::AUTO ? env.bands == Overrides::ON : hook && !one_wave)) {
+      const int target = env.band_tiles > 0 ? env.band_tiles : (b.cols * b.rows + 1) / 2;
+      int rpb = std::max(1, (target + b.cols / 2) / b.cols);
+      if ((b.rows + rpb - 1) / rpb > MAX_CHUNKS) rpb = (b.rows + MAX_CHUNKS - 1) / MAX_CHUNKS;
+      p.rows_per_band = rpb; p.bands = (b.rows + rpb - 1) / rpb;
+    }
+  }
+  p.banded = p.bands > 1 && (hook || env.bands == Overrides::ON);
+  p.overlap = !p.banded && one_wave;
+  p.tail = devfe && env.overlap == Overrides::AUTO && env.tail && (!p.overlap || env.tail_force);
+  if (p.tail) p.overlap = true;
+  if (b.any_tiles) p.overlap = p.tail = false;
+  if (p.overlap && !p.tail) { p.k0_blocks_per_sm = OVERLAP_K0_BLOCKS_PER_SM; p.k1_blocks_per_sm = OVERLAP_K1_BLOCKS_PER_SM; }
+  p.common_k0 = b.all_common;
+  return p;
+}
 
 }  // namespace
 
 struct b200_decoder {
-  Pool* pool = nullptr;
+  std::unique_ptr<Pool> pool;
   std::vector<ParsedPicture> parsed;
   std::vector<int> parse_rc; std::vector<std::string> parse_msg;
   DevBuf<PicDesc> pics; DevBuf<CtuInfo> ctus; DevBuf<TuCmd> tus; DevBuf<CoefEntry> coefs; DevBuf<SliceInfo> slices;
-  DevBuf<int8_t> qp8; DevBuf<uint8_t> edge8; DevBuf<uint8_t> scaling; DevBuf<uint2> rows; DevBuf<unsigned> sync;   // sync: [0] ticket, [1] error flag, [2..] progress
+  DevBuf<int8_t> qp8; DevBuf<uint8_t> edge8; DevBuf<uint8_t> scaling; DevBuf<uint2> rows; DevBuf<unsigned> sync;   // sync: ScratchLayout
   DevBuf<uint8_t> rec; DevBuf<uint8_t> canvas; DevBuf<uint8_t> rgb2[2]; DevBuf<uint8_t> bounce;   // fused host entry points: two RGB buffers (D2H of one overlaps the kernels writing the other)
-  cudaStream_t own = nullptr, copy = nullptr; cudaEvent_t ev_band[2] = {nullptr, nullptr}, ev_k6[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
-  unsigned* err_host = nullptr; int async_slot = 0; bool async_error = false;
   // device front-end (entropy decoding on the GPU)
   DevBuf<uint8_t> rbsp; DevBuf<syn::Substream> subs; DevBuf<unsigned> equeue; DevBuf<uint16_t> ctu_slice; DevBuf<EntropyPic> epics;
   DevBuf<uint8_t> ipm4, cd8, wpp_ctx, end_state; DevBuf<unsigned> esync; DevBuf<unsigned long long> ecount;
+  // streams and events, all created by b200_decoder_create
+  Stream own, copy;                // fused host entry points: the decode stream and the D2H stream
+  Stream side;                     // K0 runs here, concurrently with K1 on the decode stream
+  Event ev_fork, ev_join;          // decode stream -> side before K0, side -> decode stream after it
+  Event t_start, t_h2d, t_entropy, t_recon, t_deblock, t_sao;   // stage ends on the decode stream (b200_decoder_get_stats)
+  Event ev_k6[2], ev_d2h[2];       // per RGB buffer: colour conversion done, D2H done
+  Event ev_bounce[2];              // pageable destination: the bounce buffer halves
+  Event ev_band[MAX_CHUNKS];       // band pipeline: RGB of the band done
+  PinnedFlags err_host;            // per RGB buffer: the error flag of the step that used it last
+  int async_slot = 0; bool async_error = false;
   int front_end = 1;               // 1 = CABAC on the GPU (default), 0 = CABAC on the host cores
-  bool used_device_front_end = false; size_t n_subs = 0;
+  int debug_stage = 0;
+  // the batch decode_grid laid out last
+  BatchShape shape;
+  ScratchLayout scratch;
+  int npics = 0; size_t n_items = 0; int max_log2_ctb = 6, info_bps = 1;
+  int band_pic[MAX_CHUNKS + 1] = {0}; size_t band_item[MAX_CHUNKS + 1] = {0};   // first picture / row-list item of each band
   size_t canvas_off[3] = {0, 0, 0}; size_t canvas_pitch[3] = {0, 0, 0};
   b200_image_info info{};
   b200_decode_stats stats{};
-  std::vector<size_t> rec_off; int npics = 0;
-  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 0 start, 1 after H2D, 5 after entropy, 2 after recon, 3 after deblock, 4 after SAO
+  bool have_result = false, last_overlapped = false, last_banded = false;
   cudaStream_t last_stream = nullptr;
-  cudaStream_t side = nullptr;     // K0 runs here, concurrently with K1 on the caller's stream
-  bool last_overlapped = false;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  bool have_result = false;
-  int debug_stage = 0;
-  size_t n_rows = 0, n_items = 0, cbytes = 0; bool canvas_fully_covered = true; int max_log2_ctb = 6, info_bps = 1;
-  // Band pipeline of the fused host entry points (large grids): after K0, the tile rows go through K1 -> K3 -> K4 -> K6 in
-  // bands (chunks), and the D2H of band c (copy stream, chunk_hook) overlaps the kernels of band c + 1.
-  int nchunks = 1, grid_cols = 1; bool last_chunked = false;
-  int chunk_pic[MAX_CHUNKS + 1] = {0}; size_t chunk_item[MAX_CHUNKS + 1] = {0};
-  std::function<int(int, cudaStream_t)> chunk_hook;   // queued after K4 of band c on the decode stream
-  cudaEvent_t ev_chunk[MAX_CHUNKS] = {nullptr};
-  ~b200_decoder() {
-    delete pool;
-    pics.release(); ctus.release(); tus.release(); coefs.release(); slices.release(); qp8.release(); edge8.release(); scaling.release(); rows.release();
-    sync.release(); rec.release(); canvas.release(); rgb2[0].release(); rgb2[1].release(); bounce.release();
-    if (own) cudaStreamDestroy(own);
-    if (copy) cudaStreamDestroy(copy);
-    for (auto& e : ev_band) if (e) cudaEventDestroy(e);
-    for (auto& e : ev_k6) if (e) cudaEventDestroy(e);
-    for (auto& e : ev_d2h) if (e) cudaEventDestroy(e);
-    if (err_host) cudaFreeHost(err_host);
-    rbsp.release(); subs.release(); equeue.release(); ctu_slice.release(); epics.release(); ipm4.release(); cd8.release(); wpp_ctx.release();
-    end_state.release(); esync.release(); ecount.release();
-    for (auto& e : ev) if (e) cudaEventDestroy(e);
-    if (ev_fork) cudaEventDestroy(ev_fork);
-    if (ev_join) cudaEventDestroy(ev_join);
-    if (side) cudaStreamDestroy(side);
-    for (auto& e : ev_chunk) if (e) cudaEventDestroy(e);
-  }
+  // Band pipeline of the synchronous fused entry point (large grids): after K0, the tile rows go through K1 -> K3 -> K4 -> K6
+  // in bands, and the D2H of band c (copy stream, band_hook) overlaps the kernels of band c + 1.
+  std::function<int(int, cudaStream_t)> band_hook;    // queued after K4 of band c on the decode stream
 };
 
 static int check_device_error(b200_decoder* d) {
   unsigned flag = 0;
-  B200_CUDA_CHECK(cudaMemcpy(&flag, d->sync.d + 1, sizeof flag, cudaMemcpyDeviceToHost));
+  B200_CUDA_CHECK(cudaMemcpy(&flag, d->sync.d + ScratchLayout::error_flag, sizeof flag, cudaMemcpyDeviceToHost));
   if (flag) return set_error(B200_E_CUDA, "reconstruction kernel gave up waiting for a CTB row dependency");
   return B200_OK;
 }
 
-// K0 (entropy) and K1 (reconstruction) can run CONCURRENTLY: K1 consumes the command stream CTB by CTB as K0 publishes
-// it.  Both kernels are persistent and ticket-driven, so they need not be fully co-resident (whatever part of either
-// grid is resident finishes the work); the caps below only share the SM's registers between them.
-// The overlap hides K1 completely while the batch is critical-path bound -- up to about one wave of sub-streams -- and
-// LOSES once the GPU is throughput bound (the two instruction streams evict each other), so it is chosen
-// per batch.  B200_OVERLAP=0/1 forces it.
-static int overlap_blocks(const char* env, int dflt) { if (const char* e = getenv(env)) { const int v = atoi(e); if (v >= 1 && v <= 4) return v; } return dflt; }
 // At most ONE overlapped K0/K1 pair is in flight per process: libheif drives many decoder instances from its own threads,
 // and the spinning K1 grids of many instances must never be able to keep all their K0 grids off the GPU.  A batch that
 // finds the slot taken simply runs its kernels back to back.
@@ -158,117 +257,361 @@ static void overlap_release() {
 }
 static void CUDART_CB overlap_done(void*) { overlap_release(); }
 
-static bool use_overlap(size_t n_subs) {
-  if (const char* e = getenv("B200_OVERLAP")) return atoi(e) != 0;
-  int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return n_subs <= (size_t)sms * 16;      // one wave of K0: 4 CTAs x 4 warps per SM
-}
-// TAIL overlap, for batches of more than one wave: K0 keeps the whole GPU (4 CTAs per SM, launched first) and the LIVE K1
-// is queued behind it on the other stream, so K1's CTAs become resident only where K0's persistent CTAs have left -- which
-// they do over the last ~30 % of K0's run time, once every sub-stream has been handed out and the wavefronts of the tiles
-// drain.  K1 (and, with bands, K3 / K4 / K6 / D2H of the first band) then runs in SM slots that would otherwise idle.
-// B200_TAIL_OVERLAP=0 switches it off; 1 (default): with row bands, one live K1 per band (the first band's K1 ends with K0, its
-// filters / K6 / D2H overlap the second band's K1); 2: ONE live K1 over the whole grid, bands only for K3 / K4 / K6 / D2H
-// (slower end to end: nothing is left to overlap the first band's D2H).
-static int use_tail_overlap() {
-  if (const char* e = getenv("B200_TAIL_OVERLAP")) return atoi(e);
-  return 1;
-}
-
-// Device half: K0 entropy decoding (device front-end only) on the side stream, concurrently K1 reconstruction on `s`
-// consuming the command stream CTB by CTB as K0 publishes it, then deblocking and SAO / paste on `s`.
-static int run_device_pipeline(b200_decoder* d, int n, cudaStream_t s, int* launches_out) {
+// Device half, as the plan says: K0 entropy decoding (device front-end only), on the side stream when it overlaps K1
+// reconstruction on `s`, then deblocking and SAO / paste on `s` -- for the whole batch or band by band.
+static int run_device_pipeline(b200_decoder* d, const LaunchPlan& plan, cudaStream_t s, int* launches_out) {
   int rc;
   int launches = 0;
-  const bool devfe = d->used_device_front_end;
-  // bands only pay for the caller that takes them one by one (the synchronous fused entry point); everything else -- the
-  // composition API, b200_decoder_rerun_device, the asynchronous entry point whose D2H already overlaps the next picture --
-  // runs one launch per kernel (the band-major row list is a valid ticket order for that, too)
-  const char* force = getenv("B200_CHUNKS");
-  const bool chunked = d->nchunks > 1 && (d->chunk_hook || (force && atoi(force) != 0));
-  bool overlap = devfe && !chunked && use_overlap(d->n_subs);
-  const int tail_mode = use_tail_overlap();
-  const bool tail = devfe && !getenv("B200_OVERLAP") && tail_mode != 0 && (!overlap || getenv("B200_TAIL_FORCE"));   // B200_TAIL_FORCE: small batches too (tests)
-  if (tail) overlap = true;
-  // K1 follows K0 through per-row progress counters in raster order; sub-streams of HEVC tiles produce CTBs tile by tile
-  for (int i = 0; i < d->npics && overlap; i++) if (d->epics.h[i].sp.tiles) overlap = false;
-  if (overlap) overlap = overlap_acquire(d);
+  const bool devfe = d->shape.device_front_end;
+  const bool overlap = plan.overlap && overlap_acquire(d);
   struct Release { bool armed; ~Release() { if (armed) overlap_release(); } } release{overlap};   // error paths
-  d->last_overlapped = overlap; d->last_chunked = chunked;
-  cudaEventRecord(d->ev[1], s);
+  d->last_overlapped = overlap; d->last_banded = plan.banded;
+  cudaEventRecord(d->t_h2d, s);
+  const ScratchLayout& L = d->scratch;
   DeviceBatch b{};
-  b.pics = d->pics.d; b.npics = n; b.ctus = d->ctus.d; b.tus = d->tus.d; b.coefs = d->coefs.d; b.slices = d->slices.d;
-  b.qp8 = d->qp8.d; b.edge8 = d->edge8.d; b.scaling = d->scaling.d; b.ticket = d->sync.d + 2 + 3 * d->n_rows; b.error_flag = d->sync.d + 1; b.progress = d->sync.d + 2; b.row_list = d->rows.d; b.nrows = (int)d->n_items; b.max_log2_ctb = d->max_log2_ctb; b.wide_samples = d->info_bps == 2;
+  b.pics = d->pics.d; b.npics = d->npics; b.ctus = d->ctus.d; b.tus = d->tus.d; b.coefs = d->coefs.d; b.slices = d->slices.d;
+  b.qp8 = d->qp8.d; b.edge8 = d->edge8.d; b.scaling = d->scaling.d; b.ticket = d->sync.d + L.tickets(); b.error_flag = d->sync.d + L.error_flag; b.progress = d->sync.d + L.progress;
+  b.row_list = d->rows.d; b.nrows = (int)d->n_items; b.max_log2_ctb = d->max_log2_ctb; b.wide_samples = d->info_bps == 2;
   if (devfe) {
     EntropyBatch e{};
-    e.pics = d->epics.d; e.npics = d->npics; e.subs = d->subs.d; e.nsubs = (int)d->n_subs;
-    e.qhead = d->equeue.d; e.qtail = d->equeue.d + 1; e.queue = d->equeue.d + 2; e.deps = d->equeue.d + 2 + d->n_subs;
-    e.progress = d->esync.d + 1; e.sub_done = d->esync.d + 1 + d->n_rows; e.error_flag = d->sync.d + 1;
-    e.common = 1;
-    if (getenv("B200_ENTROPY_GENERIC")) e.common = 0;
-    for (int i = 0; i < d->npics && e.common; i++) if (!syn::matches_common(d->epics.h[i].sp)) e.common = 0;
+    e.pics = d->epics.d; e.npics = d->npics; e.subs = d->subs.d; e.nsubs = (int)L.n_subs;
+    e.qhead = d->equeue.d + L.qhead; e.qtail = d->equeue.d + L.qtail; e.queue = d->equeue.d + L.queue; e.deps = d->equeue.d + L.deps();
+    e.progress = d->esync.d + L.entropy_progress; e.sub_done = d->esync.d + L.sub_done(); e.error_flag = d->sync.d + L.error_flag;
+    e.common = plan.common_k0;
     if (overlap) {
-      if (!d->side) { B200_CUDA_CHECK(cudaStreamCreateWithFlags(&d->side, cudaStreamNonBlocking)); B200_CUDA_CHECK(cudaEventCreate(&d->ev_fork)); B200_CUDA_CHECK(cudaEventCreate(&d->ev_join)); }
-      e.blocks_per_sm = tail ? 0 : overlap_blocks("B200_OVERLAP_K0_BLOCKS", 3);
-      b.blocks_per_sm = tail ? 0 : overlap_blocks("B200_OVERLAP_K1_BLOCKS", 2);
+      e.blocks_per_sm = plan.k0_blocks_per_sm;
+      b.blocks_per_sm = plan.k1_blocks_per_sm;
       b.entropy_progress = e.progress;
       cudaEventRecord(d->ev_fork, s);
       B200_CUDA_CHECK(cudaStreamWaitEvent(d->side, d->ev_fork, 0));
       int k0_warps = 0;
       if ((rc = launch_entropy(e, d->side, &k0_warps))) return rc;
-      cudaEventRecord(d->ev[5], d->side);
+      cudaEventRecord(d->t_entropy, d->side);
       if ((rc = launch_entropy_stats(e, d->ecount.d, d->side))) return rc;
       cudaEventRecord(d->ev_join, d->side);
-      if (tail) { if ((rc = launch_entropy_gate(e, k0_warps, s))) return rc; launches += 1; }   // K1 (next on s) must not take the SMs before K0 has them
+      if (plan.tail) { if ((rc = launch_entropy_gate(e, k0_warps, s))) return rc; launches += 1; }   // K1 (next on s) must not take the SMs before K0 has them
     } else {
       if ((rc = launch_entropy(e, s))) return rc;
-      cudaEventRecord(d->ev[5], s);
+      cudaEventRecord(d->t_entropy, s);
       if ((rc = launch_entropy_stats(e, d->ecount.d, s))) return rc;
     }
     launches += 1;
-  } else cudaEventRecord(d->ev[5], s);
-  if (chunked) {
+  } else cudaEventRecord(d->t_entropy, s);
+  if (plan.banded) {
     // Row bands of a large grid leave the pipeline one after the other: K1 -> K3 -> K4 of band c, then the caller's hook
     // (K6 of the band + its D2H on the copy stream, which overlaps the kernels of band c + 1).  K0 is NOT part of this:
     // letting the bands leave K0 in order (priority queues) and running these kernels beside it was measured slower --
     // K0 loses more from the co-residency (3 instead of 4 CTAs per SM) and the priorities than the overlap gains.
-    const bool one_k1 = overlap && tail_mode == 2;
-    if (one_k1) { if ((rc = launch_recon(b, s))) return rc; launches += 1; }   // the band-major row list is a valid ticket order for one launch
-    for (int c = 0; c < d->nchunks; c++) {
+    for (int c = 0; c < d->shape.bands; c++) {
       DeviceBatch bc = b;
-      bc.row_list = d->rows.d + d->chunk_item[c]; bc.nrows = (int)(d->chunk_item[c + 1] - d->chunk_item[c]); bc.ticket = b.ticket + c;
-      if (!one_k1 && (rc = launch_recon(bc, s))) return rc;
-      if (overlap && (one_k1 ? c == 0 : c + 1 == d->nchunks)) {   // (tail overlap) K0 has finished before anything that follows the last K1
+      bc.row_list = d->rows.d + d->band_item[c]; bc.nrows = (int)(d->band_item[c + 1] - d->band_item[c]); bc.ticket = b.ticket + c;
+      if ((rc = launch_recon(bc, s))) return rc;
+      if (overlap && c + 1 == d->shape.bands) {   // (tail overlap) K0 has finished before anything that follows the last K1
         B200_CUDA_CHECK(cudaStreamWaitEvent(s, d->ev_join, 0));
         B200_CUDA_CHECK(cudaLaunchHostFunc(s, overlap_done, nullptr));
         release.armed = false;
       }
       DeviceBatch bf = b;
-      const int p0 = d->chunk_pic[c];
-      bf.pics = d->pics.d + p0; bf.npics = d->chunk_pic[c + 1] - p0;
+      const int p0 = d->band_pic[c];
+      bf.pics = d->pics.d + p0; bf.npics = d->band_pic[c + 1] - p0;
       if (d->debug_stage != 1 && (rc = launch_deblock(bf, d->pics.h + p0, s))) return rc;
       int nsao = 0;
       if (d->debug_stage == 0 && (rc = launch_sao(bf, d->pics.h + p0, s, &nsao))) return rc;
       launches += 3 + nsao;
-      if (d->chunk_hook && (rc = d->chunk_hook(c, s))) return rc;
+      if (d->band_hook && (rc = d->band_hook(c, s))) return rc;
     }
-    cudaEventRecord(d->ev[2], s); cudaEventRecord(d->ev[3], s); cudaEventRecord(d->ev[4], s);   // recon_ms = the whole band pipeline (incl. the hooks' K6)
+    cudaEventRecord(d->t_recon, s); cudaEventRecord(d->t_deblock, s); cudaEventRecord(d->t_sao, s);   // recon_ms = the whole band pipeline (incl. the hooks' K6)
     if (launches_out) *launches_out = launches;
     return B200_OK;
   }
   if ((rc = launch_recon(b, s))) return rc;
-  if (devfe && overlap) {
+  if (overlap) {
     B200_CUDA_CHECK(cudaStreamWaitEvent(s, d->ev_join, 0));
     B200_CUDA_CHECK(cudaLaunchHostFunc(s, overlap_done, nullptr));   // the slot is free once K0 and K1 have both finished
     release.armed = false;
   }
-  cudaEventRecord(d->ev[2], s);
+  cudaEventRecord(d->t_recon, s);
   launches += 1;
   if (d->debug_stage != 1) { if ((rc = launch_deblock(b, d->pics.h, s))) return rc; launches += 2; }
-  cudaEventRecord(d->ev[3], s);
+  cudaEventRecord(d->t_deblock, s);
   if (d->debug_stage == 0) { int nsao = 0; if ((rc = launch_sao(b, d->pics.h, s, &nsao))) return rc; launches += nsao; }
-  cudaEventRecord(d->ev[4], s);
+  cudaEventRecord(d->t_sao, s);
   if (launches_out) *launches_out = launches;
+  return B200_OK;
+}
+
+// ---- the stages of b200_decoder_decode_grid
+
+// Host stage, one tile per task.  Host front-end: headers + CABAC + syntax (serial per sub-stream).  Device front-end:
+// headers only (NAL split, emulation prevention removal, parameter sets, entry points).
+static int parse_stage(b200_decoder* d, int n, const uint8_t* const* au, const size_t* au_size, uint64_t max_pixels, bool devfe) {
+  d->parsed.resize((size_t)n); d->parse_rc.assign((size_t)n, 0); d->parse_msg.assign((size_t)n, std::string());
+  ParseLimits lim; lim.max_image_size_pixels = max_pixels;
+  d->pool->parallel_for(n, [&](int i) {
+    ParsedPicture& pp = d->parsed[(size_t)i];
+    int rc = devfe ? parse_headers(au[i], au_size[i], lim, pp.hdr) : parse_access_unit(au[i], au_size[i], lim, pp);
+    if (!rc && devfe) pp.desc = pp.hdr.desc;
+    d->parse_rc[(size_t)i] = rc;
+    if (rc) d->parse_msg[(size_t)i] = b200_last_error();
+  });
+  for (int i = 0; i < n; i++) if (d->parse_rc[(size_t)i]) return set_error(d->parse_rc[(size_t)i], "tile %d: %s", i, d->parse_msg[(size_t)i].c_str());
+  return B200_OK;
+}
+
+struct Layout {                 // the sizes of one batch and where each picture sits in the batch-wide arrays
+  int n = 0, cols = 1, rows = 1, tw = 0, th = 0, bd = 8, chroma = 0, bps = 1, csx = 0, csy = 0, cw = 0, ch = 0;
+  size_t n_ctu = 0, n_tu = 0, n_coef = 0, n_slice = 0, n_map = 0, n_map4 = 0, n_rows = 0, n_rbsp = 0, n_subs = 0;
+  size_t rec_bytes = 0, canvas_bytes = 0, bits = 0;
+  int n_scaling = 0;            // pictures with scaling lists: one 780-byte factor table each (784-byte slots)
+  std::vector<size_t> rec_off, rbsp_off, sub_off, map4_off;   // per picture (rec_off: per plane)
+  bool canvas_covered = true;   // the tiles cover the whole canvas
+};
+
+// Checks that the tiles agree, gives every picture its offsets in the batch-wide arrays (written into its PicDesc) and
+// lays out the canvas planes.
+static int layout_stage(b200_decoder* d, int cols, int rows, const size_t* au_size, int canvas_w, int canvas_h, bool devfe, Layout& L) {
+  const int n = cols * rows;
+  L.n = n; L.cols = cols; L.rows = rows;
+  const PicDesc& p0 = d->parsed[0].desc;
+  L.tw = p0.out_w; L.th = p0.out_h; L.bd = p0.bit_depth; L.chroma = p0.chroma; L.bps = L.bd > 8 ? 2 : 1;
+  for (int i = 1; i < n; i++) {
+    const PicDesc& p = d->parsed[(size_t)i].desc;
+    if (p.out_w != L.tw || p.out_h != L.th || p.bit_depth != L.bd || p.chroma != L.chroma)
+      return set_error(B200_E_UNSUPPORTED, "grid tiles differ in size or format (tile %d)", i);   // grid.cc:261-375 requires equal tiles
+  }
+  L.csx = (L.chroma == 1 || L.chroma == 2) ? 1 : 0; L.csy = L.chroma == 1 ? 1 : 0;          // chroma sub-sampling shifts (Table 6-1)
+  if (n > 1 && (((L.tw & 1) && L.csx) || ((L.th & 1) && L.csy))) return set_error(B200_E_UNSUPPORTED, "grid tiles of odd size with sub-sampled chroma");
+  L.cw = canvas_w > 0 ? canvas_w : L.tw * cols; L.ch = canvas_h > 0 ? canvas_h : L.th * rows;
+  L.rec_off.resize((size_t)n * 3); L.rbsp_off.resize((size_t)n); L.sub_off.resize((size_t)n); L.map4_off.resize((size_t)n);
+  for (int i = 0; i < n; i++) {
+    ParsedPicture& pp = d->parsed[(size_t)i]; PicDesc& p = pp.desc;
+    const size_t nctb = (size_t)p.wctb * p.hctb;
+    p.ctu_base = (uint32_t)L.n_ctu; p.tu_base = (uint32_t)L.n_tu; p.coef_base = L.n_coef; p.slice_base = (uint32_t)L.n_slice; p.map8_base = (uint32_t)L.n_map;
+    p.progress_base = (uint32_t)L.n_rows;
+    L.rbsp_off[(size_t)i] = L.n_rbsp; L.sub_off[(size_t)i] = L.n_subs; L.map4_off[(size_t)i] = L.n_map4;
+    L.n_ctu += nctb; L.n_slice += (devfe ? pp.hdr.slices.size() : pp.slices.size()); L.n_map += (size_t)p.w8 * p.h8; L.n_map4 += (size_t)p.w8 * p.h8 * 4; L.n_rows += (size_t)p.hctb;
+    if (devfe) { L.n_tu += nctb * (size_t)pp.hdr.sp.tu_slots; L.n_coef += nctb * (size_t)pp.hdr.sp.coef_slots; L.n_rbsp += (pp.hdr.rbsp.size() + 15) & ~(size_t)15; L.n_subs += pp.hdr.subs.size(); }
+    else { L.n_tu += pp.n_tus; L.n_coef += pp.n_coefs; }
+    L.bits += au_size[i];
+    for (int c = 0; c < (L.chroma ? 3 : 1); c++) {
+      const int w = c ? p.width >> L.csx : p.width, h = c ? p.height >> L.csy : p.height;
+      const int st = (w + 63) & ~63;
+      p.rec_stride[c] = st;
+      L.rec_off[(size_t)i * 3 + c] = L.rec_bytes;
+      L.rec_bytes += (size_t)st * h * L.bps; L.rec_bytes = (L.rec_bytes + 255) & ~(size_t)255;
+    }
+  }
+  for (int i = 0; i < n; i++) { ParsedPicture& pp = d->parsed[(size_t)i]; pp.desc.scaling_idx = pp.hdr.scaling_enabled ? L.n_scaling++ : -1; }
+  if (L.n_tu > 0xffffffffull) return set_error(B200_E_UNSUPPORTED, "batch too large");
+  for (int c = 0; c < (L.chroma ? 3 : 1); c++) {
+    const int w = c ? (L.cw + L.csx) >> L.csx : L.cw, h = c ? (L.ch + L.csy) >> L.csy : L.ch;
+    d->canvas_pitch[c] = (((size_t)w * L.bps) + 255) & ~(size_t)255;
+    d->canvas_off[c] = L.canvas_bytes; L.canvas_bytes += d->canvas_pitch[c] * h;
+  }
+  L.canvas_covered = L.tw * cols >= L.cw && L.th * rows >= L.ch;
+  return B200_OK;
+}
+
+static int reserve_stage(b200_decoder* d, const Layout& L, const ScratchLayout& S, bool devfe) {
+  int rc;
+  if ((rc = d->scaling.reserve((size_t)L.n_scaling * 784 + 16))) return rc;
+  if ((rc = d->pics.reserve((size_t)L.n)) || (rc = d->ctus.reserve(L.n_ctu, !devfe)) || (rc = d->tus.reserve(L.n_tu, !devfe)) || (rc = d->coefs.reserve(L.n_coef + 1, !devfe)) ||
+      (rc = d->slices.reserve(L.n_slice)) || (rc = d->qp8.reserve(L.n_map, !devfe)) || (rc = d->edge8.reserve(L.n_map, !devfe)) || (rc = d->rows.reserve(3 * L.n_rows)) ||
+      (rc = d->sync.reserve(S.sync_size(), false)) || (rc = d->rec.reserve(L.rec_bytes, false)))
+    return rc;
+  if (devfe && ((rc = d->rbsp.reserve(L.n_rbsp + 16)) || (rc = d->subs.reserve(L.n_subs)) || (rc = d->equeue.reserve(S.equeue_size())) || (rc = d->ctu_slice.reserve(L.n_ctu)) ||
+                (rc = d->epics.reserve((size_t)L.n)) || (rc = d->ipm4.reserve(L.n_map4, false)) || (rc = d->cd8.reserve(L.n_map, false)) ||
+                (rc = d->wpp_ctx.reserve(L.n_rows * syn::CTX_STRIDE, false)) || (rc = d->end_state.reserve(L.n_subs * syn::CTX_STRIDE + 16, false)) ||
+                (rc = d->esync.reserve(S.esync_size(), false)) || (rc = d->ecount.reserve(2, true))))
+    return rc;
+  return d->canvas.reserve(L.canvas_bytes, false);
+}
+
+// Picture descriptors with their device pointers and paste positions, the scaling factors, and the row list: the CTB rows in
+// launch order, row-major ACROSS pictures (all first rows, then all second rows, ...) within each band.  A row's predecessor
+// always holds a smaller ticket (deadlock freedom), and the resident warps spread over every tile's wavefront instead of
+// idling behind one tile's 2-CTB stagger.
+static void pack_pictures(b200_decoder* d, const Layout& L, const LaunchPlan& plan) {
+  const int n = L.n;
+  for (int i = 0; i < n; i++) {
+    ParsedPicture& pp = d->parsed[(size_t)i]; PicDesc& p = pp.desc;
+    if (p.scaling_idx >= 0) memcpy(d->scaling.h + (size_t)p.scaling_idx * 784, &pp.hdr.scaling, sizeof(sl::Factors));
+    const int col = i % L.cols, row = i / L.cols;
+    const int px = col * L.tw, py = row * L.th;
+    p.out_w = std::max(0, std::min(L.tw, L.cw - px)); p.out_h = std::max(0, std::min(L.th, L.ch - py));     // clip like copy_image_to
+    for (int c = 0; c < 3; c++) {
+      if (c && !L.chroma) { p.rec[c] = nullptr; p.dst[c] = nullptr; continue; }
+      p.rec[c] = d->rec.d + L.rec_off[(size_t)i * 3 + c];
+      const int sx = c ? px >> L.csx : px, sy = c ? py >> L.csy : py;
+      p.dst[c] = d->canvas.d + d->canvas_off[c] + (size_t)sy * d->canvas_pitch[c] + (size_t)sx * L.bps;
+      p.dst_stride[c] = (int)(d->canvas_pitch[c] / L.bps);
+    }
+    d->pics.h[i] = p;
+  }
+  for (int c = 0; c <= plan.bands; c++) d->band_pic[c] = std::min(n, c * plan.rows_per_band * L.cols);
+  d->band_pic[plan.bands] = n;
+  size_t row_cursor = 0; d->max_log2_ctb = 4;
+  for (int i = 0; i < n; i++) d->max_log2_ctb = std::max(d->max_log2_ctb, d->parsed[(size_t)i].desc.log2_ctb);
+  for (int c = 0; c < plan.bands; c++) {
+    d->band_item[c] = row_cursor;
+    int max_h = 0;
+    for (int i = d->band_pic[c]; i < d->band_pic[c + 1]; i++) max_h = std::max(max_h, d->parsed[(size_t)i].desc.hctb);
+    for (int r = 0; r < max_h; r++) for (int i = d->band_pic[c]; i < d->band_pic[c + 1]; i++) if (r < d->parsed[(size_t)i].desc.hctb) {
+      d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r);                                        // luma
+      if (L.chroma == 1) d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r | (1u << 30));         // Cb + Cr of a 4:2:0 picture on the two half-warps
+      else if (L.chroma >= 2) { d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r | (2u << 30)); d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r | (3u << 30)); }   // Cb, Cr planes (4:2:2 / 4:4:4)
+    }
+  }
+  d->band_item[plan.bands] = row_cursor;
+  d->n_items = row_cursor; d->info_bps = L.bps;
+}
+
+// Host front-end: each picture's command stream into the page-locked staging (parallel)
+static void pack_host_front_end(b200_decoder* d, const Layout& L) {
+  d->pool->parallel_for(L.n, [&](int i) {
+    const ParsedPicture& pp = d->parsed[(size_t)i]; const PicDesc& p = pp.desc;
+    memcpy(d->ctus.h + p.ctu_base, pp.ctus.data(), (size_t)p.wctb * p.hctb * sizeof(CtuInfo));
+    memcpy(d->tus.h + p.tu_base, pp.tus.data(), pp.n_tus * sizeof(TuCmd));
+    memcpy(d->coefs.h + p.coef_base, pp.coefs.data(), pp.n_coefs * sizeof(CoefEntry));
+    memcpy(d->slices.h + p.slice_base, pp.slices.data(), pp.slices.size() * sizeof(SliceInfo));
+    memcpy(d->qp8.h + p.map8_base, pp.qp8.data(), (size_t)p.w8 * p.h8);
+    memcpy(d->edge8.h + p.map8_base, pp.edge8.data(), (size_t)p.w8 * p.h8);
+  });
+}
+
+// Device front-end: each picture's slice data, sub-streams and entropy descriptor into the page-locked staging (parallel)
+static void pack_device_front_end(b200_decoder* d, const Layout& L) {
+  d->pool->parallel_for(L.n, [&](int i) {
+    const ParsedPicture& pp = d->parsed[(size_t)i]; const PicDesc& p = pp.desc;
+    const PictureHeaders& H = pp.hdr;
+    memcpy(d->slices.h + p.slice_base, H.slices.data(), H.slices.size() * sizeof(SliceInfo));
+    memcpy(d->rbsp.h + L.rbsp_off[(size_t)i], H.rbsp.data(), H.rbsp.size());
+    memcpy(d->ctu_slice.h + p.ctu_base, H.ctu_slice.data(), H.ctu_slice.size() * sizeof(uint16_t));
+    // Ready-queue links (batch-wide indices): which sub-stream each one releases, and how many events each waits for before
+    // its first bin -- the conditions of run_substream (b200_hevc_syntax.h): the contexts stored after the 2nd CTB of the
+    // row above (WPP, 9.3.2.2) and the end state of the slice segment it continues.
+    const size_t so = L.sub_off[(size_t)i];
+    for (size_t k = 0; k < H.subs.size(); k++) { syn::Substream ss = H.subs[k]; ss.pic = (uint32_t)i; ss.wake_ctb2 = ss.wake_end = -1; ss.deps = 0; d->subs.h[so + k] = ss; }
+    for (size_t k = 0; k < H.subs.size(); k++) {
+      syn::Substream& ss = d->subs.h[so + k];
+      if (ss.prev >= 0) { ss.deps++; d->subs.h[so + (size_t)ss.prev].wake_end = (int32_t)(so + k); }
+      const int wctb = H.desc.wctb, rx0 = (int)(ss.ctb_begin % (uint32_t)wctb), ry0 = (int)(ss.ctb_begin / (uint32_t)wctb);
+      if (H.sp.wpp && rx0 == 0 && (!ss.init_contexts || ss.prev >= 0) && ss.ctb_begin != ss.slice_addr_rs && ry0 > 0 && (1 << H.desc.log2_ctb) < H.desc.width &&
+          H.ctu_slice[(size_t)(ry0 - 1) * wctb + 1] == (uint16_t)ss.slice_idx) {
+        const uint32_t a = (uint32_t)(ry0 - 1) * (uint32_t)wctb + 1;
+        for (size_t j = 0; j < H.subs.size(); j++) if (H.subs[j].ctb_begin <= a && a < H.subs[j].ctb_end) { ss.deps++; d->subs.h[so + j].wake_ctb2 = (int32_t)(so + k); break; }
+      }
+    }
+    EntropyPic ep{};
+    ep.sp = H.sp; ep.sp.dense = 0;
+    ep.pb.rbsp = d->rbsp.d + L.rbsp_off[(size_t)i]; ep.pb.rbsp_size = (uint32_t)H.rbsp.size();
+    ep.pb.tus = d->tus.d + p.tu_base; ep.pb.coefs = d->coefs.d + p.coef_base; ep.pb.ctus = d->ctus.d + p.ctu_base; ep.pb.slices = d->slices.d + p.slice_base;
+    ep.pb.ctu_slice = d->ctu_slice.d + p.ctu_base; ep.pb.qp8 = d->qp8.d + p.map8_base; ep.pb.edge8 = d->edge8.d + p.map8_base;
+    ep.pb.ipm4 = d->ipm4.d + L.map4_off[(size_t)i]; ep.pb.cd8 = d->cd8.d + p.map8_base;
+    ep.pb.wpp_ctx = d->wpp_ctx.d + (size_t)p.progress_base * syn::CTX_STRIDE; ep.pb.end_state = d->end_state.d + L.sub_off[(size_t)i] * syn::CTX_STRIDE;
+    ep.progress_base = p.progress_base; ep.sub_base = (uint32_t)L.sub_off[(size_t)i];
+    d->epics.h[i] = ep;
+  });
+}
+
+// Ready queue image (device front-end): cursors, the sub-streams without prerequisites in "k-th sub-stream of every
+// picture" order (so that whatever a popped sub-stream polls for was popped before it), empty slots, the dependency counters
+static void build_ready_queue(b200_decoder* d, const Layout& L, const ScratchLayout& S) {
+  unsigned* q = d->equeue.h; size_t cur = 0, maxs = 0;
+  for (int i = 0; i < L.n; i++) maxs = std::max(maxs, d->parsed[(size_t)i].hdr.subs.size());
+  for (size_t k = 0; k < maxs; k++) for (int i = 0; i < L.n; i++)
+    if (k < d->parsed[(size_t)i].hdr.subs.size() && d->subs.h[L.sub_off[(size_t)i] + k].deps == 0) q[S.queue + cur++] = (unsigned)(L.sub_off[(size_t)i] + k) + 1u;
+  q[S.qhead] = 0; q[S.qtail] = (unsigned)cur;
+  for (size_t k = cur; k < L.n_subs; k++) q[S.queue + k] = 0;
+  for (size_t k = 0; k < L.n_subs; k++) q[S.deps() + k] = d->subs.h[k].deps;
+}
+
+// Clears the counters of a run (and restores K0's ready queue), on `s`
+static int reset_scratch(b200_decoder* d, const ScratchLayout& S, bool devfe, cudaStream_t s) {
+  if (devfe) {
+    B200_CUDA_CHECK(cudaMemsetAsync(d->esync.d, 0, S.esync_size() * sizeof(unsigned), s));
+    B200_CUDA_CHECK(cudaMemsetAsync(d->ecount.d, 0, 2 * sizeof(unsigned long long), s));
+  }
+  B200_CUDA_CHECK(cudaMemsetAsync(d->sync.d, 0, S.sync_size() * sizeof(unsigned), s));
+  return B200_OK;
+}
+
+// H2D of the staged batch on `s`; *h2d = the bytes copied
+static int upload_stage(b200_decoder* d, const Layout& L, const ScratchLayout& S, bool devfe, cudaStream_t s, size_t* h2d) {
+  const int n = L.n;
+  B200_CUDA_CHECK(cudaMemcpyAsync(d->pics.d, d->pics.h, (size_t)n * sizeof(PicDesc), cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d->slices.d, d->slices.h, L.n_slice * sizeof(SliceInfo), cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(d->rows.d, d->rows.h, d->n_items * sizeof(uint2), cudaMemcpyHostToDevice, s));
+  if (L.n_scaling) B200_CUDA_CHECK(cudaMemcpyAsync(d->scaling.d, d->scaling.h, (size_t)L.n_scaling * 784, cudaMemcpyHostToDevice, s));
+  *h2d = (size_t)L.n_scaling * 784 + (size_t)n * sizeof(PicDesc) + L.n_slice * sizeof(SliceInfo) + d->n_items * sizeof(uint2);
+  if (!devfe) {
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->ctus.d, d->ctus.h, L.n_ctu * sizeof(CtuInfo), cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->tus.d, d->tus.h, L.n_tu * sizeof(TuCmd), cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->coefs.d, d->coefs.h, L.n_coef * sizeof(CoefEntry), cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->qp8.d, d->qp8.h, L.n_map, cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->edge8.d, d->edge8.h, L.n_map, cudaMemcpyHostToDevice, s));
+    *h2d += L.n_ctu * sizeof(CtuInfo) + L.n_tu * sizeof(TuCmd) + L.n_coef * sizeof(CoefEntry) + 2 * L.n_map;
+  } else {
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->rbsp.d, d->rbsp.h, L.n_rbsp, cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->subs.d, d->subs.h, L.n_subs * sizeof(syn::Substream), cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->equeue.d, d->equeue.h, S.equeue_size() * sizeof(unsigned), cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->ctu_slice.d, d->ctu_slice.h, L.n_ctu * sizeof(uint16_t), cudaMemcpyHostToDevice, s));
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->epics.d, d->epics.h, (size_t)n * sizeof(EntropyPic), cudaMemcpyHostToDevice, s));
+    *h2d += L.n_rbsp + L.n_subs * (sizeof(syn::Substream) + 2 * sizeof(unsigned)) + L.n_ctu * sizeof(uint16_t) + (size_t)n * sizeof(EntropyPic);
+  }
+  int rc;
+  if ((rc = reset_scratch(d, S, devfe, s))) return rc;
+  if (!L.canvas_covered) B200_CUDA_CHECK(cudaMemsetAsync(d->canvas.d, 0, L.canvas_bytes, s));     // uncovered canvas stays zero (calloc in the reference)
+  return B200_OK;
+}
+
+static int decode_grid(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size, uint64_t max_pixels,
+                       int canvas_w, int canvas_h, b200_image_info* info, cudaStream_t s, const Overrides& env) {
+  if (!d || !au || !au_size || cols <= 0 || rows <= 0) return set_error(B200_E_INVALID, "bad argument");
+  const double t0 = now_ms();
+  const bool devfe = d->front_end != 0;
+  d->have_result = false;
+  int rc;
+  if ((rc = parse_stage(d, cols * rows, au, au_size, max_pixels, devfe))) return rc;
+  const double t1 = now_ms();
+  Layout L;
+  if ((rc = layout_stage(d, cols, rows, au_size, canvas_w, canvas_h, devfe, L))) return rc;
+  BatchShape shape;
+  shape.cols = cols; shape.rows = rows; shape.device_front_end = devfe; shape.n_subs = L.n_subs; shape.all_common = devfe;
+  if (devfe) for (int i = 0; i < L.n; i++) {
+    syn::SeqParams sp = d->parsed[(size_t)i].hdr.sp; sp.dense = 0;       // as K0 sees it (EntropyPic::sp)
+    shape.any_tiles |= sp.tiles != 0; shape.all_common &= syn::matches_common(sp);
+  }
+  const LaunchPlan plan = plan_launches(shape, bool(d->band_hook), env);
+  shape.bands = plan.bands;
+  const ScratchLayout S{L.n_rows, L.n_subs};
+  if ((rc = reserve_stage(d, L, S, devfe))) return rc;
+  pack_pictures(d, L, plan);
+  if (devfe) { pack_device_front_end(d, L); build_ready_queue(d, L, S); }
+  else pack_host_front_end(d, L);
+  const double t2 = now_ms();
+  cudaEventRecord(d->t_start, s);
+  size_t h2d = 0;
+  if ((rc = upload_stage(d, L, S, devfe, s, &h2d))) return rc;
+  d->shape = shape; d->scratch = S; d->npics = L.n;
+  b200_image_info& inf = d->info;
+  inf.width = L.cw; inf.height = L.ch; inf.tile_width = L.tw; inf.tile_height = L.th; inf.chroma = L.chroma;        /* B200_CHROMA_MONO / 420 / 422 / 444 = chroma_format_idc */ inf.bit_depth = L.bd;
+  inf.colour_primaries = d->parsed[0].hdr.colour_primaries; inf.transfer_characteristics = d->parsed[0].hdr.transfer_characteristics;
+  inf.matrix_coefficients = d->parsed[0].hdr.matrix_coefficients; inf.full_range = d->parsed[0].hdr.full_range;
+  if (info) *info = inf;
+  int launches = 0;
+  if ((rc = run_device_pipeline(d, plan, s, &launches))) return rc;
+  d->last_stream = s; d->have_result = true;
+  b200_decode_stats& st = d->stats;
+  memset(&st, 0, sizeof st);
+  st.parse_ms = t1 - t0; st.pack_ms = t2 - t1; st.total_ms = now_ms() - t0;
+  st.bitstream_bytes = L.bits; st.ctus = L.n_ctu;
+  if (!devfe) {
+    st.coefficient_entries = L.n_coef; st.transform_units = L.n_tu;
+    st.command_bytes = L.n_ctu * sizeof(CtuInfo) + L.n_tu * sizeof(TuCmd) + L.n_coef * sizeof(CoefEntry) + L.n_slice * sizeof(SliceInfo) + 2 * L.n_map + (size_t)L.n * sizeof(PicDesc);
+  }
+  st.h2d_bytes = h2d;
+  st.pixels = (uint64_t)L.cw * L.ch; st.kernel_launches = launches;
   return B200_OK;
 }
 
@@ -279,10 +622,16 @@ int b200_decoder_create(b200_decoder** out, int host_threads) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_error(B200_E_CUDA, "no CUDA device: libb200heif has no CPU fallback");
   if (host_threads <= 0) { long n = sysconf(_SC_NPROCESSORS_ONLN); host_threads = n > 0 ? (int)n : 1; }
-  b200_decoder* d = new b200_decoder;
-  d->pool = new Pool(host_threads);
-  for (auto& e : d->ev) if (cudaEventCreate(&e) != cudaSuccess) { delete d; return set_error(B200_E_CUDA, "cudaEventCreate failed"); }
-  *out = d;
+  std::unique_ptr<b200_decoder> d(new b200_decoder);
+  d->pool.reset(new Pool(host_threads));
+  for (Stream* st : {&d->own, &d->copy, &d->side}) B200_CUDA_CHECK(cudaStreamCreateWithFlags(&st->h, cudaStreamNonBlocking));
+  for (Event* e : {&d->t_start, &d->t_h2d, &d->t_entropy, &d->t_recon, &d->t_deblock, &d->t_sao, &d->ev_fork, &d->ev_join}) B200_CUDA_CHECK(cudaEventCreate(&e->h));
+  for (int i = 0; i < 2; i++)
+    for (Event* e : {&d->ev_k6[i], &d->ev_d2h[i], &d->ev_bounce[i]}) B200_CUDA_CHECK(cudaEventCreateWithFlags(&e->h, cudaEventDisableTiming));
+  for (Event& e : d->ev_band) B200_CUDA_CHECK(cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming));
+  B200_CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&d->err_host.h), 2 * sizeof(unsigned), cudaHostAllocDefault));
+  d->err_host.h[0] = d->err_host.h[1] = 0;
+  *out = d.release();
   return B200_OK;
 }
 
@@ -294,256 +643,36 @@ int b200_decoder_set_front_end(b200_decoder* d, int device) { if (!d) return B20
 
 int b200_decoder_decode_grid(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
                              uint64_t max_pixels, int canvas_w, int canvas_h, b200_image_info* info, void* stream_) {
-  if (!d || !au || !au_size || cols <= 0 || rows <= 0) return set_error(B200_E_INVALID, "bad argument");
-  cudaStream_t s = (cudaStream_t)stream_;
-  const int n = cols * rows;
-  const double t0 = now_ms();
-  const bool devfe = d->front_end != 0;
-  d->have_result = false;
-  d->parsed.resize((size_t)n); d->parse_rc.assign((size_t)n, 0); d->parse_msg.assign((size_t)n, std::string());
-  ParseLimits lim; lim.max_image_size_pixels = max_pixels;
-  // ---- 1. host stage, one tile per task.  Host front-end: headers + CABAC + syntax (serial per sub-stream).
-  //         Device front-end: headers only (NAL split, emulation prevention removal, parameter sets, entry points).
-  d->pool->parallel_for(n, [&](int i) {
-    ParsedPicture& pp = d->parsed[(size_t)i];
-    int rc = devfe ? parse_headers(au[i], au_size[i], lim, pp.hdr) : parse_access_unit(au[i], au_size[i], lim, pp);
-    if (!rc && devfe) pp.desc = pp.hdr.desc;
-    d->parse_rc[(size_t)i] = rc;
-    if (rc) d->parse_msg[(size_t)i] = b200_last_error();
-  });
-  for (int i = 0; i < n; i++) if (d->parse_rc[(size_t)i]) return set_error(d->parse_rc[(size_t)i], "tile %d: %s", i, d->parse_msg[(size_t)i].c_str());
-  const double t1 = now_ms();
-  // ---- 2. layout
-  const PicDesc& p0 = d->parsed[0].desc;
-  const int tw = p0.out_w, th = p0.out_h, bd = p0.bit_depth, chroma = p0.chroma, bps = bd > 8 ? 2 : 1;
-  for (int i = 1; i < n; i++) {
-    const PicDesc& p = d->parsed[(size_t)i].desc;
-    if (p.out_w != tw || p.out_h != th || p.bit_depth != bd || p.chroma != chroma)
-      return set_error(B200_E_UNSUPPORTED, "grid tiles differ in size or format (tile %d)", i);   // grid.cc:261-375 requires equal tiles
-  }
-  const int csx = (chroma == 1 || chroma == 2) ? 1 : 0, csy = chroma == 1 ? 1 : 0;          // chroma sub-sampling shifts (Table 6-1)
-  if (n > 1 && (((tw & 1) && csx) || ((th & 1) && csy))) return set_error(B200_E_UNSUPPORTED, "grid tiles of odd size with sub-sampled chroma");
-  const int cw = canvas_w > 0 ? canvas_w : tw * cols, chh = canvas_h > 0 ? canvas_h : th * rows;
-  size_t n_ctu = 0, n_tu = 0, n_coef = 0, n_slice = 0, n_map = 0, n_rows = 0, rec_bytes = 0, bits = 0, n_rbsp = 0, n_subs = 0, n_map4 = 0;
-  d->rec_off.resize((size_t)n * 3);
-  std::vector<size_t> rbsp_off((size_t)n), sub_off((size_t)n), map4_off((size_t)n);
-  for (int i = 0; i < n; i++) {
-    ParsedPicture& pp = d->parsed[(size_t)i]; PicDesc& p = pp.desc;
-    const size_t nctb = (size_t)p.wctb * p.hctb;
-    p.ctu_base = (uint32_t)n_ctu; p.tu_base = (uint32_t)n_tu; p.coef_base = n_coef; p.slice_base = (uint32_t)n_slice; p.map8_base = (uint32_t)n_map;
-    p.progress_base = (uint32_t)n_rows;
-    rbsp_off[(size_t)i] = n_rbsp; sub_off[(size_t)i] = n_subs; map4_off[(size_t)i] = n_map4;
-    n_ctu += nctb; n_slice += (devfe ? pp.hdr.slices.size() : pp.slices.size()); n_map += (size_t)p.w8 * p.h8; n_map4 += (size_t)p.w8 * p.h8 * 4; n_rows += (size_t)p.hctb;
-    if (devfe) { n_tu += nctb * (size_t)pp.hdr.sp.tu_slots; n_coef += nctb * (size_t)pp.hdr.sp.coef_slots; n_rbsp += (pp.hdr.rbsp.size() + 15) & ~(size_t)15; n_subs += pp.hdr.subs.size(); }
-    else { n_tu += pp.n_tus; n_coef += pp.n_coefs; }
-    bits += au_size[i];
-    for (int c = 0; c < (chroma ? 3 : 1); c++) {
-      const int w = c ? p.width >> csx : p.width, h = c ? p.height >> csy : p.height;
-      const int st = (w + 63) & ~63;
-      p.rec_stride[c] = st;
-      d->rec_off[(size_t)i * 3 + c] = rec_bytes;
-      rec_bytes += (size_t)st * h * bps; rec_bytes = (rec_bytes + 255) & ~(size_t)255;
-    }
-  }
-  // scaling lists: one 780-byte factor table per picture that enables them (784-byte slots)
-  int n_scaling = 0;
-  for (int i = 0; i < n; i++) { ParsedPicture& pp = d->parsed[(size_t)i]; pp.desc.scaling_idx = pp.hdr.scaling_enabled ? n_scaling++ : -1; }
-  if (n_tu > 0xffffffffull) return set_error(B200_E_UNSUPPORTED, "batch too large");
-  int rc;
-  if ((rc = d->scaling.reserve((size_t)n_scaling * 784 + 16))) return rc;
-  for (int i = 0; i < n; i++) { const ParsedPicture& pp = d->parsed[(size_t)i]; if (pp.desc.scaling_idx >= 0) memcpy(d->scaling.h + (size_t)pp.desc.scaling_idx * 784, &pp.hdr.scaling, sizeof(sl::Factors)); }
-  if ((rc = d->pics.reserve((size_t)n)) || (rc = d->ctus.reserve(n_ctu, !devfe)) || (rc = d->tus.reserve(n_tu, !devfe)) || (rc = d->coefs.reserve(n_coef + 1, !devfe)) ||
-      (rc = d->slices.reserve(n_slice)) || (rc = d->qp8.reserve(n_map, !devfe)) || (rc = d->edge8.reserve(n_map, !devfe)) || (rc = d->rows.reserve(3 * n_rows)) ||
-      (rc = d->sync.reserve(3 * n_rows + 2 + MAX_CHUNKS, false)) || (rc = d->rec.reserve(rec_bytes, false)))
-    return rc;
-  if (devfe && ((rc = d->rbsp.reserve(n_rbsp + 16)) || (rc = d->subs.reserve(n_subs)) || (rc = d->equeue.reserve(2 + 2 * n_subs)) || (rc = d->ctu_slice.reserve(n_ctu)) ||
-                (rc = d->epics.reserve((size_t)n)) || (rc = d->ipm4.reserve(n_map4, false)) || (rc = d->cd8.reserve(n_map, false)) ||
-                (rc = d->wpp_ctx.reserve(n_rows * syn::CTX_STRIDE, false)) || (rc = d->end_state.reserve(n_subs * syn::CTX_STRIDE + 16, false)) ||
-                (rc = d->esync.reserve(1 + n_rows + n_subs, false)) || (rc = d->ecount.reserve(2, true))))
-    return rc;
-  // canvas planes
-  size_t cbytes = 0;
-  for (int c = 0; c < (chroma ? 3 : 1); c++) {
-    const int w = c ? (cw + csx) >> csx : cw, h = c ? (chh + csy) >> csy : chh;
-    d->canvas_pitch[c] = (((size_t)w * bps) + 255) & ~(size_t)255;
-    d->canvas_off[c] = cbytes; cbytes += d->canvas_pitch[c] * h;
-  }
-  const bool canvas_fully_covered = tw * cols >= cw && th * rows >= chh;
-  if ((rc = d->canvas.reserve(cbytes, false))) return rc;
-  // ---- 3. pack into pinned staging (parallel) and fix up device pointers
-  for (int i = 0; i < n; i++) {
-    ParsedPicture& pp = d->parsed[(size_t)i]; PicDesc& p = pp.desc;
-    const int col = i % cols, row = i / cols;
-    const int px = col * tw, py = row * th;
-    p.out_w = std::max(0, std::min(tw, cw - px)); p.out_h = std::max(0, std::min(th, chh - py));     // clip like copy_image_to
-    for (int c = 0; c < 3; c++) {
-      if (c && !chroma) { p.rec[c] = nullptr; p.dst[c] = nullptr; continue; }
-      p.rec[c] = d->rec.d + d->rec_off[(size_t)i * 3 + c];
-      const int sx = c ? px >> csx : px, sy = c ? py >> csy : py;
-      p.dst[c] = d->canvas.d + d->canvas_off[c] + (size_t)sy * d->canvas_pitch[c] + (size_t)sx * bps;
-      p.dst_stride[c] = (int)(d->canvas_pitch[c] / bps);
-    }
-    d->pics.h[i] = p;
-  }
-  // Launch order of the CTB rows: row-major ACROSS pictures (all first rows, then all second rows, ...).  A row's
-  // predecessor always holds a smaller ticket (deadlock freedom), and the resident warps spread over every tile's
-  // wavefront instead of idling behind one tile's 2-CTB stagger.
-  // Chunks: bands of whole tile rows for callers that take the result band by band (the fused host
-  // entry points: D2H of band c overlaps the kernels of band c + 1), when the batch is larger than what K0 and K1 overlap
-  // CTB by CTB (use_overlap).  One chunk = the classic back-to-back pipeline.
-  { int nch = 1, rpc = rows;
-    const char* ce = getenv("B200_CHUNKS");
-    if (rows >= 2 && (ce ? atoi(ce) != 0 : (d->chunk_hook && (!devfe || !use_overlap(n_subs))))) {      // B200_CHUNKS=0 / 1: never / always (tests, diagnostics)
-      // two bands by default: every K1 launch costs one tile's wavefront latency (~5 ms for 1024x1024), so more bands lose
-      // more than their finer D2H overlap gains
-      int target = (n + 1) / 2; if (const char* e = getenv("B200_CHUNK_TILES")) { const int v = atoi(e); if (v > 0) target = v; }
-      rpc = std::max(1, (target + cols / 2) / cols);
-      nch = (rows + rpc - 1) / rpc;
-      if (nch > MAX_CHUNKS) { rpc = (rows + MAX_CHUNKS - 1) / MAX_CHUNKS; nch = (rows + rpc - 1) / rpc; }
-    }
-    d->nchunks = nch; d->grid_cols = cols;
-    for (int c = 0; c <= nch; c++) d->chunk_pic[c] = std::min(n, c * rpc * cols);
-    d->chunk_pic[nch] = n; }
-  { size_t row_cursor = 0; d->max_log2_ctb = 4;
-    for (int i = 0; i < n; i++) d->max_log2_ctb = std::max(d->max_log2_ctb, d->parsed[(size_t)i].desc.log2_ctb);
-    for (int c = 0; c < d->nchunks; c++) {
-      d->chunk_item[c] = row_cursor;
-      int max_h = 0;
-      for (int i = d->chunk_pic[c]; i < d->chunk_pic[c + 1]; i++) max_h = std::max(max_h, d->parsed[(size_t)i].desc.hctb);
-      for (int r = 0; r < max_h; r++) for (int i = d->chunk_pic[c]; i < d->chunk_pic[c + 1]; i++) if (r < d->parsed[(size_t)i].desc.hctb) {
-        d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r);                                        // luma
-        if (chroma == 1) d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r | (1u << 30));           // Cb + Cr of a 4:2:0 picture on the two half-warps
-        else if (chroma >= 2) { d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r | (2u << 30)); d->rows.h[row_cursor++] = make_uint2((unsigned)i, (unsigned)r | (3u << 30)); }   // Cb, Cr planes (4:2:2 / 4:4:4)
-      }
-    }
-    d->chunk_item[d->nchunks] = row_cursor;
-    d->n_items = row_cursor; d->info_bps = bps; }
-  d->pool->parallel_for(n, [&](int i) {
-    const ParsedPicture& pp = d->parsed[(size_t)i]; const PicDesc& p = pp.desc;
-    if (!devfe) {
-      memcpy(d->ctus.h + p.ctu_base, pp.ctus.data(), (size_t)p.wctb * p.hctb * sizeof(CtuInfo));
-      memcpy(d->tus.h + p.tu_base, pp.tus.data(), pp.n_tus * sizeof(TuCmd));
-      memcpy(d->coefs.h + p.coef_base, pp.coefs.data(), pp.n_coefs * sizeof(CoefEntry));
-      memcpy(d->slices.h + p.slice_base, pp.slices.data(), pp.slices.size() * sizeof(SliceInfo));
-      memcpy(d->qp8.h + p.map8_base, pp.qp8.data(), (size_t)p.w8 * p.h8);
-      memcpy(d->edge8.h + p.map8_base, pp.edge8.data(), (size_t)p.w8 * p.h8);
-    } else {
-      const PictureHeaders& H = pp.hdr;
-      memcpy(d->slices.h + p.slice_base, H.slices.data(), H.slices.size() * sizeof(SliceInfo));
-      memcpy(d->rbsp.h + rbsp_off[(size_t)i], H.rbsp.data(), H.rbsp.size());
-      memcpy(d->ctu_slice.h + p.ctu_base, H.ctu_slice.data(), H.ctu_slice.size() * sizeof(uint16_t));
-      // Ready-queue links (batch-wide indices): which sub-stream each one releases, and how many events each waits for before
-      // its first bin -- the conditions of run_substream (b200_hevc_syntax.h): the contexts stored after the 2nd CTB of the
-      // row above (WPP, 9.3.2.2) and the end state of the slice segment it continues.
-      const size_t so = sub_off[(size_t)i];
-      for (size_t k = 0; k < H.subs.size(); k++) { syn::Substream ss = H.subs[k]; ss.pic = (uint32_t)i; ss.wake_ctb2 = ss.wake_end = -1; ss.deps = 0; d->subs.h[so + k] = ss; }
-      for (size_t k = 0; k < H.subs.size(); k++) {
-        syn::Substream& ss = d->subs.h[so + k];
-        if (ss.prev >= 0) { ss.deps++; d->subs.h[so + (size_t)ss.prev].wake_end = (int32_t)(so + k); }
-        const int wctb = H.desc.wctb, rx0 = (int)(ss.ctb_begin % (uint32_t)wctb), ry0 = (int)(ss.ctb_begin / (uint32_t)wctb);
-        if (H.sp.wpp && rx0 == 0 && (!ss.init_contexts || ss.prev >= 0) && ss.ctb_begin != ss.slice_addr_rs && ry0 > 0 && (1 << H.desc.log2_ctb) < H.desc.width &&
-            H.ctu_slice[(size_t)(ry0 - 1) * wctb + 1] == (uint16_t)ss.slice_idx) {
-          const uint32_t a = (uint32_t)(ry0 - 1) * (uint32_t)wctb + 1;
-          for (size_t j = 0; j < H.subs.size(); j++) if (H.subs[j].ctb_begin <= a && a < H.subs[j].ctb_end) { ss.deps++; d->subs.h[so + j].wake_ctb2 = (int32_t)(so + k); break; }
-        }
-      }
-      EntropyPic ep{};
-      ep.sp = H.sp; ep.sp.dense = 0;
-      ep.pb.rbsp = d->rbsp.d + rbsp_off[(size_t)i]; ep.pb.rbsp_size = (uint32_t)H.rbsp.size();
-      ep.pb.tus = d->tus.d + p.tu_base; ep.pb.coefs = d->coefs.d + p.coef_base; ep.pb.ctus = d->ctus.d + p.ctu_base; ep.pb.slices = d->slices.d + p.slice_base;
-      ep.pb.ctu_slice = d->ctu_slice.d + p.ctu_base; ep.pb.qp8 = d->qp8.d + p.map8_base; ep.pb.edge8 = d->edge8.d + p.map8_base;
-      ep.pb.ipm4 = d->ipm4.d + map4_off[(size_t)i]; ep.pb.cd8 = d->cd8.d + p.map8_base;
-      ep.pb.wpp_ctx = d->wpp_ctx.d + (size_t)p.progress_base * syn::CTX_STRIDE; ep.pb.end_state = d->end_state.d + sub_off[(size_t)i] * syn::CTX_STRIDE;
-      ep.progress_base = p.progress_base; ep.sub_base = (uint32_t)sub_off[(size_t)i];
-      d->epics.h[i] = ep;
-    }
-  });
-  if (devfe) {
-    // ready queue image: cursors, the sub-streams without prerequisites in "k-th sub-stream of every picture" order (so
-    // that whatever a popped sub-stream polls for was popped before it), empty slots, the dependency counters
-    unsigned* q = d->equeue.h; size_t cur = 0, maxs = 0;
-    for (int i = 0; i < n; i++) maxs = std::max(maxs, d->parsed[(size_t)i].hdr.subs.size());
-    for (size_t k = 0; k < maxs; k++) for (int i = 0; i < n; i++) if (k < d->parsed[(size_t)i].hdr.subs.size() && d->subs.h[sub_off[(size_t)i] + k].deps == 0) q[2 + cur++] = (unsigned)(sub_off[(size_t)i] + k) + 1u;
-    q[0] = 0; q[1] = (unsigned)cur;
-    for (size_t k = cur; k < n_subs; k++) q[2 + k] = 0;
-    for (size_t k = 0; k < n_subs; k++) q[2 + n_subs + k] = d->subs.h[k].deps;
-  }
-  const double t2 = now_ms();
-  // ---- 4. H2D + kernels
-  cudaEventRecord(d->ev[0], s);
-  B200_CUDA_CHECK(cudaMemcpyAsync(d->pics.d, d->pics.h, (size_t)n * sizeof(PicDesc), cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(d->slices.d, d->slices.h, n_slice * sizeof(SliceInfo), cudaMemcpyHostToDevice, s));
-  B200_CUDA_CHECK(cudaMemcpyAsync(d->rows.d, d->rows.h, d->n_items * sizeof(uint2), cudaMemcpyHostToDevice, s));
-  if (n_scaling) B200_CUDA_CHECK(cudaMemcpyAsync(d->scaling.d, d->scaling.h, (size_t)n_scaling * 784, cudaMemcpyHostToDevice, s));
-  size_t h2d = (size_t)n_scaling * 784 + (size_t)n * sizeof(PicDesc) + n_slice * sizeof(SliceInfo) + d->n_items * sizeof(uint2);
-  if (!devfe) {
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->ctus.d, d->ctus.h, n_ctu * sizeof(CtuInfo), cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->tus.d, d->tus.h, n_tu * sizeof(TuCmd), cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->coefs.d, d->coefs.h, n_coef * sizeof(CoefEntry), cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->qp8.d, d->qp8.h, n_map, cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->edge8.d, d->edge8.h, n_map, cudaMemcpyHostToDevice, s));
-    h2d += n_ctu * sizeof(CtuInfo) + n_tu * sizeof(TuCmd) + n_coef * sizeof(CoefEntry) + 2 * n_map;
-  } else {
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->rbsp.d, d->rbsp.h, n_rbsp, cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->subs.d, d->subs.h, n_subs * sizeof(syn::Substream), cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->equeue.d, d->equeue.h, (2 + 2 * n_subs) * sizeof(unsigned), cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->ctu_slice.d, d->ctu_slice.h, n_ctu * sizeof(uint16_t), cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->epics.d, d->epics.h, (size_t)n * sizeof(EntropyPic), cudaMemcpyHostToDevice, s));
-    B200_CUDA_CHECK(cudaMemsetAsync(d->esync.d, 0, (1 + n_rows + n_subs) * sizeof(unsigned), s));
-    B200_CUDA_CHECK(cudaMemsetAsync(d->ecount.d, 0, 2 * sizeof(unsigned long long), s));
-    h2d += n_rbsp + n_subs * (sizeof(syn::Substream) + 2 * sizeof(unsigned)) + n_ctu * sizeof(uint16_t) + (size_t)n * sizeof(EntropyPic);
-  }
-  B200_CUDA_CHECK(cudaMemsetAsync(d->sync.d, 0, (3 * n_rows + 2 + MAX_CHUNKS) * sizeof(unsigned), s));
-  if (!canvas_fully_covered) B200_CUDA_CHECK(cudaMemsetAsync(d->canvas.d, 0, cbytes, s));     // uncovered canvas stays zero (calloc in the reference)
-  d->n_rows = n_rows; d->cbytes = cbytes; d->canvas_fully_covered = canvas_fully_covered; d->npics = n; d->n_subs = n_subs; d->used_device_front_end = devfe;
-  b200_image_info& inf = d->info;
-  inf.width = cw; inf.height = chh; inf.tile_width = tw; inf.tile_height = th; inf.chroma = chroma;        /* B200_CHROMA_MONO / 420 / 422 / 444 = chroma_format_idc */ inf.bit_depth = bd;
-  inf.colour_primaries = d->parsed[0].hdr.colour_primaries; inf.transfer_characteristics = d->parsed[0].hdr.transfer_characteristics;
-  inf.matrix_coefficients = d->parsed[0].hdr.matrix_coefficients; inf.full_range = d->parsed[0].hdr.full_range;
-  if (info) *info = inf;
-  int launches = 0;
-  if ((rc = run_device_pipeline(d, n, s, &launches))) return rc;
-  d->last_stream = s; d->have_result = true;
-  b200_decode_stats& st = d->stats;
-  memset(&st, 0, sizeof st);
-  st.parse_ms = t1 - t0; st.pack_ms = t2 - t1; st.total_ms = now_ms() - t0;
-  st.bitstream_bytes = bits; st.ctus = n_ctu;
-  if (!devfe) {
-    st.coefficient_entries = n_coef; st.transform_units = n_tu;
-    st.command_bytes = n_ctu * sizeof(CtuInfo) + n_tu * sizeof(TuCmd) + n_coef * sizeof(CoefEntry) + n_slice * sizeof(SliceInfo) + 2 * n_map + (size_t)n * sizeof(PicDesc);
-  }
-  st.h2d_bytes = h2d;
-  st.pixels = (uint64_t)cw * chh; st.kernel_launches = launches;
-  return B200_OK;
+  return decode_grid(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, info, (cudaStream_t)stream_, Overrides::read());
 }
 
 // Re-run only the device kernels on the already uploaded command stream ("inputs resident in HBM" timing leg).
 int b200_decoder_rerun_device(b200_decoder* d, void* stream_) {
   if (!d || !d->have_result) return set_error(B200_E_INVALID, "no decode result");
   cudaStream_t s = (cudaStream_t)stream_;
-  B200_CUDA_CHECK(cudaMemsetAsync(d->sync.d, 0, (3 * d->n_rows + 2 + MAX_CHUNKS) * sizeof(unsigned), s));
-  if (d->used_device_front_end) {
-    B200_CUDA_CHECK(cudaMemsetAsync(d->esync.d, 0, (1 + d->n_rows + d->n_subs) * sizeof(unsigned), s));
-    B200_CUDA_CHECK(cudaMemsetAsync(d->ecount.d, 0, 2 * sizeof(unsigned long long), s));
-    B200_CUDA_CHECK(cudaMemcpyAsync(d->equeue.d, d->equeue.h, (2 + 2 * d->n_subs) * sizeof(unsigned), cudaMemcpyHostToDevice, s));
-  }
+  const LaunchPlan plan = plan_launches(d->shape, false, Overrides::read());
+  int rc;
+  if ((rc = reset_scratch(d, d->scratch, d->shape.device_front_end, s))) return rc;
+  if (d->shape.device_front_end)
+    B200_CUDA_CHECK(cudaMemcpyAsync(d->equeue.d, d->equeue.h, d->scratch.equeue_size() * sizeof(unsigned), cudaMemcpyHostToDevice, s));
   int launches = 0;
-  int rc = run_device_pipeline(d, d->npics, s, &launches);
+  rc = run_device_pipeline(d, plan, s, &launches);
   d->last_stream = s;
   return rc;
 }
 
 int b200_decoder_get_stats(b200_decoder* d, b200_decode_stats* out) {
   if (!d || !out || !d->have_result) return set_error(B200_E_INVALID, "no decode result");
-  B200_CUDA_CHECK(cudaEventSynchronize(d->ev[4]));
+  B200_CUDA_CHECK(cudaEventSynchronize(d->t_sao));
   float a = 0, en = 0, b = 0, c = 0, e = 0;
-  cudaEventElapsedTime(&a, d->ev[0], d->ev[1]); cudaEventElapsedTime(&en, d->ev[1], d->ev[5]); cudaEventElapsedTime(&b, d->ev[5], d->ev[2]);
-  cudaEventElapsedTime(&c, d->ev[2], d->ev[3]); cudaEventElapsedTime(&e, d->ev[3], d->ev[4]);
+  cudaEventElapsedTime(&a, d->t_start, d->t_h2d); cudaEventElapsedTime(&en, d->t_h2d, d->t_entropy); cudaEventElapsedTime(&b, d->t_entropy, d->t_recon);
+  cudaEventElapsedTime(&c, d->t_recon, d->t_deblock); cudaEventElapsedTime(&e, d->t_deblock, d->t_sao);
   if (b < 0) { en += b; b = 0; }   // K0 and K1 overlap: recon_ms is the part of K1 that runs after K0 has finished
   d->stats.h2d_ms = a; d->stats.entropy_ms = en; d->stats.recon_ms = b; d->stats.deblock_ms = c; d->stats.sao_ms = e; d->stats.gpu_ms = en + b + c + e;
-  d->stats.front_end = d->used_device_front_end ? (d->last_chunked ? 3 : (d->last_overlapped ? 2 : 1)) : 0;
-  d->stats.bands = d->last_chunked ? d->nchunks : 1;
-  if (d->used_device_front_end) {
+  const bool devfe = d->shape.device_front_end;
+  d->stats.front_end = devfe ? (d->last_banded ? 3 : (d->last_overlapped ? 2 : 1)) : 0;
+  d->stats.bands = d->last_banded ? d->shape.bands : 1;
+  if (devfe) {
     B200_CUDA_CHECK(cudaMemcpy(d->ecount.h, d->ecount.d, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     d->stats.transform_units = d->ecount.h[0]; d->stats.coefficient_entries = d->ecount.h[1];
     d->stats.command_bytes = d->stats.ctus * sizeof(CtuInfo) + d->ecount.h[0] * sizeof(TuCmd) + d->ecount.h[1] * sizeof(CoefEntry) + 2 * (d->stats.pixels / 64);
@@ -594,20 +723,25 @@ int b200_decoder_debug_read_tile(b200_decoder* d, int index, int stage, void* y,
   return B200_OK;
 }
 
-// Common part of the fused entry points: decode -> colour conversion into one of the two device RGB buffers.
+}  // extern "C"
+
+struct DeviceRgb {                  // where decode_to_rgb_device left the RGB of a call
+  size_t rowb = 0, pitch = 0;       // bytes per output row, pitch of the device RGB buffer
+  int height = 0;                   // output rows
+  bool bands_copied = false;        // the bands already left for the destination through the copy stream
+};
+
+// Common part of the fused entry points: decode -> colour conversion into one of the two device RGB buffers.  `direct_out`:
+// the page-locked destination the bands may be copied into as they are finished (nullptr: none).  The synchronous entry point
+// takes bands whenever the plan gives them; the asynchronous one, whose D2H already overlaps the next call's kernels, only
+// when B200_CHUNKS asks for them.
 static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size, uint64_t max_pixels, int canvas_w,
-                                int canvas_h, const b200_geometry* geom, const b200_color_options* opt, b200_image_info* info, int slot, size_t* rowb_out,
-                                size_t* pitch_out, int* out_h, void* direct_out, size_t direct_stride, bool* bands_copied, bool allow_bands) {
-  if (!d->own) {
-    B200_CUDA_CHECK(cudaStreamCreateWithFlags(&d->own, cudaStreamNonBlocking));
-    B200_CUDA_CHECK(cudaStreamCreateWithFlags(&d->copy, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) { B200_CUDA_CHECK(cudaEventCreateWithFlags(&d->ev_k6[i], cudaEventDisableTiming)); B200_CUDA_CHECK(cudaEventCreateWithFlags(&d->ev_d2h[i], cudaEventDisableTiming)); }
-    B200_CUDA_CHECK(cudaHostAlloc((void**)&d->err_host, 2 * sizeof(unsigned), cudaHostAllocDefault));
-    d->err_host[0] = d->err_host[1] = 0;
-  }
+                                int canvas_h, const b200_geometry* geom, const b200_color_options* opt, b200_image_info* info, int slot,
+                                void* direct_out, size_t direct_stride, bool async, DeviceRgb* res) {
+  const Overrides env = Overrides::read();
   cudaStream_t s = d->own;
   // the page-locked staging of the previous call must have left for the device before the host overwrites it
-  B200_CUDA_CHECK(cudaEventSynchronize(d->ev[1]));
+  B200_CUDA_CHECK(cudaEventSynchronize(d->t_h2d));
   b200_image_info inf;
   size_t bpp;
   switch (opt->out_chroma) {
@@ -621,12 +755,11 @@ static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8
   // whole-picture one for the reference's default planner choice (nearest-neighbour chroma, per-sample arithmetic) without
   // rotate / mirror / crop; every other request converts the finished canvas in one go, below.
   bool banded = false; int hook_rc = B200_OK;
-  *bands_copied = false;
-  if (!geom && opt->chroma_upsampling == 0 && direct_out && allow_bands) {
-    d->chunk_hook = [&, slot, bpp](int c, cudaStream_t side) -> int {
+  if (!geom && opt->chroma_upsampling == 0 && direct_out && (!async || env.bands == Overrides::ON)) {
+    d->band_hook = [&, slot, bpp](int c, cudaStream_t side) -> int {
       const b200_image_info& I = d->info;
-      const int th = I.tile_height, y0 = std::min(I.height, (d->chunk_pic[c] / d->grid_cols) * th);
-      const int y1 = c + 1 == d->nchunks ? I.height : std::min(I.height, (d->chunk_pic[c + 1] / d->grid_cols) * th);
+      const int th = I.tile_height, y0 = std::min(I.height, (d->band_pic[c] / d->shape.cols) * th);
+      const int y1 = c + 1 == d->shape.bands ? I.height : std::min(I.height, (d->band_pic[c + 1] / d->shape.cols) * th);
       const size_t rowb = (size_t)I.width * bpp, pitch = (rowb + 255) & ~(size_t)255;
       int rc2;
       if (c == 0) {
@@ -635,7 +768,6 @@ static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8
         banded = true;
       }
       if (y1 <= y0) return B200_OK;
-      const int bps = I.bit_depth > 8 ? 2 : 1; (void)bps;
       b200_planes pl; memset(&pl, 0, sizeof pl);
       pl.y = d->canvas.d + d->canvas_off[0] + (size_t)y0 * d->canvas_pitch[0]; pl.y_stride = d->canvas_pitch[0];
       if (I.chroma != B200_CHROMA_MONO) {
@@ -648,21 +780,18 @@ static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8
       b200_geometry g; b200_geometry_identity(pl.width, pl.height, &g);
       uint8_t* dst = d->rgb2[slot].d + (size_t)y0 * pitch;
       if ((rc2 = b200_color_convert_device(&pl, &g, opt, dst, nullptr, nullptr, pitch, side, nullptr))) return hook_rc = rc2;
-      if (direct_out) {
-        if (!d->ev_chunk[c]) B200_CUDA_CHECK(cudaEventCreateWithFlags(&d->ev_chunk[c], cudaEventDisableTiming));
-        B200_CUDA_CHECK(cudaEventRecord(d->ev_chunk[c], side));
-        B200_CUDA_CHECK(cudaStreamWaitEvent(d->copy, d->ev_chunk[c], 0));
-        B200_CUDA_CHECK(cudaMemcpy2DAsync(static_cast<uint8_t*>(direct_out) + (size_t)y0 * direct_stride, direct_stride, dst, pitch, rowb, (size_t)(y1 - y0), cudaMemcpyDeviceToHost, d->copy));
-      }
+      B200_CUDA_CHECK(cudaEventRecord(d->ev_band[c], side));
+      B200_CUDA_CHECK(cudaStreamWaitEvent(d->copy, d->ev_band[c], 0));
+      B200_CUDA_CHECK(cudaMemcpy2DAsync(static_cast<uint8_t*>(direct_out) + (size_t)y0 * direct_stride, direct_stride, dst, pitch, rowb, (size_t)(y1 - y0), cudaMemcpyDeviceToHost, d->copy));
       return B200_OK;
     };
   }
-  int rc = b200_decoder_decode_grid(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, &inf, s);
-  d->chunk_hook = nullptr;
+  int rc = decode_grid(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, &inf, s, env);
+  d->band_hook = nullptr;
   if (rc) return rc;
   if (hook_rc) return hook_rc;
   if (info) *info = inf;
-  B200_CUDA_CHECK(cudaMemcpyAsync(&d->err_host[slot], d->sync.d + 1, sizeof(unsigned), cudaMemcpyDeviceToHost, s));   // this step's error flag (the next step clears the device copy)
+  B200_CUDA_CHECK(cudaMemcpyAsync(&d->err_host.h[slot], d->sync.d + ScratchLayout::error_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, s));   // this step's error flag (the next step clears the device copy)
   b200_planes pl; if ((rc = b200_decoder_get_planes(d, &pl))) return rc;
   b200_geometry g; if (geom) g = *geom; else b200_geometry_identity(inf.width, inf.height, &g);
   const size_t rowb = (size_t)g.out_w * bpp, pitch = (rowb + 255) & ~(size_t)255;
@@ -672,8 +801,7 @@ static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8
     if ((rc = b200_color_convert_device(&pl, &g, opt, d->rgb2[slot].d, nullptr, nullptr, pitch, s, nullptr))) return rc;
   }
   B200_CUDA_CHECK(cudaEventRecord(d->ev_k6[slot], s));
-  *bands_copied = banded && direct_out != nullptr;
-  *rowb_out = rowb; *pitch_out = pitch; *out_h = g.out_h;
+  res->rowb = rowb; res->pitch = pitch; res->height = g.out_h; res->bands_copied = banded;
   return B200_OK;
 }
 
@@ -684,42 +812,44 @@ static bool is_page_locked(const void* p) {
   return pinned;
 }
 
+extern "C" {
+
 int b200_decode_grid_to_rgb_host(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
                                  uint64_t max_pixels, int canvas_w, int canvas_h, const b200_geometry* geom,
                                  const b200_color_options* opt, void* out, size_t out_stride, b200_image_info* info) {
   if (!d || !opt || !out) return set_error(B200_E_INVALID, "null argument");
-  size_t rowb = 0, pitch = 0; int oh = 0; bool copied = false;
   const bool pinned = is_page_locked(out);
-  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, info, 0, &rowb, &pitch, &oh, pinned ? out : nullptr, out_stride, &copied, true);
+  DeviceRgb r;
+  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, info, 0, pinned ? out : nullptr, out_stride, false, &r);
   if (rc) return rc;
   cudaStream_t s = d->own;
   uint8_t* rgb = d->rgb2[0].d;
+  const size_t rowb = r.rowb, pitch = r.pitch;
   // D2H: straight into the caller's buffer when it is page-locked (b200_host_alloc, cudaHostAlloc, cudaHostRegister);
   // pageable memory goes through a page-locked bounce buffer in row bands, the copy of band i overlapping the memcpy of
   // band i - 1 on the decoder's host threads
-  if (copied) {                                         // the bands left through the copy stream as they were finished
+  if (r.bands_copied) {                                 // the bands left through the copy stream as they were finished
     B200_CUDA_CHECK(cudaEventRecord(d->ev_d2h[0], d->copy));
     B200_CUDA_CHECK(cudaStreamSynchronize(s));
     B200_CUDA_CHECK(cudaStreamSynchronize(d->copy));
   } else if (pinned) {
-    B200_CUDA_CHECK(cudaMemcpy2DAsync(out, out_stride, rgb, pitch, rowb, (size_t)oh, cudaMemcpyDeviceToHost, s));
+    B200_CUDA_CHECK(cudaMemcpy2DAsync(out, out_stride, rgb, pitch, rowb, (size_t)r.height, cudaMemcpyDeviceToHost, s));
     B200_CUDA_CHECK(cudaEventRecord(d->ev_d2h[0], s));
     B200_CUDA_CHECK(cudaStreamSynchronize(s));
   } else {
-    const size_t band_rows = std::max<size_t>(1, (size_t)(32u << 20) / rowb);
-    const int nb = (int)(((size_t)oh + band_rows - 1) / band_rows);
+    const size_t oh = (size_t)r.height, band_rows = std::max<size_t>(1, (size_t)(32u << 20) / rowb);
+    const int nb = (int)((oh + band_rows - 1) / band_rows);
     if ((rc = d->bounce.reserve(2 * band_rows * rowb, true))) return rc;
-    for (auto& e : d->ev_band) if (!e) B200_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     for (int k = 0; k <= nb; k++) {
       if (k < nb) {
-        const size_t y0 = (size_t)k * band_rows, h = std::min(band_rows, (size_t)oh - y0);
+        const size_t y0 = (size_t)k * band_rows, h = std::min(band_rows, oh - y0);
         B200_CUDA_CHECK(cudaMemcpy2DAsync(d->bounce.h + (size_t)(k & 1) * band_rows * rowb, rowb, rgb + y0 * pitch, pitch, rowb, h, cudaMemcpyDeviceToHost, s));
-        B200_CUDA_CHECK(cudaEventRecord(d->ev_band[k & 1], s));
+        B200_CUDA_CHECK(cudaEventRecord(d->ev_bounce[k & 1], s));
       }
       if (k > 0) {
         const int j = k - 1;
-        const size_t y0 = (size_t)j * band_rows, h = std::min(band_rows, (size_t)oh - y0);
-        B200_CUDA_CHECK(cudaEventSynchronize(d->ev_band[j & 1]));
+        const size_t y0 = (size_t)j * band_rows, h = std::min(band_rows, oh - y0);
+        B200_CUDA_CHECK(cudaEventSynchronize(d->ev_bounce[j & 1]));
         const uint8_t* src = d->bounce.h + (size_t)(j & 1) * band_rows * rowb;
         const int parts = 8;
         d->pool->parallel_for(parts, [&](int t) {
@@ -731,7 +861,7 @@ int b200_decode_grid_to_rgb_host(b200_decoder* d, int cols, int rows, const uint
     B200_CUDA_CHECK(cudaEventRecord(d->ev_d2h[0], s));
     B200_CUDA_CHECK(cudaStreamSynchronize(s));
   }
-  if (d->err_host[0]) return set_error(B200_E_CUDA, "a decoding kernel gave up waiting for a dependency or met corrupt slice data");
+  if (d->err_host.h[0]) return set_error(B200_E_CUDA, "a decoding kernel gave up waiting for a dependency or met corrupt slice data");
   return B200_OK;
 }
 
@@ -745,13 +875,13 @@ int b200_decode_grid_to_rgb_host_async(b200_decoder* d, int cols, int rows, cons
   if (!d || !opt || !out) return set_error(B200_E_INVALID, "null argument");
   if (!is_page_locked(out)) return set_error(B200_E_INVALID, "the asynchronous entry point needs a page-locked output buffer (b200_host_alloc / b200_host_register)");
   const int slot = d->async_slot; d->async_slot ^= 1;
-  if (d->err_host && d->err_host[slot]) d->async_error = true;                 // the step that used this slot two calls ago failed
-  size_t rowb = 0, pitch = 0; int oh = 0; bool copied = false;
-  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, info, slot, &rowb, &pitch, &oh, out, out_stride, &copied, getenv("B200_CHUNKS") && atoi(getenv("B200_CHUNKS")) != 0);
+  if (d->err_host.h[slot]) d->async_error = true;                 // the step that used this slot two calls ago failed
+  DeviceRgb r;
+  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, info, slot, out, out_stride, true, &r);
   if (rc) return rc;
-  if (!copied) {
+  if (!r.bands_copied) {
     B200_CUDA_CHECK(cudaStreamWaitEvent(d->copy, d->ev_k6[slot], 0));
-    B200_CUDA_CHECK(cudaMemcpy2DAsync(out, out_stride, d->rgb2[slot].d, pitch, rowb, (size_t)oh, cudaMemcpyDeviceToHost, d->copy));
+    B200_CUDA_CHECK(cudaMemcpy2DAsync(out, out_stride, d->rgb2[slot].d, r.pitch, r.rowb, (size_t)r.height, cudaMemcpyDeviceToHost, d->copy));
   }
   B200_CUDA_CHECK(cudaEventRecord(d->ev_d2h[slot], d->copy));
   return B200_OK;
@@ -759,10 +889,9 @@ int b200_decode_grid_to_rgb_host_async(b200_decoder* d, int cols, int rows, cons
 
 int b200_decoder_wait(b200_decoder* d) {
   if (!d) return set_error(B200_E_INVALID, "null argument");
-  if (!d->own) return B200_OK;
   B200_CUDA_CHECK(cudaStreamSynchronize(d->own));
   B200_CUDA_CHECK(cudaStreamSynchronize(d->copy));
-  const bool bad = d->async_error || d->err_host[0] || d->err_host[1];
+  const bool bad = d->async_error || d->err_host.h[0] || d->err_host.h[1];
   d->async_error = false;
   if (bad) return set_error(B200_E_CUDA, "a decoding kernel gave up waiting for a dependency or met corrupt slice data");
   return B200_OK;

@@ -181,7 +181,6 @@ int launch_entropy(const EntropyBatch& b, cudaStream_t s, int* resident_warps) {
   int occ = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, EWARPS * 32, 0);
   if (occ < 1) occ = 1;
   if (b.blocks_per_sm > 0 && b.blocks_per_sm < occ) occ = b.blocks_per_sm;
-  if (const char* e = getenv("B200_ENTROPY_BLOCKS_PER_SM")) { const int v = atoi(e); if (v >= 1 && v < occ) occ = v; }   // tuning knob
   const int want = (b.nsubs + EWARPS - 1) / EWARPS;
   const int grid = want < sms * occ ? want : sms * occ;
   if (resident_warps) *resident_warps = grid * EWARPS;

@@ -154,124 +154,14 @@ __device__ __noinline__ int sao_sample_generic(const DeviceBatch& b, const PicDe
   return clip3d(0, maxv, v + off);
 }
 
-// One thread = 8 horizontally adjacent samples of one row of one component (always inside one CTB: a chroma CTB is at
-// least 8 samples wide); block = 64 segments x 4 rows; grid.z = picture * 3 + component.  The CTB's SAO parameters are
-// fetched once per thread, the three source rows with 8- / 16-byte loads, the result leaves with one vector store.
-template <typename T>
-__global__ void __launch_bounds__(256) sao_kernel(const DeviceBatch b) {
-  const int pi = blockIdx.z / 3, c = blockIdx.z % 3;
-  const PicDesc& pic = b.pics[pi];
-  if (c > 0 && !pic.chroma) return;
-  const int sh = (c && (pic.chroma == 1 || pic.chroma == 2)) ? 1 : 0, shy = (c && pic.chroma == 1) ? 1 : 0;     // horizontal / vertical sub-sampling of the component
-  const int w = pic.width >> sh, h = pic.height >> shy;
-  const int x0 = (blockIdx.x * 64 + threadIdx.x) * 8, y = blockIdx.y * 4 + threadIdx.y;
-  if (x0 >= w || y >= h) return;
-  const int cx = pic.crop_x >> sh, cy = pic.crop_y >> shy, ow = (pic.out_w + sh) >> sh, oh = (pic.out_h + shy) >> shy;
-  const int oy = y - cy;
-  if (oy < 0 || oy >= oh) return;                                     // outside the conformance window: never output
-  const T* src = static_cast<const T*>(pic.rec[c]);
-  const int st = pic.rec_stride[c];
-  const int lg = pic.log2_ctb - sh, lgy = pic.log2_ctb - shy;
-  const CtuInfo* ctus = b.ctus + pic.ctu_base;
-  const int n = min(8, w - x0);
-  int res[8];
-  if (pic.nslices > 1) {
-#pragma unroll
-    for (int k = 0; k < 8; k++) res[k] = k < n ? sao_sample_generic<T>(b, pic, ctus, src, st, c, x0 + k, y, w, h, lg, lgy) : 0;
-  } else {
-    // centre row: samples x0-1 .. x0+8 in cur[0..9]
-    int cur[10], up[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, dn[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-    const T* row = src + (size_t)y * st + x0;
-    auto load8 = [&](const T* p, int* d) {                            // 8 samples, vector load (rows and x0 are 8-sample aligned)
-      if (sizeof(T) == 1) { const uint2 q = *reinterpret_cast<const uint2*>(p); for (int k = 0; k < 4; k++) { d[k] = (q.x >> (8 * k)) & 0xff; d[4 + k] = (q.y >> (8 * k)) & 0xff; } }
-      else { const uint4 q = *reinterpret_cast<const uint4*>(p); const unsigned u[4] = {q.x, q.y, q.z, q.w}; for (int k = 0; k < 4; k++) { d[2 * k] = u[k] & 0xffff; d[2 * k + 1] = u[k] >> 16; } }
-    };
-    if (n == 8) load8(row, cur + 1);
-    else {
-#pragma unroll
-      for (int k = 0; k < 8; k++) cur[1 + k] = k < n ? (int)row[k] : 0;
-    }
-    const SaoComp sp = ctus[(y >> lgy) * pic.wctb + (x0 >> lg)].sao[c];
-    const int bd = pic.bit_depth, maxv = (1 << bd) - 1;
-    const unsigned offs = (unsigned)(uint8_t)sp.offset[0] | ((unsigned)(uint8_t)sp.offset[1] << 8) | ((unsigned)(uint8_t)sp.offset[2] << 16) | ((unsigned)(uint8_t)sp.offset[3] << 24);
-    auto offset = [&](int i) { return (int)(int8_t)(offs >> (8 * i)); };     // register-resident SaoOffsetVal[1..4]
-    const bool on = pic.sao_enabled && sp.type;
-    if (!on) { for (int k = 0; k < 8; k++) res[k] = cur[1 + k]; }
-    else if (sp.type == 1) {
-#pragma unroll
-      for (int k = 0; k < 8; k++) {
-        const int v = cur[1 + k], kk = ((v >> (bd - 5)) - sp.band_or_class) & 31;
-        res[k] = clip3d(0, maxv, v + (kk < 4 ? offset(kk) : 0));
-      }
-    } else {
-      const int e = sp.band_or_class;
-      const int hx = e == 1 ? 0 : (e == 3 ? 1 : -1);
-      const bool vert = e != 0;                                        // neighbours in the rows above / below
-      const bool has_l = x0 > 0, has_r = x0 + 8 < w;
-      cur[0] = has_l ? (int)row[-1] : 0; cur[9] = has_r ? (int)row[8] : 0;
-      const bool rows_ok = !vert || (y > 0 && y + 1 < h);
-      if (vert && rows_ok) {
-        const T* ru = row - st; const T* rd = row + st;
-        if (n == 8) { load8(ru, up + 1); load8(rd, dn + 1); }
-        else {
-#pragma unroll
-          for (int k = 0; k < 8; k++) { up[1 + k] = k < n ? (int)ru[k] : 0; dn[1 + k] = k < n ? (int)rd[k] : 0; }
-        }
-        up[0] = has_l ? (int)ru[-1] : 0; up[9] = has_r ? (int)ru[8] : 0;
-        dn[0] = has_l ? (int)rd[-1] : 0; dn[9] = has_r ? (int)rd[8] : 0;
-      }
-#pragma unroll
-      for (int k = 0; k < 8; k++) {
-        const int v = cur[1 + k];
-        int off = 0;
-        const int xa = x0 + k + hx, xb = x0 + k - hx;
-        if (rows_ok && xa >= 0 && xb >= 0 && xa < w && xb < w) {
-          // static indices only (hx is uniform per CTB): the arrays stay in registers
-          const int a_l = vert ? up[k] : cur[k], a_m = up[1 + k], a_r = vert ? up[2 + k] : cur[2 + k];
-          const int b_l = vert ? dn[k] : cur[k], b_m = dn[1 + k], b_r = vert ? dn[2 + k] : cur[2 + k];
-          const int a = hx < 0 ? a_l : (hx > 0 ? a_r : a_m), bb = hx < 0 ? b_r : (hx > 0 ? b_l : b_m);
-          const int ei = 2 + (v > a) - (v < a) + (v > bb) - (v < bb);
-          if (ei != 2) off = offset(ei < 2 ? ei : ei - 1);              // edgeIdx 0,1,3,4 -> SaoOffsetVal[1..4]
-        }
-        res[k] = clip3d(0, maxv, v + off);
-      }
-    }
-  }
-  {
-    // cu_transquant_bypass / pcm + pcm_loop_filter_disabled (8.7.3: SaoTypeIdx is treated as 0 there): bit 2 of the 8x8 luma cells
-    const uint8_t* cell = b.edge8 + pic.map8_base + ((y << shy) >> 3) * pic.w8 + ((x0 << sh) >> 3);
-    const bool k0 = cell[0] & 4, k1 = sh ? (((x0 + 4) << 1) < pic.width && (cell[1] & 4)) : k0;
-    if (k0 | k1) {
-      const T* row = src + (size_t)y * st + x0;
-#pragma unroll
-      for (int k = 0; k < 8; k++) if (k < n && (k < 4 ? k0 : k1)) res[k] = (int)row[k];
-    }
-  }
-  // store (conformance window applied; destination already offset to the tile's paste position)
-  T* drow = static_cast<T*>(pic.dst[c]) + (size_t)oy * pic.dst_stride[c];
-  const int ox0 = x0 - cx;
-  if (n == 8 && ox0 >= 0 && ox0 + 8 <= ow && ((reinterpret_cast<uintptr_t>(drow + ox0) & (8 * sizeof(T) - 1)) == 0)) {
-    if (sizeof(T) == 1) {
-      uint2 q; q.x = res[0] | (res[1] << 8) | (res[2] << 16) | (res[3] << 24); q.y = res[4] | (res[5] << 8) | (res[6] << 16) | (res[7] << 24);
-      *reinterpret_cast<uint2*>(drow + ox0) = q;
-    } else {
-      uint4 q; q.x = res[0] | (res[1] << 16); q.y = res[2] | (res[3] << 16); q.z = res[4] | (res[5] << 16); q.w = res[6] | (res[7] << 16);
-      *reinterpret_cast<uint4*>(drow + ox0) = q;
-    }
-  } else {
-#pragma unroll
-    for (int k = 0; k < 8; k++) { const int ox = ox0 + k; if (k < n && ox >= 0 && ox < ow) drow[ox] = (T)res[k]; }
-  }
-}
-
-// ---- K4, second form (default): one thread = 8 horizontally adjacent samples (one SAO unit: always inside one CTB) of FOUR
-// consecutive rows (a 4-aligned row group never straddles a CTB either).  All six source rows a thread needs (the row above
-// its group .. the row below) are requested up front with 8- / 16-byte loads -- six independent loads in flight per thread
-// instead of a dependent chain of three -- and the horizontal neighbours come from the adjacent lanes by shuffle (one warp =
-// 256 consecutive samples of a row; only lanes 0 and 31 load their outer neighbour).  The CTB's parameters, the
-// bypass / PCM cell and the picture descriptor are fetched once per 32 samples.
-// (The first form above walks one row per thread: its 393 K blocks of 2 KB were bound by block turnover and load latency; walking
-// four rows one after the other in a rolled loop was slower still.)
+// ---- K4: one thread = 8 horizontally adjacent samples (one SAO unit: always inside one CTB) of FOUR consecutive rows (a
+// 4-aligned row group never straddles a CTB either).  All six source rows a thread needs (the row above its group .. the row
+// below) are requested up front with 8- / 16-byte loads -- six independent loads in flight per thread instead of a dependent
+// chain of three -- and the horizontal neighbours come from the adjacent lanes by shuffle (one warp = 256 consecutive samples
+// of a row; only lanes 0 and 31 load their outer neighbour).  The CTB's parameters, the bypass / PCM cell and the picture
+// descriptor are fetched once per 32 samples.
+// (One row per thread was bound by block turnover and load latency, with 393 K blocks of 2 KB; walking four rows one after
+// the other in a rolled loop was slower still.)
 template <typename T> struct SaoPack;
 template <> struct SaoPack<uint8_t> {
   uint2 q;
@@ -546,21 +436,14 @@ int launch_sao(const DeviceBatch& b, const PicDesc* hp, cudaStream_t s, int* lau
   }
   if (launches) *launches = 0;
   if (!b.npics) return B200_OK;
-  static const bool first_form = getenv("B200_SAO_ROW_PER_THREAD") != nullptr;            // the first form of the kernel (one row per thread), kept for A / B measurements
-  if (first_form) {
-    const dim3 block(64, 4), grid((max_w / 8 + 63) / 64, (max_h + 3) / 4, b.npics * 3);
-    if (any16) sao_kernel<uint16_t><<<grid, block, 0, s>>>(b); else sao_kernel<uint8_t><<<grid, block, 0, s>>>(b);
-    if (launches) *launches = 1;
-  } else {
-    const dim3 block(32, 8);
-    const dim3 grid_y((max_w + 255) / 256, (max_h + 8 * SAO_ROWS - 1) / (8 * SAO_ROWS), b.npics);
-    if (any16) sao_rows_kernel<uint16_t><<<grid_y, block, 0, s>>>(b, 0, 1); else sao_rows_kernel<uint8_t><<<grid_y, block, 0, s>>>(b, 0, 1);
-    if (launches) *launches = 1;
-    if (max_cw > 0 && max_ch > 0) {
-      const dim3 grid_c((max_cw + 255) / 256, (max_ch + 8 * SAO_ROWS - 1) / (8 * SAO_ROWS), b.npics * 2);
-      if (any16) sao_rows_kernel<uint16_t><<<grid_c, block, 0, s>>>(b, 1, 2); else sao_rows_kernel<uint8_t><<<grid_c, block, 0, s>>>(b, 1, 2);
-      if (launches) *launches = 2;
-    }
+  const dim3 block(32, 8);
+  const dim3 grid_y((max_w + 255) / 256, (max_h + 8 * SAO_ROWS - 1) / (8 * SAO_ROWS), b.npics);
+  if (any16) sao_rows_kernel<uint16_t><<<grid_y, block, 0, s>>>(b, 0, 1); else sao_rows_kernel<uint8_t><<<grid_y, block, 0, s>>>(b, 0, 1);
+  if (launches) *launches = 1;
+  if (max_cw > 0 && max_ch > 0) {
+    const dim3 grid_c((max_cw + 255) / 256, (max_ch + 8 * SAO_ROWS - 1) / (8 * SAO_ROWS), b.npics * 2);
+    if (any16) sao_rows_kernel<uint16_t><<<grid_c, block, 0, s>>>(b, 1, 2); else sao_rows_kernel<uint8_t><<<grid_c, block, 0, s>>>(b, 1, 2);
+    if (launches) *launches = 2;
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(B200_E_CUDA, "sao launch: %s", cudaGetErrorString(e));

@@ -22,4 +22,4 @@ for _ in range(reps + 1):
     en.append(st.entropy_ms); rc.append(st.recon_ms); db.append(st.deblock_ms); sa.append(st.sao_ms)
 md5 = hashlib.md5(out.cpu().numpy().tobytes()).hexdigest()
 print(json.dumps({"lib": os.path.basename(os.environ.get("B200_LIB", "libb200heif.so")), "tail": os.environ.get("B200_TAIL_OVERLAP", ""), "side": side, "entropy_ms_min": min(en[1:]), "entropy_ms_mean": sum(en[1:]) / reps,
-                  "recon_ms_mean": sum(rc[1:]) / reps, "deblock_ms_mean": sum(db[1:]) / reps, "sao_ms_mean": sum(sa[1:]) / reps, "sao_form": "row per thread" if os.environ.get("B200_SAO_ROW_PER_THREAD") else "four rows per thread", "front_end": st.front_end, "md5": md5}))
+                  "recon_ms_mean": sum(rc[1:]) / reps, "deblock_ms_mean": sum(db[1:]) / reps, "sao_ms_mean": sum(sa[1:]) / reps, "front_end": st.front_end, "md5": md5}))

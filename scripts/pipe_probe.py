@@ -27,8 +27,7 @@ for d in decs:
 outs = [torch.empty((H, W * 3), dtype=torch.uint8, pin_memory=True).numpy() for _ in range(2)]
 KEYS = ["B200_TAIL_OVERLAP"]
 res = {"side": side, "steps": steps, "runs": {}}
-for name, env, ndec in [("one_decoder", {}, 1), ("two_decoders", {}, 2), ("one_decoder_tail2", {"B200_TAIL_OVERLAP": "2"}, 1), ("two_decoders_tail2", {"B200_TAIL_OVERLAP": "2"}, 2),
-                        ("two_decoders_again", {}, 2), ("one_decoder_again", {}, 1)]:
+for name, env, ndec in [("one_decoder", {}, 1), ("two_decoders", {}, 2), ("two_decoders_again", {}, 2), ("one_decoder_again", {}, 1)]:
     for k in KEYS:
         os.environ.pop(k, None)
     os.environ.update(env)

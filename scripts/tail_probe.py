@@ -30,10 +30,8 @@ host_t = torch.empty((H, W * 3), dtype=torch.uint8, pin_memory=True)
 host_out = host_t.numpy()
 stream = torch.cuda.current_stream()
 Q = str(side * side // 4)
-configs = [("default", {}), ("tail1_2bands", {"B200_TAIL_OVERLAP": "1"}), ("tail2_2bands", {"B200_TAIL_OVERLAP": "2"}),
-           ("tail2_4bands", {"B200_TAIL_OVERLAP": "2", "B200_CHUNK_TILES": Q}), ("tail2_8bands", {"B200_TAIL_OVERLAP": "2", "B200_CHUNK_TILES": str(side * side // 8)}),
-           ("tail_1band", {"B200_TAIL_OVERLAP": "1", "B200_CHUNKS": "0"}), ("notail_4bands", {"B200_CHUNK_TILES": Q}),
-           ("tail2_2bands_again", {"B200_TAIL_OVERLAP": "2"}), ("default_again", {})]
+configs = [("default", {}), ("tail1_2bands", {"B200_TAIL_OVERLAP": "1"}), ("tail_1band", {"B200_TAIL_OVERLAP": "1", "B200_CHUNKS": "0"}),
+           ("notail_4bands", {"B200_CHUNK_TILES": Q}), ("default_again", {})]
 KEYS = ["B200_TAIL_OVERLAP", "B200_CHUNK_TILES", "B200_CHUNKS"]
 out = {"side": side, "steps": steps, "configs": {}}
 for name, env in configs:
