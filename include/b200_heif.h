@@ -101,8 +101,9 @@ int b200_color_convert_device(const b200_planes* in, const b200_geometry* geom, 
 
 /* Host -> host form with H2D / D2H inside (what a libheif ColorConversionOperation calls: integration/b200_color_op.cc).
    Pageable operands move through a page-locked bounce buffer in bands (host threads fill / drain band k while the DMA
-   engine moves band k - 1); the device buffers, the bounce buffer and the stream are kept for the life of the process and
-   concurrent callers are serialised.  Page-locked operands (b200_host_alloc / b200_host_register) are copied directly. */
+   engine moves band k - 1); the device buffers, the bounce buffer and the stream are kept per GPU for the life of the
+   process and concurrent callers are serialised.  Page-locked operands (b200_host_alloc / b200_host_register) are copied
+   directly. */
 int b200_color_convert_host(const b200_planes* in, const b200_geometry* geom, const b200_color_options* opt,
                             void* out, void* out_g, void* out_b, size_t out_stride, int* pipeline);
 
@@ -119,6 +120,8 @@ int b200_color_convert_host(const b200_planes* in, const b200_geometry* geom, co
    full_range are inputs.  matrix_coefficients 0, 8, 11, 14 -> B200_E_UNSUPPORTED (the reference's op refuses them as
    well, rgb2yuv.cc:536-539). */
 int b200_rgb_to_ycbcr_device(const void* rgb, size_t rgb_stride, int has_alpha, const b200_planes* out, void* stream);
+/* Host -> host form: stages its operands as b200_color_convert_host does, with the same buffers, kept per GPU for the life
+   of the process. */
 int b200_rgb_to_ycbcr_host(const void* rgb, size_t rgb_stride, int has_alpha, const b200_planes* out);
 
 /* nclx helper: the 4 float coefficients exactly as nclx.cc:84-173 derives them */

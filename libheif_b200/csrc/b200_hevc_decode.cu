@@ -7,14 +7,12 @@
 // independent tiles at once, which is how ImageItem_Grid::decode_full_grid_image (libheif/image-items/grid.cc:250-468)
 // consumes it.  All expensive state (device arenas, pinned staging, streams, events) lives here and is reused.
 #include "b200_hevc.h"
-#include <atomic>
+#include "b200_staging.h"
 #include <chrono>
-#include <condition_variable>
 #include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
-#include <thread>
 #include <unistd.h>
 
 using namespace b200;
@@ -22,73 +20,6 @@ using namespace b200;
 namespace {
 
 double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
-// minimal persistent thread pool: parallel_for over [0, n)
-class Pool {
- public:
-  explicit Pool(int n) : stop_(false), gen_(0), next_(0), total_(0), pending_(0) { for (int i = 0; i < n; i++) th_.emplace_back([this] { run(); }); }
-  ~Pool() { { std::lock_guard<std::mutex> l(mu_); stop_ = true; } cv_.notify_all(); for (auto& t : th_) t.join(); }
-  void parallel_for(int n, const std::function<void(int)>& fn) {
-    if (n <= 0) return;
-    if (th_.empty() || n == 1) { for (int i = 0; i < n; i++) fn(i); return; }
-    { std::lock_guard<std::mutex> l(mu_); fn_ = &fn; total_ = n; next_.store(0); pending_ = (int)th_.size(); gen_++; }
-    cv_.notify_all();
-    std::unique_lock<std::mutex> l(mu_);
-    done_.wait(l, [this] { return pending_ == 0; });
-  }
- private:
-  void run() {
-    unsigned seen = 0;
-    for (;;) {
-      const std::function<void(int)>* fn; int total;
-      { std::unique_lock<std::mutex> l(mu_); cv_.wait(l, [&] { return stop_ || gen_ != seen; }); if (stop_) return; seen = gen_; fn = fn_; total = total_; }
-      for (;;) { int i = next_.fetch_add(1); if (i >= total) break; (*fn)(i); }
-      { std::lock_guard<std::mutex> l(mu_); if (--pending_ == 0) done_.notify_all(); }
-    }
-  }
-  std::vector<std::thread> th_; std::mutex mu_; std::condition_variable cv_, done_;
-  bool stop_; unsigned gen_; std::atomic<int> next_; int total_, pending_; const std::function<void(int)>* fn_ = nullptr;
-};
-
-template <typename T>
-struct DevBuf {   // grow-only device buffer with optional pinned host staging of the same capacity; owns both (move-only)
-  T* d = nullptr; T* h = nullptr; size_t cap = 0, hcap = 0;
-  DevBuf() = default;
-  DevBuf(DevBuf&& o) noexcept : d(o.d), h(o.h), cap(o.cap), hcap(o.hcap) { o.d = o.h = nullptr; o.cap = o.hcap = 0; }
-  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(d, o.d); std::swap(h, o.h); std::swap(cap, o.cap); std::swap(hcap, o.hcap); return *this; }
-  ~DevBuf() { if (d) cudaFree(d); if (h) cudaFreeHost(h); }
-  int reserve(size_t n, bool host = true) {
-    if (n > cap) {
-      const size_t nc = n + n / 4 + 1024;
-      if (d) cudaFree(d);
-      d = nullptr; cap = 0;
-      B200_CUDA_CHECK(cudaMalloc(&d, nc * sizeof(T)));
-      cap = nc;
-    }
-    if (host && n > hcap) {
-      if (h) cudaFreeHost(h);
-      h = nullptr; hcap = 0;
-      B200_CUDA_CHECK(cudaMallocHost(&h, cap * sizeof(T)));
-      hcap = cap;
-    }
-    return B200_OK;
-  }
-};
-
-// owning handle of a stream, an event or a page-locked block
-template <typename H, cudaError_t (*Destroy)(H)>
-struct Owned {
-  H h = nullptr;
-  Owned() = default;
-  Owned(const Owned&) = delete;
-  Owned& operator=(const Owned&) = delete;
-  ~Owned() { if (h) Destroy(h); }
-  operator H() const { return h; }
-};
-cudaError_t free_pinned(unsigned* p) { return cudaFreeHost(p); }
-using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
-using Event = Owned<cudaEvent_t, cudaEventDestroy>;
-using PinnedFlags = Owned<unsigned*, free_pinned>;
 
 // The counters and queues the kernels share, one batch-wide array each.  Their offsets follow from the batch's CTB rows and
 // sub-streams alone; sizing, clearing and the kernels' batch descriptors all go through this one layout.
@@ -200,7 +131,7 @@ struct b200_decoder {
   std::vector<int> parse_rc; std::vector<std::string> parse_msg;
   DevBuf<PicDesc> pics; DevBuf<CtuInfo> ctus; DevBuf<TuCmd> tus; DevBuf<CoefEntry> coefs; DevBuf<SliceInfo> slices;
   DevBuf<int8_t> qp8; DevBuf<uint8_t> edge8; DevBuf<uint8_t> scaling; DevBuf<uint2> rows; DevBuf<unsigned> sync;   // sync: ScratchLayout
-  DevBuf<uint8_t> rec; DevBuf<uint8_t> canvas; DevBuf<uint8_t> rgb2[2]; DevBuf<uint8_t> bounce;   // fused host entry points: two RGB buffers (D2H of one overlaps the kernels writing the other)
+  DevBuf<uint8_t> rec; DevBuf<uint8_t> canvas; DevBuf<uint8_t> rgb2[2];   // fused host entry points: two RGB buffers (D2H of one overlaps the kernels writing the other)
   // device front-end (entropy decoding on the GPU)
   DevBuf<uint8_t> rbsp; DevBuf<syn::Substream> subs; DevBuf<unsigned> equeue; DevBuf<uint16_t> ctu_slice; DevBuf<EntropyPic> epics;
   DevBuf<uint8_t> ipm4, cd8, wpp_ctx, end_state; DevBuf<unsigned> esync; DevBuf<unsigned long long> ecount;
@@ -210,9 +141,9 @@ struct b200_decoder {
   Event ev_fork, ev_join;          // decode stream -> side before K0, side -> decode stream after it
   Event t_start, t_h2d, t_entropy, t_recon, t_deblock, t_sao;   // stage ends on the decode stream (b200_decoder_get_stats)
   Event ev_k6[2], ev_d2h[2];       // per RGB buffer: colour conversion done, D2H done
-  Event ev_bounce[2];              // pageable destination: the bounce buffer halves
   Event ev_band[MAX_CHUNKS];       // band pipeline: RGB of the band done
-  PinnedFlags err_host;            // per RGB buffer: the error flag of the step that used it last
+  Pinned<unsigned> err_host;       // per RGB buffer: the error flag of the step that used it last
+  Bounce bounce;                   // synchronous fused entry point: the D2H into pageable memory
   int async_slot = 0; bool async_error = false;
   int front_end = 1;               // 1 = CABAC on the GPU (default), 0 = CABAC on the host cores
   int debug_stage = 0;
@@ -627,7 +558,7 @@ int b200_decoder_create(b200_decoder** out, int host_threads) {
   for (Stream* st : {&d->own, &d->copy, &d->side}) B200_CUDA_CHECK(cudaStreamCreateWithFlags(&st->h, cudaStreamNonBlocking));
   for (Event* e : {&d->t_start, &d->t_h2d, &d->t_entropy, &d->t_recon, &d->t_deblock, &d->t_sao, &d->ev_fork, &d->ev_join}) B200_CUDA_CHECK(cudaEventCreate(&e->h));
   for (int i = 0; i < 2; i++)
-    for (Event* e : {&d->ev_k6[i], &d->ev_d2h[i], &d->ev_bounce[i]}) B200_CUDA_CHECK(cudaEventCreateWithFlags(&e->h, cudaEventDisableTiming));
+    for (Event* e : {&d->ev_k6[i], &d->ev_d2h[i]}) B200_CUDA_CHECK(cudaEventCreateWithFlags(&e->h, cudaEventDisableTiming));
   for (Event& e : d->ev_band) B200_CUDA_CHECK(cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming));
   B200_CUDA_CHECK(cudaHostAlloc(reinterpret_cast<void**>(&d->err_host.h), 2 * sizeof(unsigned), cudaHostAllocDefault));
   d->err_host.h[0] = d->err_host.h[1] = 0;
@@ -805,13 +736,6 @@ static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8
   return B200_OK;
 }
 
-static bool is_page_locked(const void* p) {
-  cudaPointerAttributes pa{};
-  const bool pinned = cudaPointerGetAttributes(&pa, p) == cudaSuccess && (pa.type == cudaMemoryTypeHost || pa.type == cudaMemoryTypeManaged);
-  cudaGetLastError();
-  return pinned;
-}
-
 extern "C" {
 
 int b200_decode_grid_to_rgb_host(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
@@ -823,41 +747,12 @@ int b200_decode_grid_to_rgb_host(b200_decoder* d, int cols, int rows, const uint
   int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, info, 0, pinned ? out : nullptr, out_stride, false, &r);
   if (rc) return rc;
   cudaStream_t s = d->own;
-  uint8_t* rgb = d->rgb2[0].d;
-  const size_t rowb = r.rowb, pitch = r.pitch;
-  // D2H: straight into the caller's buffer when it is page-locked (b200_host_alloc, cudaHostAlloc, cudaHostRegister);
-  // pageable memory goes through a page-locked bounce buffer in row bands, the copy of band i overlapping the memcpy of
-  // band i - 1 on the decoder's host threads
   if (r.bands_copied) {                                 // the bands left through the copy stream as they were finished
     B200_CUDA_CHECK(cudaEventRecord(d->ev_d2h[0], d->copy));
     B200_CUDA_CHECK(cudaStreamSynchronize(s));
     B200_CUDA_CHECK(cudaStreamSynchronize(d->copy));
-  } else if (pinned) {
-    B200_CUDA_CHECK(cudaMemcpy2DAsync(out, out_stride, rgb, pitch, rowb, (size_t)r.height, cudaMemcpyDeviceToHost, s));
-    B200_CUDA_CHECK(cudaEventRecord(d->ev_d2h[0], s));
-    B200_CUDA_CHECK(cudaStreamSynchronize(s));
-  } else {
-    const size_t oh = (size_t)r.height, band_rows = std::max<size_t>(1, (size_t)(32u << 20) / rowb);
-    const int nb = (int)((oh + band_rows - 1) / band_rows);
-    if ((rc = d->bounce.reserve(2 * band_rows * rowb, true))) return rc;
-    for (int k = 0; k <= nb; k++) {
-      if (k < nb) {
-        const size_t y0 = (size_t)k * band_rows, h = std::min(band_rows, oh - y0);
-        B200_CUDA_CHECK(cudaMemcpy2DAsync(d->bounce.h + (size_t)(k & 1) * band_rows * rowb, rowb, rgb + y0 * pitch, pitch, rowb, h, cudaMemcpyDeviceToHost, s));
-        B200_CUDA_CHECK(cudaEventRecord(d->ev_bounce[k & 1], s));
-      }
-      if (k > 0) {
-        const int j = k - 1;
-        const size_t y0 = (size_t)j * band_rows, h = std::min(band_rows, oh - y0);
-        B200_CUDA_CHECK(cudaEventSynchronize(d->ev_bounce[j & 1]));
-        const uint8_t* src = d->bounce.h + (size_t)(j & 1) * band_rows * rowb;
-        const int parts = 8;
-        d->pool->parallel_for(parts, [&](int t) {
-          const size_t r0 = h * (size_t)t / parts, r1 = h * (size_t)(t + 1) / parts;
-          for (size_t y = r0; y < r1; y++) memcpy(static_cast<uint8_t*>(out) + (y0 + y) * out_stride, src + y * rowb, rowb);
-        });
-      }
-    }
+  } else {                                              // pageable memory is drained from the bounce buffer by the decoder's host threads
+    if ((rc = d->bounce.download(out, out_stride, d->rgb2[0].d, r.pitch, r.rowb, (size_t)r.height, s, *d->pool))) return rc;
     B200_CUDA_CHECK(cudaEventRecord(d->ev_d2h[0], s));
     B200_CUDA_CHECK(cudaStreamSynchronize(s));
   }
