@@ -69,6 +69,7 @@ struct EntropyBatch {
   int blocks_per_sm;             // > 0: cap of resident CTAs per SM (co-residency with K1)
   int common;                    // 1: every picture matches syn::CfgCommon (specialised kernel)
 };
+int entropy_warps_per_sm(bool common);    // resident K0 decoders (warps) per SM at full occupancy (common: the CfgCommon instantiation)
 int launch_entropy(const EntropyBatch& b, cudaStream_t s, int* resident_warps = nullptr);   // resident_warps: decoders of the launched grid (all co-resident)
 int launch_entropy_gate(const EntropyBatch& b, int resident_warps, cudaStream_t s);            // returns (in stream order) once every K0 warp has taken its first sub-stream
 int launch_entropy_stats(const EntropyBatch& b, unsigned long long* out2, cudaStream_t s);

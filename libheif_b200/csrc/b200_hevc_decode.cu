@@ -68,7 +68,10 @@ struct BatchShape {            // what the launch schedule depends on in a batch
   int bands = 0;               // row bands the row list is laid out in (0: not laid out yet)
 };
 
-enum { OVERLAP_K0_BLOCKS_PER_SM = 3, OVERLAP_K1_BLOCKS_PER_SM = 2 };   // resident CTAs per SM while K0 and K1 share the SMs
+// Resident CTAs per SM while K0 and K1 share the SMs.  Both kernels run 128 threads per CTA at 96 registers (K0: CfgCommon),
+// so 3 + 2 CTAs fill 60 K of the SM's 64 K registers.  (K0 with CfgRuntime needs 124 registers: there the 2nd K1 CTA does
+// not fit and waits for a free slot.)
+enum { OVERLAP_K0_BLOCKS_PER_SM = 3, OVERLAP_K1_BLOCKS_PER_SM = 2 };
 
 struct LaunchPlan {
   int bands = 1, rows_per_band = 1;   // row bands of whole tile rows (rows_per_band: when the plan lays them out)
@@ -92,7 +95,7 @@ int sm_count() { int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttri
 // is resident finishes the work); the CTA caps only share the SM's registers between them.  Running them concurrently hides
 // K1 completely while the batch is critical-path bound -- up to about one wave of sub-streams -- and LOSES once the GPU is
 // throughput bound (the two instruction streams evict each other).
-// Tail overlap, for batches of more than one wave: K0 keeps the whole GPU (4 CTAs per SM, launched first) and the live K1 is
+// Tail overlap, for batches of more than one wave: K0 keeps the whole GPU (5 CTAs per SM for CfgCommon, else 4; launched first) and the live K1 is
 // queued behind it on the other stream, so K1's CTAs become resident only where K0's persistent CTAs have left -- which they
 // do over the last ~30 % of K0's run time, once every sub-stream has been handed out and the wavefronts of the tiles drain.
 // K1 (and, with bands, K3 / K4 / K6 / D2H of the first band; one K1 per band) then runs in SM slots that would otherwise idle.
@@ -101,7 +104,7 @@ int sm_count() { int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttri
 LaunchPlan plan_launches(const BatchShape& b, bool hook, const Overrides& env) {
   LaunchPlan p;
   const bool devfe = b.device_front_end;
-  const bool one_wave = devfe && (env.overlap == Overrides::AUTO ? b.n_subs <= (size_t)sm_count() * 16       // 4 CTAs x 4 warps of K0 per SM
+  const bool one_wave = devfe && (env.overlap == Overrides::AUTO ? b.n_subs <= (size_t)sm_count() * entropy_warps_per_sm(b.all_common)   // K0 decoders per SM: 20 (CfgCommon) or 16
                                                                   : env.overlap == Overrides::ON);
   p.bands = b.bands;
   if (!p.bands) {

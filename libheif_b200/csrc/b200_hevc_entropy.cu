@@ -94,10 +94,22 @@ struct DevSync {
 #ifndef B200_ENTROPY_MIN_BLOCKS
 #define B200_ENTROPY_MIN_BLOCKS 1
 #endif
+// Compile-time cap of resident K0 CTAs per SM (0: none, occupancy decides) -- for measuring how K0 scales with the number of
+// decoders per SM.
+#ifndef B200_ENTROPY_MAX_BLOCKS_PER_SM
+#define B200_ENTROPY_MAX_BLOCKS_PER_SM 0
+#endif
+// CfgCommon's call chain (kernel -> decode_ctb -> residual -> refill) fits in 96 registers without spilling, which makes 5 CTAs
+// (20 decoders) per SM: registers are allocated for all 32 lanes of a warp, so they, not the work, cap the number of decoders.
+// The bound holds that figure: should a change need more, ptxas reports spills (-Xptxas -v) instead of silently dropping
+// to 4 CTAs.  CfgRuntime needs 124 registers: 4 CTAs.
+template <class Cfg> constexpr int entropy_min_blocks() { return B200_ENTROPY_MIN_BLOCKS; }
+template <> constexpr int entropy_min_blocks<syn::CfgCommon>() { return B200_ENTROPY_MIN_BLOCKS > 5 ? B200_ENTROPY_MIN_BLOCKS : 5; }
 template <class Cfg>
-__global__ void __launch_bounds__(EWARPS * 32, B200_ENTROPY_MIN_BLOCKS) hevc_entropy_kernel(const EntropyBatch b) {
+__global__ void __launch_bounds__(EWARPS * 32, entropy_min_blocks<Cfg>()) hevc_entropy_kernel(const EntropyBatch b) {
   __shared__ __align__(8) syn::U2 s_ctx[EWARPS][syn::CTX_COUNT];   // context variables: one state-table entry each
   __shared__ syn::DecoderT<Cfg> s_dec[EWARPS];                    // per-warp decoder state (see run_substream)
+  __shared__ DevSync s_sync[EWARPS];                              // per-warp hand-shake pointers (shared: no register holds them across the CTB loop)
   for (int i = threadIdx.x; i < 64; i += blockDim.x) { syn::s_kLps4[i] = syn::d_kLps4[i]; syn::s_kTransLps[i] = syn::d_kTransLps[i]; }
   for (int i = threadIdx.x; i < syn::CTX_COUNT; i += blockDim.x) syn::s_kInitI[i] = syn::d_kInitI[i];
   for (int i = threadIdx.x; i < 256; i += blockDim.x) syn::s_kNextState[i] = syn::d_kNextState[i];
@@ -131,7 +143,7 @@ __global__ void __launch_bounds__(EWARPS * 32, B200_ENTROPY_MIN_BLOCKS) hevc_ent
     }
     const syn::Substream& gs = b.subs[item - 1u];
     const EntropyPic& ep = b.pics[gs.pic];
-    DevSync sync;
+    DevSync& sync = s_sync[slot_w];
     sync.progress = b.progress + ep.progress_base; sync.sub_done = b.sub_done + ep.sub_base; sync.error_flag = b.error_flag;
     sync.queue = b.queue; sync.qtail = b.qtail; sync.deps = b.deps;
     sync.dense_tu = sync.dense_coef = sync.dense_tu_cap = sync.dense_coef_cap = 0; sync.end_bit_position = 0;
@@ -172,14 +184,24 @@ int launch_entropy_gate(const EntropyBatch& b, int resident_warps, cudaStream_t 
   return B200_OK;
 }
 
+// resident CTAs per SM of the entropy kernel, before a caller's cap (EntropyBatch::blocks_per_sm).  common: every picture of
+// the batch has the CfgCommon parameter combination -> the specialised (smaller) kernel
+static int entropy_blocks_per_sm(bool common) {
+  auto kern = common ? hevc_entropy_kernel<syn::CfgCommon> : hevc_entropy_kernel<syn::CfgRuntime>;
+  int occ = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, EWARPS * 32, 0);
+  if (occ < 1) occ = 1;
+  if (B200_ENTROPY_MAX_BLOCKS_PER_SM > 0 && occ > B200_ENTROPY_MAX_BLOCKS_PER_SM) occ = B200_ENTROPY_MAX_BLOCKS_PER_SM;
+  return occ;
+}
+
+int entropy_warps_per_sm(bool common) { return entropy_blocks_per_sm(common) * EWARPS; }
+
 int launch_entropy(const EntropyBatch& b, cudaStream_t s, int* resident_warps) {
   if (resident_warps) *resident_warps = 0;
   if (b.nsubs <= 0) return B200_OK;
   int dev = 0, sms = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  // b.common: every picture of the batch has the CfgCommon parameter combination -> the specialised (smaller) kernel
   auto kern = b.common ? hevc_entropy_kernel<syn::CfgCommon> : hevc_entropy_kernel<syn::CfgRuntime>;
-  int occ = 1; cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, EWARPS * 32, 0);
-  if (occ < 1) occ = 1;
+  int occ = entropy_blocks_per_sm(b.common != 0);
   if (b.blocks_per_sm > 0 && b.blocks_per_sm < occ) occ = b.blocks_per_sm;
   const int want = (b.nsubs + EWARPS - 1) / EWARPS;
   const int grid = want < sms * occ ? want : sms * occ;

@@ -313,6 +313,7 @@ struct DecoderT {
   int is_dqp_coded, dqp_val, qpy_prev_qg, last_cu_qpy, first_qg, cur_qpy, err;
   int cu_bypass;                                  // cu_transquant_bypass_flag of the current coding unit
   uint32_t tu_n, coef_n, tu_cap, coef_cap;        // write cursors / limits of the current CTB (or of the picture when dense)
+  uint32_t ctb_tu0;                               // first TU of the current CTB
   int cur_ctb_x, cur_ctb_y;
   int ctb_x0, ctb_y0, left_ok, up_ok;            // current CTB: origin, availability of the CTB to the left / above (same region: slice and tile)
   int left_lf, up_lf;                            // deblocking across the CTB's left / upper boundary is allowed (8.7.2.3: slice and tile rules)
@@ -383,7 +384,7 @@ struct DecoderT {
     Cabac cb_ = cabac; const CtxPtr cx = ctx;
     const int bypass_cu = B200_SPC(tq_bypass) && cu_bypass;            // 7.3.8.11: no transform_skip_flag, no sign data hiding
     const int sign_hiding = B200_SPC(sign_hiding) && !bypass_cu;
-    CoefEntry* const coef_out = pb.coefs; uint32_t cn = coef_n; const uint32_t ccap = coef_cap;
+    uint32_t cn = coef_n;
     tskip = 0;
     if (B200_SPC(transform_skip) && log2n == 2 && !bypass_cu) tskip = cb_.bin(ctx_at(cx, CTX_TSKIP + (c ? 1 : 0)), stream);
     const int cmax = (log2n << 1) - 1;
@@ -417,20 +418,19 @@ struct DecoderT {
     if (scan == 2) { const int t = lx; lx = ly; ly = t; }
     if (lx >= n || ly >= n) { err = SYN_E_BITSTREAM; cabac = cb_; return 0; }
     const int l2sb = log2n - 2;
-    const uint8_t *sbx = B200_T(kScanX)[l2sb][scan], *sby = B200_T(kScanY)[l2sb][scan], *spos = B200_T(kScanPos)[scan];
+    const TabPtr sbx = B200_TADDR(kScanX) + 64 * (3 * l2sb + scan), sby = B200_TADDR(kScanY) + 64 * (3 * l2sb + scan), spos = B200_TADDR(kScanPos) + 16 * scan;
     const int last_sb = B200_T(kSbInv)[l2sb][scan][((ly >> 2) << 3) + (lx >> 2)];
     const int last_pos = B200_T(kScanInv)[scan][((ly & 3) << 2) + (lx & 3)];
     uint64_t csbf = 0;                                  // coded_sub_block_flag, bit (ys * 8 + xs)
-    int carry = 1, count = 0; bool first_done = false;
-    const int nsbw = 1 << l2sb;
-    const int dc_ctx = CTX_SIG + (c ? 27 : 0);
-    const int sig_base = log2n == 2 ? dc_ctx : (c == 0 ? CTX_SIG + (log2n == 3 ? (scan == 0 ? 9 : 15) : 21) : CTX_SIG + 27 + (log2n == 3 ? 9 : 12));
+    int carry = 1;                                      // greater1Ctx carried over (9.3.4.2.6); not 0 before the first coded sub-block
+    const int sig_base = log2n == 2 ? CTX_SIG + (c ? 27 : 0) : (c == 0 ? CTX_SIG + (log2n == 3 ? (scan == 0 ? 9 : 15) : 21) : CTX_SIG + 27 + (log2n == 3 ? 9 : 12));
     B200_NOUNROLL for (int i = last_sb; i >= 0; i--) {
-      const int xs = sbx[i], ys = sby[i];
-      const int right = (xs + 1 < nsbw) ? (int)((csbf >> (ys * 8 + xs + 1)) & 1) : 0;
-      const int below = (ys + 1 < nsbw) ? (int)((csbf >> ((ys + 1) * 8 + xs)) & 1) : 0;
+      const int xs = (int)tab_ld8(sbx, i), ys = (int)tab_ld8(sby, i);
+      const int right = ((xs + 1) >> l2sb) == 0 ? (int)((csbf >> (ys * 8 + xs + 1)) & 1) : 0;
+      const int below = ((ys + 1) >> l2sb) == 0 ? (int)((csbf >> ((ys + 1) * 8 + xs)) & 1) : 0;
+      const bool is_last = csbf == 0;                   // the sub-block of the last significant coefficient is the first one coded
       int infer_dc = 0;
-      if (i < last_sb && i > 0) { if (!cb_.bin(ctx_at(cx, CTX_CSBF + ((right | below) ? 1 : 0) + (c ? 2 : 0)), stream)) continue; infer_dc = 1; }
+      if (!is_last && i > 0) { if (!cb_.bin(ctx_at(cx, CTX_CSBF + ((right | below) ? 1 : 0) + (c ? 2 : 0)), stream)) continue; infer_dc = 1; }
       csbf |= 1ull << (ys * 8 + xs);
       // sig_coeff_flag (9.3.4.2.5): context = per-sub-block base + table entry per scan position; DC of the block has its own
       const TabPtr tab = log2n == 2 ? B200_TADDR(kSigCtx4) + 16 * scan : B200_TADDR(kSigCtxN) + (64 * scan + 16 * (right | (below << 1)));
@@ -438,11 +438,11 @@ struct DecoderT {
       // flags are shifted in from the right: after the last position (k = 0) bit k of `sig` is the flag of scan position k
       unsigned sig = 0;
       int k = 15;
-      if (i == last_sb) { sig = 1u; k = last_pos - 1; }
+      if (is_last) { sig = 1u; k = last_pos - 1; }
       if (k >= 0) {
         // software pipeline: the entry of position k - 1 is in flight while position k is decoded (the contexts depend on the
         // position only, 9.3.4.2.5); same context twice in a row -> forward the new entry in registers
-        const CtxPtr a0 = i == 0 ? ctx_at(cx, dc_ctx) : ctx_at(cbase, (int)tab_ld8(tab, 0));
+        const CtxPtr a0 = i == 0 ? ctx_at(cx, CTX_SIG + (c ? 27 : 0)) : ctx_at(cbase, (int)tab_ld8(tab, 0));
         CtxPtr a_cur = k > 0 ? ctx_at(cbase, (int)tab_ld8(tab, k)) : a0;
         U2 e_cur = ctx_ld(a_cur);
         B200_NOUNROLL for (; k > 0; k--) {
@@ -459,8 +459,7 @@ struct DecoderT {
       unsigned g1 = 0;
       int g1ctx = 1, g2 = 0;
       int ctx_set = (i == 0 || c > 0) ? 0 : 2;
-      if (first_done && carry == 0) ctx_set++;
-      first_done = true;
+      if (carry == 0) ctx_set++;
       const int last_sig = hi_bit(sig), first_sig = lo_bit(sig);
       { unsigned m = sig; const CtxPtr gbase = ctx_at(cx, CTX_GT1 + ctx_set * 4 + (c ? 16 : 0));
         B200_NOUNROLL for (int ng1 = 0; m && ng1 < 8; ng1++) {
@@ -480,7 +479,7 @@ struct DecoderT {
         int a = base;
         if (base == ((nsig < 8) ? ((kk == last_g1) ? 3 : 2) : 1)) {
           int pre = 0; B200_NOUNROLL while (pre < 32 && cb_.bypass(stream)) pre++;
-          if (pre > 20) { err = SYN_E_BITSTREAM; cabac = cb_; coef_n = cn; return count; }   // far outside the 16-bit range of TransCoeffLevel: corrupt data
+          if (pre > 20) { err = SYN_E_BITSTREAM; cabac = cb_; const int count = (int)(cn - coef_n); coef_n = cn; return count; }   // far outside the 16-bit range of TransCoeffLevel: corrupt data
           const int rem = (pre <= 3 ? (pre << rice) : (((1 << (pre - 3)) + 3 - 1) << rice)) + (int)cb_.bypass_bits(pre <= 3 ? rice : pre - 3 + rice, stream);
           a = base + rem;
           if (a > 3 * (1 << rice)) rice = imin(rice + 1, 4);
@@ -489,13 +488,15 @@ struct DecoderT {
         if (!hidden || kk != first_sig) { sidx--; neg = (int)((signs >> sidx) & 1); }
         int v = neg ? -a : a;
         if (hidden) { sum += a; if (kk == first_sig && (sum & 1)) v = -v; }
-        if (cn >= ccap) { err = SYN_E_OVERFLOW; cabac = cb_; coef_n = cn; return count; }
-        const int p = spos[kk];
+        if (cn >= coef_cap) { err = SYN_E_OVERFLOW; cabac = cb_; const int count = (int)(cn - coef_n); coef_n = cn; return count; }
+        const int p = (int)tab_ld8(spos, kk);
         CoefEntry e; e.pos = (uint16_t)((((ys << 2) + (p >> 2)) << log2n) + (xs << 2) + (p & 3)); e.level = (int16_t)clip3(-32768, 32767, v);
-        coef_out[cn++] = e; count++;
+        pb.coefs[cn++] = e;
       }
     }
-    cabac = cb_; coef_n = cn;
+    cabac = cb_;
+    const int count = (int)(cn - coef_n);                 // coefficients written
+    coef_n = cn;
     return count;
   }
 
@@ -530,29 +531,32 @@ struct DecoderT {
     const int pu = cu.nxn ? ((y0 >= cu.y0 + (1 << (cu.log2cb - 1))) ? 2 : 0) + ((x0 >= cu.x0 + (1 << (cu.log2cb - 1))) ? 1 : 0) : 0;
     const int lmode = cu.lmode[pu];
     const uint32_t coef0 = coef_n;
-    int ts_l = 0, ts_cb = 0, ts_cr = 0, nl = 0, ncb = 0, ncr = 0;
     int chroma_here = 0, ccb = 0, ccr = 0;
     if (B200_SPC(chroma)) {
       if (log2n > 2) { chroma_here = 1; ccb = cbf_cb; ccr = cbf_cr; }
       else if (blk == 3) { chroma_here = 1; ccb = pcb; ccr = pcr; }      // 4x4 chroma blocks of the parent 8x8 node
     }
+    // The command is assembled before the residuals and only its packed words (plus the loop counter) are live across the
+    // residual_coding calls: position, size, cbf flags, modes, later the transform-skip flags and coefficient counts.
+    TuCmd t;
+    t.w0 = (uint32_t)(x0 >> 2) | ((uint32_t)(y0 >> 2) << 12) | ((uint32_t)(log2n - 2) << 24) | ((uint32_t)cbf_l << 26) | ((uint32_t)ccb << 27) |
+           ((uint32_t)ccr << 28) | ((uint32_t)chroma_here << 29);
+    t.w1 = (uint32_t)lmode | ((uint32_t)cu.cmode << 6) | ((B200_SPC(tq_bypass) && cu_bypass) ? 1u << 22 : 0u);
+    t.w2 = coef0;
+    t.w3 = 0;
     // one residual_coding site serves the three components (it is inlined: call frames of a lone lane cost a 128-byte
     // line of L1 per saved register)
     B200_NOUNROLL for (int c = 0; c < 3; c++) {
-      const int coded = c == 0 ? cbf_l : (c == 1 ? ccb : ccr);
-      if (!coded) continue;
+      if (!((t.w0 >> (26 + c)) & 1u)) continue;                          // cbf of the component
+      const int l2 = (int)((t.w0 >> 24) & 3u) + 2;
       int ts = 0;
-      const int cnt = residual(c == 0 ? log2n : (log2n > 2 ? log2n - 1 : 2), c, c == 0 ? lmode : cu.cmode, ts);
-      if (c == 0) { nl = cnt; ts_l = ts; } else if (c == 1) { ncb = cnt; ts_cb = ts; } else { ncr = cnt; ts_cr = ts; }
+      const int cnt = residual(c == 0 ? l2 : (l2 > 2 ? l2 - 1 : 2), c, (int)((t.w1 >> (c == 0 ? 0 : 6)) & 63u), ts);
+      t.w3 |= (uint32_t)cnt << (c == 0 ? 0 : (c == 1 ? 11 : 21));
+      if (c == 0) t.w0 |= (uint32_t)ts << 30; else if (c == 1) t.w0 |= (uint32_t)ts << 31; else t.w1 |= (uint32_t)ts << 20;
     }
-    mark_tu(x0, y0, log2n);
+    mark_tu((int)(t.w0 & 0xfffu) << 2, (int)((t.w0 >> 12) & 0xfffu) << 2, (int)((t.w0 >> 24) & 3u) + 2);
     if (tu_n >= tu_cap) { err = SYN_E_OVERFLOW; return; }
-    TuCmd t;
-    t.w0 = (uint32_t)(x0 >> 2) | ((uint32_t)(y0 >> 2) << 12) | ((uint32_t)(log2n - 2) << 24) | ((uint32_t)cbf_l << 26) | ((uint32_t)ccb << 27) |
-           ((uint32_t)ccr << 28) | ((uint32_t)chroma_here << 29) | ((uint32_t)ts_l << 30) | ((uint32_t)ts_cb << 31);
-    t.w1 = (uint32_t)lmode | ((uint32_t)cu.cmode << 6) | ((uint32_t)(cur_qpy + 64) << 12) | ((uint32_t)ts_cr << 20) | ((B200_SPC(tq_bypass) && cu_bypass) ? 1u << 22 : 0u);
-    t.w2 = coef0;
-    t.w3 = (uint32_t)nl | ((uint32_t)ncb << 11) | ((uint32_t)ncr << 21);
+    t.w1 |= (uint32_t)(cur_qpy + 64) << 12;
     pb.tus[tu_n++] = t;
   }
 
@@ -808,14 +812,17 @@ struct DecoderT {
 
   // -------- 7.3.8.4
   // coding_quadtree (7.3.8.4) of one CTB, iteratively over minimum coding blocks in z-order (same walk as transform_tree)
-  B200_HDI void coding_quadtree(int xc, int yc) {
-    const int log2min = B200_SPC(log2_min_cb), levels = sp->log2ctb - log2min, total = 1 << (2 * levels);
-    B200_NOUNROLL for (int i = 0; i < total && !err;) {
-      int depth = node_depth((unsigned)i, levels);
+  // Only the z-order position and the depth stay in registers across the calls of the walk: the CTB origin and the tree
+  // size are read again from the decoder state (shared memory on the device, see run_substream) where they are needed.
+  B200_HD inline int cq_levels() const { return sp->log2ctb - B200_SPC(log2_min_cb); }
+  B200_HDI void coding_quadtree() {
+    const int log2min = B200_SPC(log2_min_cb);
+    B200_NOUNROLL for (int i = 0; i < (1 << (2 * cq_levels())) && !err;) {
+      int depth = node_depth((unsigned)i, cq_levels());
       B200_NOUNROLL for (;;) {
         const int log2cb = sp->log2ctb - depth, n = 1 << log2cb;
-        const int x0 = xc + (zx((unsigned)i) << log2min), y0 = yc + (zx((unsigned)i >> 1) << log2min);
-        if (x0 >= sp->W || y0 >= sp->H) { i += 1 << (2 * (levels - depth)); break; }      // node outside the picture: not coded
+        const int x0 = ctb_x0 + (zx((unsigned)i) << log2min), y0 = ctb_y0 + (zx((unsigned)i >> 1) << log2min);
+        if (x0 >= sp->W || y0 >= sp->H) { i += 1 << (2 * (cq_levels() - depth)); break; }      // node outside the picture: not coded
         int split;
         if (x0 + n <= sp->W && y0 + n <= sp->H && log2cb > log2min) {
           int inc = 0;
@@ -829,7 +836,7 @@ struct DecoderT {
         }
         if (split) { depth++; continue; }
         coding_unit(x0, y0, log2cb, depth);
-        i += 1 << (2 * (levels - depth));
+        i += 1 << (2 * (cq_levels() - depth));
         break;
       }
     }
@@ -851,14 +858,15 @@ struct DecoderT {
     CtuInfo& ci = pb.ctus[addr];
     ci.slice_idx = (uint16_t)ss->slice_idx;
     if (!B200_SPC(dense)) { tu_n = (uint32_t)addr * (uint32_t)sp->tu_slots; tu_cap = tu_n + (uint32_t)sp->tu_slots; coef_n = (uint32_t)addr * (uint32_t)sp->coef_slots; coef_cap = coef_n + (uint32_t)sp->coef_slots; }
-    const uint32_t t0 = tu_n;
+    ctb_tu0 = tu_n;
     if (B200_SPC(sao_enabled)) parse_sao(rx, ry, ci);
     else for (int c = 0; c < 3; c++) { ci.sao[c].type = 0; ci.sao[c].band_or_class = 0; B200_NOUNROLL for (int k = 0; k < 4; k++) ci.sao[c].offset[k] = 0; }
     // 4x4 luma transform units only OR their edge bits: clear this CTB's flags first
     { const int b0x = rx << (sp->log2ctb - 3), b0y = ry << (sp->log2ctb - 3), nb = 1 << (sp->log2ctb - 3);
       B200_NOUNROLL for (int y = 0; y < nb && b0y + y < sp->h8; y++) B200_NOUNROLL for (int x = 0; x < nb && b0x + x < sp->w8; x++) pb.edge8[(b0y + y) * sp->w8 + b0x + x] = 0; }
-    coding_quadtree(rx << sp->log2ctb, ry << sp->log2ctb);
-    ci.tu_start = t0; ci.tu_count = (uint16_t)(tu_n - t0);
+    coding_quadtree();
+    CtuInfo& ce = pb.ctus[cur_ctb_y * sp->wctb + cur_ctb_x];        // (read again, like the quadtree's state)
+    ce.tu_start = ctb_tu0; ce.tu_count = (uint16_t)(tu_n - ctb_tu0);
   }
 };
 
@@ -899,37 +907,39 @@ B200_HD int run_substream(DecoderT<Cfg>& d, const SeqParams& sp, const PicBuffer
   }
   d.stream.d = pb.rbsp; d.stream.size = pb.rbsp_size;
   d.cabac.start(d.stream, ss.byte_begin);
+  // From here on every parameter is read through `d` (and `sync`), never through the references above: on the device
+  // both live in shared memory, and whatever is read again after a call into the decoder costs a shared-memory load per CTB
+  // instead of a register for the whole call chain (its register count sets how many decoders fit on an SM).
   const bool tiles = B200_SPR(tiles) != 0;
   int rx = rx0, ry = ry0;
-  const uint32_t nctb = ss.ctb_end - ss.ctb_begin;
-  B200_NOUNROLL for (uint32_t k = 0; k < nctb; k++, rx++) {
-    if (rx == (int)ss.tile_x1) { rx = (int)ss.tile_x0; ry++; }    // next row of the tile (of the picture without tiles)
-    const uint32_t a = (uint32_t)ry * (uint32_t)sp.wctb + (uint32_t)rx;
+  B200_NOUNROLL for (uint32_t left = ss.ctb_end - ss.ctb_begin; left > 0; left--, rx++) {
+    if (rx == (int)d.ss->tile_x1) { rx = (int)d.ss->tile_x0; ry++; }    // next row of the tile (of the picture without tiles)
+    const uint32_t a = (uint32_t)ry * (uint32_t)d.sp->wctb + (uint32_t)rx;
     // split_cu_flag context / SAO merge-up read the CTB above (same column).  With tiles that CTB belongs to this very
     // sub-stream or is unavailable (another tile / slice), and rows are not produced in raster order: no hand-shake.
     if (ry > 0 && !tiles) sync.wait_row(ry - 1, rx + 1);
-    if (B200_SPR(wpp) && rx == 0 && a != ss.ctb_begin) {
+    if (B200_SPR(wpp) && rx == 0 && a != d.ss->ctb_begin) {
       // only reached without WPP sub-stream splitting (never: WPP rows are separate sub-streams); kept for safety
       d.first_qg = 1;
     }
-    if (!B200_SPR(wpp) && rx == 0 && a != ss.ctb_begin) { /* QG state simply continues */ }
     d.decode_ctb((int)a);
     if (d.err) break;
-    if (B200_SPR(wpp) && rx == 1) { uint8_t* st = pb.wpp_ctx + (size_t)ry * CTX_STRIDE; B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) st[i] = (uint8_t)(ctx_ld(ctx_at(ctx, i)).y >> 24); }
+    rx = d.cur_ctb_x; ry = d.cur_ctb_y;
+    if (B200_SPR(wpp) && rx == 1) { uint8_t* st = d.pb.wpp_ctx + (size_t)ry * CTX_STRIDE; B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) st[i] = (uint8_t)(ctx_ld(ctx_at(d.ctx, i)).y >> 24); }
     const int end = d.cabac.terminate(d.stream);                          // end_of_slice_segment_flag
-    const bool last = k + 1 == nctb;
-    if (end != ((last && ss.last_of_segment) ? 1 : 0)) { d.err = SYN_E_BITSTREAM; break; }
-    if (last && !ss.last_of_segment) { if (!d.cabac.terminate(d.stream)) { d.err = SYN_E_BITSTREAM; break; } }   // end_of_subset_one_bit
+    const bool last = left == 1;
+    if (end != ((last && d.ss->last_of_segment) ? 1 : 0)) { d.err = SYN_E_BITSTREAM; break; }
+    if (last && !d.ss->last_of_segment) { if (!d.cabac.terminate(d.stream)) { d.err = SYN_E_BITSTREAM; break; } }   // end_of_subset_one_bit
     if (!tiles) sync.publish_row(ry, rx + 1);
-    if (B200_SPR(wpp) && rx == 1) sync.notify(ss.wake_ctb2);           // the row below may start (its context hand-over is stored)
-    if (d.cabac.pos > pb.rbsp_size + 64u) { d.err = SYN_E_BITSTREAM; break; }
+    if (B200_SPR(wpp) && rx == 1) sync.notify(d.ss->wake_ctb2);           // the row below may start (its context hand-over is stored)
+    if (d.cabac.pos > d.pb.rbsp_size + 64u) { d.err = SYN_E_BITSTREAM; break; }
   }
   // end state for a dependent continuation + dense cursors
-  { uint8_t* st = pb.end_state + (size_t)index * CTX_STRIDE; B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) st[i] = (uint8_t)(ctx_ld(ctx_at(ctx, i)).y >> 24); st[CTX_COUNT] = (uint8_t)(int8_t)d.last_cu_qpy; }
+  { uint8_t* st = d.pb.end_state + (size_t)index * CTX_STRIDE; B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) st[i] = (uint8_t)(ctx_ld(ctx_at(d.ctx, i)).y >> 24); st[CTX_COUNT] = (uint8_t)(int8_t)d.last_cu_qpy; }
   if (B200_SPR(dense)) { sync.dense_tu = d.tu_n; sync.dense_coef = d.coef_n; }
   sync.end_bit_position = d.cabac.bit_position();
   sync.finish_substream(index, d.err);
-  if (!d.err) sync.notify(ss.wake_end);
+  if (!d.err) sync.notify(d.ss->wake_end);
   return d.err;
 }
 
