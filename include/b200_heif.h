@@ -124,6 +124,55 @@ int b200_rgb_to_ycbcr_device(const void* rgb, size_t rgb_stride, int has_alpha, 
    of the process. */
 int b200_rgb_to_ycbcr_host(const void* rgb, size_t rgb_stride, int has_alpha, const b200_planes* out);
 
+/* Encoder-side direction for every RGB layout heif_context_encode_image accepts: the chain convert_colorspace
+   (colorconversion.cc:490-623) picks from the input to YCbCr at the input's depth (output_bpp = 0, encoder.cc:168-174).
+   Replaces: Op_RGB24_32_to_YCbCr              rgb2yuv.cc:506-808 (interleaved RGB / RGBA 8 bit; b200_rgb_to_ycbcr_device's kernel)
+             Op_RRGGBBxx_HDR_to_YCbCr420       rgb2yuv.cc:311-503 (RRGGBB[AA] BE / LE, full range, 4:2:0)
+             Op_RGB_to_YCbCr<uint8_t / uint16_t> rgb2yuv.cc:30-305 (planar RGB; matrix 0 and 8 branches, limited range x219/256,
+                                               x224/256; 4:2:0 chroma from the float mean of the quad, 4:2:2 from the left pixel)
+             Op_RGB24_32_to_YCbCr444_GBR       rgb2yuv.cc:812-919 (interleaved 8 bit, matrix 0, full range, 4:4:4)
+   with the lossless steps the reference runs before Op_RGB_to_YCbCr -- Op_RRGGBBaa_swap_endianness, Op_RRGGBBaa_BE_to_RGB_HDR,
+   Op_RGB24_32_to_RGB (rgb2rgb.cc) -- folded into the kernel's loader. */
+typedef struct b200_rgb_image {
+  const void* rgb; size_t rgb_stride;            /* interleaved layouts: the one plane (> 8 bit: bytes in the layout's order) */
+  const void* r; const void* g; const void* b; const void* alpha;   /* planar (chroma B200_CHROMA_444): > 8 bit as native uint16;
+                                                                       alpha may be NULL */
+  size_t r_stride, g_stride, b_stride, alpha_stride;
+  int width, height;
+  int chroma;                 /* B200_CHROMA_INTERLEAVED_* (heif_chroma_interleaved_*), or B200_CHROMA_444 = planar R, G, B */
+  int bit_depth;              /* 8 for RGB / RGBA, 9..16 for RRGGBB[AA], 8..16 planar */
+  int alpha_bit_depth;        /* planar alpha plane: 0 = bit_depth */
+} b200_rgb_image;
+
+typedef struct b200_rgb_to_ycbcr_options {   /* the two members of heif_color_conversion_options the planner reads here */
+  int chroma_downsampling;    /* heif_chroma_downsampling_algorithm: 1 nearest neighbour, 2 average (libheif's default), 3 sharp YUV */
+  int only_use_preferred;     /* only_use_preferred_chroma_algorithm */
+} b200_rgb_to_ycbcr_options;
+
+/* *pipeline of the calls below: the reference operations of the chain (bit mask) */
+#define B200_YCC_PIPE_RGB24_32 1     /* Op_RGB24_32_to_YCbCr */
+#define B200_YCC_PIPE_GBR444 2       /* Op_RGB24_32_to_YCbCr444_GBR */
+#define B200_YCC_PIPE_HDR420 4       /* Op_RRGGBBxx_HDR_to_YCbCr420 */
+#define B200_YCC_PIPE_PLANAR 8       /* Op_RGB_to_YCbCr<T> */
+#define B200_YCC_PIPE_UNPACK 16      /* Op_RGB24_32_to_RGB / Op_RRGGBBaa_BE_to_RGB_HDR before it */
+#define B200_YCC_PIPE_SWAP 32        /* Op_RRGGBBaa_swap_endianness before that */
+
+/* Host only, no CUDA: the chain the reference would run, or the refusal the conversion would return.
+   `out`: width / height (= the input's) / chroma (B200_CHROMA_420 / 422 / 444) / bit_depth (= the input's) / colour_primaries /
+   matrix_coefficients / full_range are read (nclx "unspecified" (2) -> matrix 6 / primaries 1, colorconversion.cc:567-573).
+   opt NULL = libheif's defaults (average, not only preferred).
+   B200_E_UNSUPPORTED: matrix_coefficients 11 or 14 (the reference has no chain either); a planar alpha plane whose depth
+   differs from the colour depth (the reference adds Op_adjust_alpha_bit_depth: not mirrored); only_use_preferred with
+   average or sharp-YUV downsampling to 4:2:0 / 4:2:2 (the reference then converts to 4:4:4 and downsamples with
+   Op_YCbCr444_to_YCbCr420/422_average, or has no chain: not mirrored). */
+int b200_rgb_to_ycbcr_plan(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, int* pipeline);
+/* Device -> device.  `out` as above, plus the caller-owned planes (uint8 at 8 bit, native uint16 above), written through the
+   const-declared pointers; out->alpha is required exactly when the input has alpha (the result has an alpha plane then,
+   colorconversion.cc:575-585) and receives it unchanged.  pipeline may be NULL. */
+int b200_rgb_to_ycbcr_ex_device(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, void* stream, int* pipeline);
+/* Host -> host form: stages its operands with the buffers of b200_rgb_to_ycbcr_host. */
+int b200_rgb_to_ycbcr_ex_host(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, int* pipeline);
+
 /* nclx helper: the 4 float coefficients exactly as nclx.cc:84-173 derives them */
 void b200_ycbcr_to_rgb_coefficients(int matrix_coefficients, int colour_primaries, float out_coeffs[4] /* r_cr,g_cb,g_cr,b_cb */);
 

@@ -6,6 +6,7 @@ PyTorch is used only for device memory, streams and torch.distributed plumbing.
 """
 from ._lib import lib, B200Error, SO_PATH  # noqa: F401
 from .color import (Geometry, YCbCrImage, convert_colorspace, convert_colorspace_host, rgb_to_ycbcr, rgb_to_ycbcr_host,  # noqa: F401
+                    rgb_to_ycbcr_ex, rgb_to_ycbcr_ex_host, rgb_to_ycbcr_plan, YCC_PIPE_NAMES,
                     CHROMA_420, CHROMA_422, CHROMA_444, CHROMA_MONO, CHROMA_INTERLEAVED_RGB, CHROMA_INTERLEAVED_RGBA,
                     CHROMA_INTERLEAVED_RRGGBB_BE, CHROMA_INTERLEAVED_RRGGBBAA_BE, CHROMA_INTERLEAVED_RRGGBB_LE,
                     CHROMA_INTERLEAVED_RRGGBBAA_LE)

@@ -22,6 +22,17 @@ class Geometry(C.Structure):
                 ("pre", C.c_int * 6), ("pre_w", C.c_int), ("pre_h", C.c_int)]
 
 
+class RgbImage(C.Structure):
+    _fields_ = [("rgb", C.c_void_p), ("rgb_stride", C.c_size_t), ("r", C.c_void_p), ("g", C.c_void_p), ("b", C.c_void_p),
+                ("alpha", C.c_void_p), ("r_stride", C.c_size_t), ("g_stride", C.c_size_t), ("b_stride", C.c_size_t),
+                ("alpha_stride", C.c_size_t), ("width", C.c_int), ("height", C.c_int), ("chroma", C.c_int), ("bit_depth", C.c_int),
+                ("alpha_bit_depth", C.c_int)]
+
+
+class RgbToYCbCrOptions(C.Structure):
+    _fields_ = [("chroma_downsampling", C.c_int), ("only_use_preferred", C.c_int)]
+
+
 class ColorOptions(C.Structure):
     _fields_ = [("out_chroma", C.c_int), ("out_bit_depth", C.c_int), ("chroma_upsampling", C.c_int)]
 
@@ -59,6 +70,10 @@ def lib():
         _lib.b200_ycbcr_to_rgb_coefficients.restype = None
         _lib.b200_rgb_to_ycbcr_device.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(Planes), C.c_void_p]
         _lib.b200_rgb_to_ycbcr_host.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.POINTER(Planes)]
+        _lib.b200_rgb_to_ycbcr_plan.argtypes = [C.POINTER(RgbImage), C.POINTER(Planes), C.POINTER(RgbToYCbCrOptions), C.POINTER(C.c_int)]
+        _lib.b200_rgb_to_ycbcr_ex_device.argtypes = [C.POINTER(RgbImage), C.POINTER(Planes), C.POINTER(RgbToYCbCrOptions), C.c_void_p,
+                                                     C.POINTER(C.c_int)]
+        _lib.b200_rgb_to_ycbcr_ex_host.argtypes = [C.POINTER(RgbImage), C.POINTER(Planes), C.POINTER(RgbToYCbCrOptions), C.POINTER(C.c_int)]
     return _lib
 
 

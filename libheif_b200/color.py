@@ -176,3 +176,137 @@ def rgb_to_ycbcr_host(rgb: np.ndarray, out_chroma: int = CHROMA_420, matrix_coef
     planes = _fill_planes(img, lambda x: x.ctypes.data, lambda x: x.strides[0])
     _lib.check(_lib.lib().b200_rgb_to_ycbcr_host(C.c_void_p(rgb.ctypes.data), C.c_size_t(rgb.strides[0]), int(bpp == 4), C.byref(planes)))
     return img
+
+
+# ---- every RGB layout heif_context_encode_image accepts (b200_rgb_to_ycbcr_ex_*) ----------------------------------------
+# names of the reference operations behind the B200_YCC_PIPE_* bits, in chain order
+YCC_PIPE_NAMES = ((32, "Op_RRGGBBaa_swap_endianness"), (16, "Op_RRGGBBaa_BE_to_RGB_HDR / Op_RGB24_32_to_RGB"),
+                  (1, "Op_RGB24_32_to_YCbCr"), (2, "Op_RGB24_32_to_YCbCr444_GBR"), (4, "Op_RRGGBBxx_HDR_to_YCbCr420"),
+                  (8, "Op_RGB_to_YCbCr"))
+
+
+def _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, ptr, stride, is16, packed):
+    """b200_rgb_image for an interleaved [H, W, 3|4] array / tensor or a tuple (R, G, B[, A]) of [H, W] planes.
+    packed(a): the samples of a row (and the components of a pixel) are adjacent in memory."""
+    d = _lib.RgbImage()
+    if isinstance(rgb, (tuple, list)):
+        if len(rgb) not in (3, 4) or any(p.ndim != 2 or p.shape != rgb[0].shape or not packed(p) for p in rgb):
+            raise ValueError("planar input: 3 or 4 [H, W] planes of one size, samples adjacent within a row")
+        if is16(rgb[0]) and bit_depth is None:
+            raise ValueError("16-bit planes need bit_depth (9..16)")
+        depth, adepth = bit_depth or 8, alpha_bit_depth or bit_depth or 8
+        if any(is16(p) != (depth > 8) for p in rgb[:3]) or (len(rgb) == 4 and is16(rgb[3]) != (adepth > 8)):
+            raise ValueError("planar input: uint8 planes at 8 bit, uint16 above (alpha at alpha_bit_depth)")
+        d.r, d.g, d.b = ptr(rgb[0]), ptr(rgb[1]), ptr(rgb[2])
+        d.r_stride, d.g_stride, d.b_stride = stride(rgb[0]), stride(rgb[1]), stride(rgb[2])
+        if len(rgb) == 4:
+            d.alpha, d.alpha_stride = ptr(rgb[3]), stride(rgb[3])
+        d.height, d.width = rgb[0].shape
+        d.chroma = CHROMA_444
+        d.bit_depth = bit_depth or 8
+        d.alpha_bit_depth = alpha_bit_depth or 0
+        return d, len(rgb) == 4
+    if rgb.ndim != 3 or rgb.shape[2] not in (3, 4) or not packed(rgb):
+        raise ValueError("interleaved input: [H, W, 3 or 4], pixels and their components adjacent within a row")
+    h, w, nch = rgb.shape
+    if is16(rgb):
+        if endianness not in ("little", "big") or bit_depth is None:
+            raise ValueError("16-bit interleaved input needs endianness ('little' / 'big': the byte order of the samples as stored) and bit_depth")
+        d.chroma = {(3, "big"): CHROMA_INTERLEAVED_RRGGBB_BE, (4, "big"): CHROMA_INTERLEAVED_RRGGBBAA_BE,
+                    (3, "little"): CHROMA_INTERLEAVED_RRGGBB_LE, (4, "little"): CHROMA_INTERLEAVED_RRGGBBAA_LE}[(nch, endianness)]
+        d.bit_depth = bit_depth
+    else:
+        if bit_depth not in (None, 8):
+            raise ValueError("uint8 interleaved input is RGB / RGBA at 8 bit")
+        d.chroma = CHROMA_INTERLEAVED_RGB if nch == 3 else CHROMA_INTERLEAVED_RGBA
+        d.bit_depth = 8
+    d.rgb, d.rgb_stride = ptr(rgb), stride(rgb)
+    d.width, d.height = w, h
+    return d, nch == 4
+
+
+def _ycc_target(img_planes, w, h, out_chroma, bit_depth, mc, cp, full):
+    p = _lib.Planes()
+    if img_planes is not None:
+        y, cb, cr, a, ptr, stride = img_planes
+        p.y, p.cb, p.cr = ptr(y), ptr(cb), ptr(cr)
+        p.y_stride, p.c_stride = stride(y), stride(cb)
+        if a is not None:
+            p.alpha, p.alpha_stride = ptr(a), stride(a)
+    p.width, p.height, p.chroma, p.bit_depth = w, h, out_chroma, bit_depth
+    p.colour_primaries, p.transfer_characteristics, p.matrix_coefficients, p.full_range = cp, 2, mc, int(bool(full))
+    return p
+
+
+def _np_is16(a):
+    if a.dtype not in (np.uint8, np.uint16):
+        raise ValueError("uint8 / uint16 arrays only")
+    return a.dtype == np.uint16
+
+
+def _np_packed(a):
+    return a.strides[-1] == a.itemsize and (a.ndim == 2 or a.strides[1] == a.shape[2] * a.itemsize)
+
+
+def rgb_to_ycbcr_plan(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[int] = None, endianness: Optional[str] = None,
+                      matrix_coefficients: int = 6, colour_primaries: int = 1, full_range: bool = True, chroma_downsampling: int = 2,
+                      only_use_preferred: bool = False, alpha_bit_depth: Optional[int] = None) -> int:
+    """Host only: the B200_YCC_PIPE_* mask of the reference chain for this input (numpy arrays, arguments as for
+    rgb_to_ycbcr_ex; no pixel is read); raises B200Error (code -2) where the conversion is refused."""
+    d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda a: a.ctypes.data, lambda a: a.strides[0], _np_is16, _np_packed)
+    t = _ycc_target(None, d.width, d.height, out_chroma, d.bit_depth, matrix_coefficients, colour_primaries, full_range)
+    opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
+    pipe = C.c_int(0)
+    _lib.check(_lib.lib().b200_rgb_to_ycbcr_plan(C.byref(d), C.byref(t), C.byref(opt), C.byref(pipe)))
+    return pipe.value
+
+
+def rgb_to_ycbcr_ex(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[int] = None, endianness: Optional[str] = None,
+                    matrix_coefficients: int = 6, colour_primaries: int = 1, full_range: bool = True, chroma_downsampling: int = 2,
+                    only_use_preferred: bool = False, alpha_bit_depth: Optional[int] = None, stream=None):
+    """Encoder-side direction for every RGB layout, device -> device (b200_rgb_to_ycbcr_ex_device): what convert_colorspace
+    does before heif_context_encode_image hands the picture to an encoder (libheif/codecs/encoder.cc:116-175).
+
+    rgb: CUDA tensor [H, W, 3|4] (uint8: RGB / RGBA 8 bit; uint16: RRGGBB[AA], with `endianness` naming the byte order the
+    samples are stored in and `bit_depth` 9..16), or a tuple (R, G, B[, A]) of [H, W] planes (uint8, or uint16 with bit_depth).
+    Returns (YCbCrImage at the input depth -- uint16 planes above 8 bit, an alpha plane when the input has one --,
+    B200_YCC_PIPE_* mask of the reference chain that was mirrored)."""
+    import torch
+    first = rgb[0] if isinstance(rgb, (tuple, list)) else rgb
+    for t in (rgb if isinstance(rgb, (tuple, list)) else (rgb,)):
+        if t.device != first.device or t.device.type != "cuda" or t.dtype not in (torch.uint8, torch.uint16):
+            raise ValueError("rgb_to_ycbcr_ex: uint8 / uint16 CUDA tensors on one device")
+    is16 = lambda t: t.element_size() == 2   # noqa: E731
+    packed = lambda t: t.stride(-1) == 1 and (t.dim() == 2 or t.stride(1) == t.shape[2])   # noqa: E731
+    d, has_alpha = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda t: t.data_ptr(),
+                              lambda t: t.stride(0) * t.element_size(), is16, packed)
+    tdt = torch.uint16 if d.bit_depth > 8 else torch.uint8
+    y, cb, cr, a = _ycc_out_planes(d.width, d.height, out_chroma, has_alpha, lambda s: torch.empty(s, dtype=tdt, device=first.device))
+    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=d.bit_depth, colour_primaries=colour_primaries,
+                     matrix_coefficients=matrix_coefficients, full_range=full_range)
+    t = _ycc_target((y, cb, cr, a, lambda x: x.data_ptr(), lambda x: x.stride(0) * x.element_size()), d.width, d.height, out_chroma,
+                    d.bit_depth, matrix_coefficients, colour_primaries, full_range)
+    opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
+    pipe = C.c_int(0)
+    s = stream if stream is not None else torch.cuda.current_stream(first.device)
+    with torch.cuda.device(first.device):
+        _lib.check(_lib.lib().b200_rgb_to_ycbcr_ex_device(C.byref(d), C.byref(t), C.byref(opt), C.c_void_p(s.cuda_stream), C.byref(pipe)))
+    return img, pipe.value
+
+
+def rgb_to_ycbcr_ex_host(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[int] = None, endianness: Optional[str] = None,
+                         matrix_coefficients: int = 6, colour_primaries: int = 1, full_range: bool = True, chroma_downsampling: int = 2,
+                         only_use_preferred: bool = False, alpha_bit_depth: Optional[int] = None):
+    """Host -> host form of rgb_to_ycbcr_ex (b200_rgb_to_ycbcr_ex_host: H2D + kernel + D2H inside the call); numpy input,
+    rows may be strided."""
+    d, has_alpha = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda a: a.ctypes.data, lambda a: a.strides[0], _np_is16, _np_packed)
+    dt = np.uint16 if d.bit_depth > 8 else np.uint8
+    y, cb, cr, a = _ycc_out_planes(d.width, d.height, out_chroma, has_alpha, lambda s: np.empty(s, dt))
+    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=d.bit_depth, colour_primaries=colour_primaries,
+                     matrix_coefficients=matrix_coefficients, full_range=full_range)
+    t = _ycc_target((y, cb, cr, a, lambda x: x.ctypes.data, lambda x: x.strides[0]), d.width, d.height, out_chroma, d.bit_depth,
+                    matrix_coefficients, colour_primaries, full_range)
+    opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
+    pipe = C.c_int(0)
+    _lib.check(_lib.lib().b200_rgb_to_ycbcr_ex_host(C.byref(d), C.byref(t), C.byref(opt), C.byref(pipe)))
+    return img, pipe.value

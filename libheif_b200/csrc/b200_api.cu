@@ -207,4 +207,64 @@ int b200_rgb_to_ycbcr_host(const void* rgb, size_t rgb_stride, int has_alpha, co
   return finish(*X, rc);
 }
 
+int b200_rgb_to_ycbcr_plan(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, int* pipeline) {
+  return plan_rgb_to_ycbcr(in, out, opt, pipeline);
+}
+
+int b200_rgb_to_ycbcr_ex_device(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, void* stream, int* pipeline) {
+  return launch_rgb_to_ycbcr_ex(in, out, opt, (cudaStream_t)stream, pipeline);
+}
+
+int b200_rgb_to_ycbcr_ex_host(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, int* pipeline) {
+  int rc = plan_rgb_to_ycbcr(in, out, opt, pipeline);         // refusals before any staging
+  if (rc) return rc;
+  if (!out->y || !out->cb || !out->cr) return set_error(B200_E_INVALID, "RGB -> YCbCr: output planes missing");
+  if (out->width <= 0 || out->height <= 0) return B200_OK;
+  const bool planar = in->chroma == B200_CHROMA_444;
+  const int w = out->width, h = out->height, bps = in->bit_depth > 8 ? 2 : 1;
+  int nch;
+  switch (in->chroma) {
+    case B200_CHROMA_INTERLEAVED_RGB: nch = 3; break;
+    case B200_CHROMA_INTERLEAVED_RGBA: nch = 4; break;
+    case B200_CHROMA_INTERLEAVED_RRGGBB_BE: case B200_CHROMA_INTERLEAVED_RRGGBB_LE: nch = 3; break;
+    default: nch = planar ? 1 : 4;
+  }
+  const int nin = planar ? (in->alpha ? 4 : 3) : 1;
+  const void* src[4] = {planar ? in->r : in->rgb, in->g, in->b, in->alpha};
+  const size_t sstride[4] = {planar ? in->r_stride : in->rgb_stride, in->g_stride, in->b_stride, in->alpha_stride};
+  const int sh = out->chroma == B200_CHROMA_444 ? 0 : 1, sv = out->chroma == B200_CHROMA_420 ? 1 : 0;
+  const int cw = (w + sh) >> sh, ch = (h + sv) >> sv;
+  const size_t irow = (size_t)w * nch * bps, ipitch = (irow + 255) & ~(size_t)255;
+  // the caller's rows are read on the host: every stride is checked before anything is staged
+  for (int c = 0; c < nin; c++) {
+    if (!src[c]) return set_error(B200_E_INVALID, "RGB input planes missing");
+    if (sstride[c] < irow) return set_error(B200_E_INVALID, "RGB input plane %d: stride %zu < row of %zu bytes", c, sstride[c], irow);
+  }
+  if (out->y_stride < (size_t)w * bps || out->c_stride < (size_t)cw * bps || (out->alpha && out->alpha_stride < (size_t)w * bps))
+    return set_error(B200_E_INVALID, "YCbCr output stride smaller than a row");
+  const size_t ypitch = (((size_t)w * bps) + 255) & ~(size_t)255, cpitch = (((size_t)cw * bps) + 255) & ~(size_t)255;
+  const size_t ibytes = ipitch * (size_t)h, ybytes = ypitch * (size_t)h, cbytes = cpitch * (size_t)ch, abytes = out->alpha ? ybytes : 0;
+  std::lock_guard<std::mutex> lock(g_xfer_mu);
+  HostXfer* X = nullptr;
+  if ((rc = host_xfer(&X)) || (rc = X->dev.reserve(ibytes * nin + ybytes + 2 * cbytes + abytes, false))) return rc;
+  char* din = X->dev.d; char* dy = din + ibytes * nin; char* dcb = dy + ybytes; char* dcr = dcb + cbytes; char* da = out->alpha ? dcr + cbytes : nullptr;
+  Pool& pool = copy_pool();
+  for (int c = 0; c < nin && rc == B200_OK; c++) rc = X->bounce.upload(din + (size_t)c * ibytes, ipitch, src[c], sstride[c], irow, (size_t)h, X->s, pool);
+  if (rc == B200_OK) {
+    b200_rgb_image d = *in;
+    if (planar) {
+      d.r = din; d.g = din + ibytes; d.b = din + 2 * ibytes; d.alpha = in->alpha ? din + 3 * ibytes : nullptr;
+      d.r_stride = d.g_stride = d.b_stride = d.alpha_stride = ipitch;
+    } else { d.rgb = din; d.rgb_stride = ipitch; }
+    b200_planes o = *out;
+    o.y = dy; o.cb = dcb; o.cr = dcr; o.alpha = da; o.y_stride = ypitch; o.c_stride = cpitch; o.alpha_stride = ypitch;
+    rc = launch_rgb_to_ycbcr_ex(&d, &o, opt, X->s, pipeline);
+  }
+  if (rc == B200_OK) rc = X->bounce.download((void*)out->y, out->y_stride, dy, ypitch, (size_t)w * bps, (size_t)h, X->s, pool);
+  if (rc == B200_OK) rc = X->bounce.download((void*)out->cb, out->c_stride, dcb, cpitch, (size_t)cw * bps, (size_t)ch, X->s, pool);
+  if (rc == B200_OK) rc = X->bounce.download((void*)out->cr, out->c_stride, dcr, cpitch, (size_t)cw * bps, (size_t)ch, X->s, pool);
+  if (out->alpha && rc == B200_OK) rc = X->bounce.download((void*)out->alpha, out->alpha_stride, da, ypitch, (size_t)w * bps, (size_t)h, X->s, pool);
+  return finish(*X, rc);
+}
+
 }  // extern "C"

@@ -803,5 +803,280 @@ int launch_rgb_to_ycbcr(const void* rgb, size_t rgb_stride, int has_alpha, const
   return B200_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Encoder-side colour ops for the other RGB layouts: one kernel, templated on the sample type T (uint8 / uint16, the same
+// for input and output, as the reference ops keep the depth), the loader (interleaved RGB[A] 8 bit / RRGGBB[AA] BE or LE,
+// or planar R, G, B[, A]) and the arithmetic of one reference op:
+//   YCC_HDR420  Op_RRGGBBxx_HDR_to_YCbCr420   rgb2yuv.cc:366-503  (full range, 4:2:0 only)
+//   YCC_PLANAR  Op_RGB_to_YCbCr<T>            rgb2yuv.cc:100-305  (behind the lossless Op_RRGGBBaa_swap_endianness /
+//               Op_RRGGBBaa_BE_to_RGB_HDR / Op_RGB24_32_to_RGB steps of the chain, which the loader folds in)
+//   YCC_GBR444  Op_RGB24_32_to_YCbCr444_GBR   rgb2yuv.cc:850-919
+// Every chroma value of these ops is a float sum of whole samples (exact in float) times 0.25, or one sample, so one thread
+// converts a 2 x 2 pixel block and computes its chroma from the block: pairs of samples come in as 16- / 32-bit loads
+// (interleaved 16 bit: 12- or 16-byte loads) and luma / alpha leave as pairs when the rows are aligned.
+// ---------------------------------------------------------------------------------------------------------------
+enum { YCC_HDR420 = 0, YCC_PLANAR = 1, YCC_GBR444 = 2 };
+struct RgbExArgs {
+  const uint8_t* in[4]; long long is[4];       // interleaved: in[0]; planar: R, G, B, A
+  uint8_t *y, *cb, *cr, *a; long long ys, cs, as;
+  int w, h, sh, sv, nch, le, full, bpp, mc, vec_in, vec_out;
+  float c[3][3];
+};
+
+template <typename T, bool PLANAR_IN>
+__device__ __forceinline__ void load_pair(const RgbExArgs& p, int x0, int y, int n, int v[2][4]) {
+  if (PLANAR_IN) {
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+      if (c == 3 && !p.a) break;
+      const T* row = reinterpret_cast<const T*>(p.in[c] + (long long)y * p.is[c]) + x0;
+      if (p.vec_in && n == 2) {
+        if (sizeof(T) == 1) { const unsigned q = __ldg(reinterpret_cast<const unsigned short*>(row)); v[0][c] = q & 0xff; v[1][c] = q >> 8; }
+        else { const unsigned q = __ldg(reinterpret_cast<const unsigned*>(row)); v[0][c] = q & 0xffff; v[1][c] = q >> 16; }
+      } else {
+        v[0][c] = __ldg(row);
+        if (n == 2) v[1][c] = __ldg(row + 1);
+      }
+    }
+    return;
+  }
+  // the (up to) 16 bytes of the pair in four registers; bytes are picked with selects, not an indexed local array
+  const int bpp = p.nch * (int)sizeof(T);
+  const uint8_t* row = p.in[0] + (long long)y * p.is[0] + (long long)x0 * bpp;
+  unsigned wd[4] = {0, 0, 0, 0};
+  if (sizeof(T) == 2 && p.vec_in && n == 2) {
+    if (p.nch == 4) { const uint4 q = __ldg(reinterpret_cast<const uint4*>(row)); wd[0] = q.x; wd[1] = q.y; wd[2] = q.z; wd[3] = q.w; }
+    else {
+#pragma unroll
+      for (int k = 0; k < 3; k++) wd[k] = __ldg(reinterpret_cast<const unsigned*>(row) + k);
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < 16; k++) if (k < n * bpp) wd[k >> 2] |= (unsigned)__ldg(row + k) << ((k & 3) * 8);
+  }
+  auto byte_at = [&](int k) -> int {
+    const unsigned w = k < 4 ? wd[0] : (k < 8 ? wd[1] : (k < 12 ? wd[2] : wd[3]));
+    return (w >> ((k & 3) * 8)) & 0xff;
+  };
+#pragma unroll
+  for (int i = 0; i < 2; i++) {
+    if (i >= n) break;
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+      if (c >= p.nch) break;
+      const int k = i * bpp + c * (int)sizeof(T);
+      v[i][c] = sizeof(T) == 1 ? byte_at(k) : ((byte_at(k + p.le) << 8) | byte_at(k + 1 - p.le));   // rgb2yuv.cc:443-445, rgb2rgb.cc:464-
+    }
+  }
+}
+
+__device__ __forceinline__ float dot3f(float r, float g, float b, const float* c) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(r, c[0]), __fmul_rn(g, c[1])), __fmul_rn(b, c[2]));
+}
+__device__ __forceinline__ float scale_256(float v, float f) { return __fdiv_rn(__fmul_rn(v, f), 256.0f); }   // (v * f) / 256
+
+template <int ARITH>
+__device__ __forceinline__ int luma_ex(const RgbExArgs& p, int r, int g, int b) {
+  const int maxv = (1 << p.bpp) - 1;
+  if (ARITH == YCC_GBR444) return g;
+  if (ARITH == YCC_PLANAR && p.mc == 0) {                                     // rgb2yuv.cc:198-206
+    if (p.full) return g;
+    return clip_round(__fadd_rn(scale_256((float)g, 219.0f), (float)(16 << (p.bpp - 8))), maxv);
+  }
+  if (ARITH == YCC_PLANAR && p.mc == 8) return g / 2 + (r + b) / 4;            // :207-211
+  float v = dot3f((float)r, (float)g, (float)b, p.c[0]);                      // :213-222, :443-453
+  if (ARITH == YCC_PLANAR && !p.full) v = __fadd_rn(scale_256(v, 219.0f), (float)(16 << (p.bpp - 8)));
+  return clip_round(v, maxv);
+}
+
+// s: the sample (GBR / matrix 0 / 8: the block's top-left pixel) or, for the matrix ops, the sum of the four quad samples
+template <int ARITH>
+__device__ __forceinline__ void chroma_ex(const RgbExArgs& p, const int s[3], bool sum4, int& cb, int& cr) {
+  const int maxv = (1 << p.bpp) - 1, half = 1 << (p.bpp - 1);
+  const int r = s[0], g = s[1], b = s[2];
+  if (ARITH == YCC_GBR444 || (ARITH == YCC_PLANAR && p.mc == 0 && p.full)) { cb = b; cr = r; return; }
+  if (ARITH == YCC_PLANAR && p.mc == 0) {                                                   // rgb2yuv.cc:237-240
+    const float off = (float)(16 << (p.bpp - 8));
+    cb = clip_round(__fadd_rn(scale_256((float)b, 224.0f), off), maxv);
+    cr = clip_round(__fadd_rn(scale_256((float)r, 224.0f), off), maxv);
+    return;
+  }
+  if (ARITH == YCC_PLANAR && p.mc == 8) {                                                   // :246-250 (C division)
+    const int u = g / 2 - (r + b) / 4 + half, w = (r - b) / 2 + half;
+    cb = u < 0 ? 0 : (u > maxv ? maxv : u); cr = w < 0 ? 0 : (w > maxv ? maxv : w);
+    return;
+  }
+  float rf = (float)r, gf = (float)g, bf = (float)b;
+  if (sum4) { rf = __fmul_rn(rf, 0.25f); gf = __fmul_rn(gf, 0.25f); bf = __fmul_rn(bf, 0.25f); }     // :273-275, :485-487
+  float u = dot3f(rf, gf, bf, p.c[1]), w = dot3f(rf, gf, bf, p.c[2]);
+  if (ARITH == YCC_PLANAR && !p.full) { u = scale_256(u, 224.0f); w = scale_256(w, 224.0f); }      // :283-286
+  cb = clip_round(__fadd_rn(u, (float)half), maxv);
+  cr = clip_round(__fadd_rn(w, (float)half), maxv);
+}
+
+template <typename T>
+__device__ __forceinline__ void store_pair(uint8_t* plane, long long stride, int x0, int y, int n, int v0, int v1, bool vec) {
+  T* row = reinterpret_cast<T*>(plane + (long long)y * stride) + x0;
+  if (vec && n == 2) {
+    if (sizeof(T) == 1) *reinterpret_cast<unsigned short*>(row) = (unsigned short)(v0 | (v1 << 8));
+    else *reinterpret_cast<unsigned*>(row) = (unsigned)v0 | ((unsigned)v1 << 16);
+  } else {
+    row[0] = (T)v0;
+    if (n == 2) row[1] = (T)v1;
+  }
+}
+
+template <typename T, bool PLANAR_IN, int ARITH>
+__global__ void __launch_bounds__(256) rgb_to_ycbcr_ex_kernel(const RgbExArgs p) {
+  const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 2, y0 = (blockIdx.y * blockDim.y + threadIdx.y) * 2;
+  if (x0 >= p.w || y0 >= p.h) return;
+  const int nx = min(2, p.w - x0), ny = min(2, p.h - y0);
+  int v[2][2][4];
+#pragma unroll
+  for (int j = 0; j < 2; j++) {
+    if (j < ny) load_pair<T, PLANAR_IN>(p, x0, y0 + j, nx, v[j]);
+  }
+  const bool vo = p.vec_out != 0;
+#pragma unroll
+  for (int j = 0; j < 2; j++) {
+    if (j >= ny) break;
+    int l[2] = {0, 0};
+#pragma unroll
+    for (int i = 0; i < 2; i++) if (i < nx) l[i] = luma_ex<ARITH>(p, v[j][i][0], v[j][i][1], v[j][i][2]);
+    store_pair<T>(p.y, p.ys, x0, y0 + j, nx, l[0], l[1], vo);
+    if (p.a) store_pair<T>(p.a, p.as, x0, y0 + j, nx, v[j][0][3], nx == 2 ? v[j][1][3] : 0, vo);   // alpha copied (:295-302, :455-458)
+  }
+  int cb, cr;
+  if (p.sh == 0) {                                                                // 4:4:4: every pixel
+#pragma unroll
+    for (int j = 0; j < 2; j++) {
+      if (j >= ny) break;
+      int b2[2] = {0, 0}, r2[2] = {0, 0};
+#pragma unroll
+      for (int i = 0; i < 2; i++) if (i < nx) { chroma_ex<ARITH>(p, v[j][i], false, b2[i], r2[i]); }
+      store_pair<T>(p.cb, p.cs, x0, y0 + j, nx, b2[0], b2[1], vo);
+      store_pair<T>(p.cr, p.cs, x0, y0 + j, nx, r2[0], r2[1], vo);
+    }
+  } else if (p.sv == 0) {
+    // 4:2:2: x2 = x and y2 = y (rgb2yuv.cc:258-259), so the float "mean" is 4 x the left pixel x 0.25 = the left pixel, exactly
+#pragma unroll
+    for (int j = 0; j < 2; j++) {
+      if (j >= ny) break;
+      chroma_ex<ARITH>(p, v[j][0], false, cb, cr);
+      reinterpret_cast<T*>(p.cb + (long long)(y0 + j) * p.cs)[x0 >> 1] = (T)cb;
+      reinterpret_cast<T*>(p.cr + (long long)(y0 + j) * p.cs)[x0 >> 1] = (T)cr;
+    }
+  } else {                                                                        // 4:2:0: the quad, edge samples repeated
+    const bool special = ARITH == YCC_PLANAR && (p.mc == 0 || p.mc == 8);
+    int s[3];
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      const int a00 = v[0][0][c], a01 = nx == 2 ? v[0][1][c] : a00, a10 = ny == 2 ? v[1][0][c] : a00, a11 = ny == 2 ? (nx == 2 ? v[1][1][c] : a10) : a01;
+      s[c] = special ? a00 : a00 + a01 + a10 + a11;
+    }
+    chroma_ex<ARITH>(p, s, !special, cb, cr);
+    reinterpret_cast<T*>(p.cb + (long long)(y0 >> 1) * p.cs)[x0 >> 1] = (T)cb;
+    reinterpret_cast<T*>(p.cr + (long long)(y0 >> 1) * p.cs)[x0 >> 1] = (T)cr;
+  }
+}
+
+static bool rgb_interleaved(int chroma) { return chroma >= B200_CHROMA_INTERLEAVED_RGB && chroma <= B200_CHROMA_INTERLEAVED_RRGGBBAA_LE; }
+static bool rgb_has_alpha(const b200_rgb_image* in) {
+  return in->chroma == B200_CHROMA_INTERLEAVED_RGBA || in->chroma == B200_CHROMA_INTERLEAVED_RRGGBBAA_BE ||
+         in->chroma == B200_CHROMA_INTERLEAVED_RRGGBBAA_LE || (in->chroma == B200_CHROMA_444 && in->alpha != nullptr);
+}
+
+// The chain the reference planner (colorconversion.cc:279-435) finds from this RGB input to `out`'s YCbCr state at the input
+// depth, with convert_colorspace's target (colorconversion.cc:530-611); tabulated from its operations' state_after_conversion
+// (rgb2yuv.cc:30-98, :311-363, :506-553, :812-847, rgb2rgb.cc) and pinned by tests/test_rgb_to_ycbcr_ex_plan.py.
+int plan_rgb_to_ycbcr(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, int* pipeline) {
+  if (pipeline) *pipeline = 0;
+  if (!in || !out) return set_error(B200_E_INVALID, "null argument");
+  const int ic = in->chroma, bd = in->bit_depth;
+  const bool inter = rgb_interleaved(ic), inter8 = ic == B200_CHROMA_INTERLEAVED_RGB || ic == B200_CHROMA_INTERLEAVED_RGBA;
+  if (!inter && ic != B200_CHROMA_444) return set_error(B200_E_INVALID, "RGB input chroma %d", ic);
+  if (inter8 ? bd != 8 : (bd < (inter ? 9 : 8) || bd > 16)) return set_error(B200_E_INVALID, "RGB input chroma %d with bit depth %d", ic, bd);
+  if (out->chroma != B200_CHROMA_420 && out->chroma != B200_CHROMA_422 && out->chroma != B200_CHROMA_444)
+    return set_error(B200_E_UNSUPPORTED, "RGB -> YCbCr: target chroma %d", out->chroma);
+  if (out->bit_depth != bd) return set_error(B200_E_INVALID, "target bit depth %d: the conversion keeps the input's %d", out->bit_depth, bd);
+  if (out->width != in->width || out->height != in->height) return set_error(B200_E_INVALID, "target size differs from the input's");
+  const int mc = out->matrix_coefficients;
+  if (mc == 11 || mc == 14) return set_error(B200_E_UNSUPPORTED, "matrix_coefficients %d: no RGB -> YCbCr operation of the reference takes it (rgb2yuv.cc:57-60)", mc);
+  if (ic == B200_CHROMA_444 && in->alpha && in->alpha_bit_depth && in->alpha_bit_depth != bd)
+    return set_error(B200_E_UNSUPPORTED, "alpha depth %d differs from the colour depth %d (the reference inserts Op_adjust_alpha_bit_depth)", in->alpha_bit_depth, bd);
+  const int ds = opt ? opt->chroma_downsampling : 2;
+  if (out->chroma != B200_CHROMA_444 && opt && opt->only_use_preferred && ds != 1)
+    return set_error(B200_E_UNSUPPORTED, "only_use_preferred_chroma_algorithm with downsampling %d: the reference converts to 4:4:4 and "
+                                         "downsamples with a separate operation (or has no chain)", ds);
+  const bool full = out->full_range != 0, special = mc == 0 || mc == 8;
+  int pipe;
+  if (inter8) pipe = !special ? B200_YCC_PIPE_RGB24_32 : (mc == 0 && full && out->chroma == B200_CHROMA_444) ? B200_YCC_PIPE_GBR444 : B200_YCC_PIPE_UNPACK | B200_YCC_PIPE_PLANAR;
+  else if (inter) {
+    const bool le = ic == B200_CHROMA_INTERLEAVED_RRGGBB_LE || ic == B200_CHROMA_INTERLEAVED_RRGGBBAA_LE;
+    pipe = (full && out->chroma == B200_CHROMA_420 && !special) ? B200_YCC_PIPE_HDR420 : (le ? B200_YCC_PIPE_SWAP : 0) | B200_YCC_PIPE_UNPACK | B200_YCC_PIPE_PLANAR;
+  } else pipe = B200_YCC_PIPE_PLANAR;
+  if (pipeline) *pipeline = pipe;
+  return B200_OK;
+}
+
+int launch_rgb_to_ycbcr_ex(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, cudaStream_t stream, int* pipeline) {
+  int pipe = 0;
+  int rc = plan_rgb_to_ycbcr(in, out, opt, &pipe);
+  if (rc) return rc;
+  if (pipeline) *pipeline = pipe;
+  const bool has_alpha = rgb_has_alpha(in);
+  if (!out->y || !out->cb || !out->cr) return set_error(B200_E_INVALID, "RGB -> YCbCr: output planes missing");
+  if (has_alpha != (out->alpha != nullptr))
+    return set_error(B200_E_INVALID, "the result has an alpha plane exactly when the input has one (colorconversion.cc:575-585)");
+  const bool inter = rgb_interleaved(in->chroma);
+  if (inter ? !in->rgb : (!in->r || !in->g || !in->b)) return set_error(B200_E_INVALID, "RGB input planes missing");
+  if (pipe == B200_YCC_PIPE_RGB24_32) return launch_rgb_to_ycbcr(in->rgb, in->rgb_stride, has_alpha, out, stream);
+  if (out->width <= 0 || out->height <= 0) return B200_OK;
+  RgbExArgs a{};
+  const int bps = in->bit_depth > 8 ? 2 : 1;
+  a.nch = inter ? (has_alpha ? 4 : 3) : 1;
+  uintptr_t ai = 0;
+  if (inter) {
+    if (in->rgb_stride < (size_t)in->width * a.nch * bps) return set_error(B200_E_INVALID, "RGB stride %zu < row of %d pixels", in->rgb_stride, in->width);
+    a.in[0] = (const uint8_t*)in->rgb; a.is[0] = (long long)in->rgb_stride;
+    ai = (uintptr_t)in->rgb | (uintptr_t)in->rgb_stride;
+    a.vec_in = bps == 2 && (ai & (a.nch == 4 ? 15 : 3)) == 0;
+  } else {
+    const void* pl[4] = {in->r, in->g, in->b, in->alpha};
+    const size_t st[4] = {in->r_stride, in->g_stride, in->b_stride, in->alpha_stride};
+    for (int c = 0; c < (has_alpha ? 4 : 3); c++) {
+      if (st[c] < (size_t)in->width * bps) return set_error(B200_E_INVALID, "plane %d stride %zu < row of %d samples", c, st[c], in->width);
+      a.in[c] = (const uint8_t*)pl[c]; a.is[c] = (long long)st[c]; ai |= (uintptr_t)pl[c] | (uintptr_t)st[c];
+    }
+    a.vec_in = (ai & (2 * bps - 1)) == 0;
+  }
+  a.le = in->chroma == B200_CHROMA_INTERLEAVED_RRGGBB_LE || in->chroma == B200_CHROMA_INTERLEAVED_RRGGBBAA_LE;
+  a.y = (uint8_t*)out->y; a.cb = (uint8_t*)out->cb; a.cr = (uint8_t*)out->cr; a.a = (uint8_t*)out->alpha;
+  a.ys = (long long)out->y_stride; a.cs = (long long)out->c_stride; a.as = (long long)out->alpha_stride;
+  uintptr_t ao = (uintptr_t)out->y | (uintptr_t)out->cb | (uintptr_t)out->cr | (uintptr_t)out->y_stride | (uintptr_t)out->c_stride;
+  if (out->alpha) ao |= (uintptr_t)out->alpha | (uintptr_t)out->alpha_stride;
+  a.vec_out = (ao & (2 * bps - 1)) == 0;
+  a.w = out->width; a.h = out->height; a.full = out->full_range ? 1 : 0; a.bpp = in->bit_depth;
+  a.sh = out->chroma == B200_CHROMA_444 ? 0 : 1; a.sv = out->chroma == B200_CHROMA_420 ? 1 : 0;
+  int mc = out->matrix_coefficients, cp = out->colour_primaries;
+  if (mc == 2) mc = 6;              // unspecified -> the input's sRGB defaults (colorconversion.cc:513-515, :567-573)
+  if (cp == 2) cp = 1;
+  a.mc = mc;
+  rgb_to_ycbcr_coefficients(mc, cp, a.c);
+  const dim3 block(64, 4), grid((a.w + 127) / 128, (a.h + 7) / 8);
+  if (pipe == B200_YCC_PIPE_HDR420) rgb_to_ycbcr_ex_kernel<uint16_t, false, YCC_HDR420><<<grid, block, 0, stream>>>(a);
+  else if (pipe == B200_YCC_PIPE_GBR444) rgb_to_ycbcr_ex_kernel<uint8_t, false, YCC_GBR444><<<grid, block, 0, stream>>>(a);
+  else if (inter) {
+    if (bps == 1) rgb_to_ycbcr_ex_kernel<uint8_t, false, YCC_PLANAR><<<grid, block, 0, stream>>>(a);
+    else rgb_to_ycbcr_ex_kernel<uint16_t, false, YCC_PLANAR><<<grid, block, 0, stream>>>(a);
+  } else {
+    if (bps == 1) rgb_to_ycbcr_ex_kernel<uint8_t, true, YCC_PLANAR><<<grid, block, 0, stream>>>(a);
+    else rgb_to_ycbcr_ex_kernel<uint16_t, true, YCC_PLANAR><<<grid, block, 0, stream>>>(a);
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(B200_E_CUDA, "RGB -> YCbCr launch: %s", cudaGetErrorString(e));
+  return B200_OK;
+}
+
 
 }  // namespace b200
