@@ -1,8 +1,9 @@
 // b200_hevc_entropy.cu -- K0: CABAC entropy decoding + slice-data syntax on the GPU.
 //
 // The serial half of libde265's decode (H.265 9.3 CABAC, 7.3.8 coding-quadtree syntax, 8.4.2 / 8.6.1 derivations) for
-// a whole batch of tiles at once: ONE WARP PER CABAC SUB-STREAM (lane 0 runs the shared syntax decoder of
-// b200_hevc_syntax.h, the same source the host front-end uses).  With entropy_coding_sync every CTB row is its own
+// a whole batch of tiles at once: ONE WARP PER CABAC SUB-STREAM (all 32 lanes run the shared syntax decoder of
+// b200_hevc_syntax.h, the same source the host front-end uses, on identical data, and split the map fills, context copies
+// and coefficient emission between them).  With entropy_coding_sync every CTB row is its own
 // sub-stream, located by the slice header's entry points, so a 16384x16384 grid of 1024x1024 tiles exposes 8192
 // independent-ish streams: rows of one picture advance as a wavefront (context hand-over after the 2nd CTB of the row
 // above, 9.3.2.2), pictures are independent.  Sub-streams are handed out through a READY QUEUE: a sub-stream enters it when
@@ -55,7 +56,22 @@ __device__ __forceinline__ unsigned e_ld_acquire(const unsigned* p) {
 __device__ __forceinline__ void e_st_release(unsigned* p, unsigned v) {
   asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
+// A decoder warp's poll: lane 0's value for every lane, so that the loop it controls stays warp-uniform.
+__device__ __forceinline__ unsigned e_poll(const unsigned* p) { return __shfl_sync(0xffffffffu, e_ld_acquire(p), 0); }
+__device__ __forceinline__ bool lane0() { return syn::lane_id() == 0; }
 
+#ifdef B200_ENTROPY_TRACE
+// Per sub-stream (batch-wide index): globaltimer at the queue pop and at the end, and the SM it ran on.  For
+// scripts/k0_trace_probe.py only; b200_debug_entropy_trace() copies it out.
+constexpr int TRACE_CAP = 1 << 16;
+__device__ unsigned long long g_trace[TRACE_CAP][2];
+__device__ unsigned g_trace_sm[TRACE_CAP];
+__device__ __forceinline__ unsigned long long e_globaltimer() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+__device__ __forceinline__ unsigned e_smid() { unsigned s; asm volatile("mov.u32 %0, %%smid;" : "=r"(s)); return s; }
+#endif
+
+// Every lane of a decoder warp calls these (the decoder runs warp-wide, b200_hevc_syntax.h); the atomics and the releases
+// happen once, on lane 0, after a warp barrier that orders the other lanes' stores (map cells, contexts) before them.
 struct DevSync {
   unsigned* progress;      // per CTB row of this picture
   unsigned* sub_done;      // per sub-stream of this picture
@@ -64,30 +80,38 @@ struct DevSync {
   uint32_t dense_tu, dense_coef, dense_tu_cap, dense_coef_cap;   // unused on the device (fixed slots)
   uint64_t end_bit_position;
   // Waits inside a sub-stream are short (the row above runs two CTBs ahead): poll with a sub-microsecond back-off.  Gives
-  // up (error 3) after ~60 s -- only a lost producer can cause that.
+  // up (error 3) after ~60 s -- only a lost producer can cause that.  The caps (8 us here, 16 us for a queue slot) are the
+  // measured optimum: 1.6 / 2 us made K0 ~1 % slower and 0.8 / 1 us ~2 % (polls take issue slots from the busy decoders),
+  // 16 / 32 us gained nothing (H100 80GB HBM3 SXM at 400 W, bench.py).
   __device__ static void spin_until(const unsigned* p, unsigned need, unsigned* error_flag) {
-    if (e_ld_acquire(p) >= need) return;
+    if (e_poll(p) >= need) return;
     unsigned ns = 200, spins = 0;
     for (;;) {
       __nanosleep(ns); if (ns < 8000) ns <<= 1;
-      if (e_ld_acquire(p) >= need) return;
+      if (e_poll(p) >= need) return;
       if ((++spins & 63u) != 0) continue;
-      if (e_ld_acquire(error_flag)) return;              // a producer failed: do not wait for progress that will never come
-      if (spins > (1u << 23)) { atomicExch(error_flag, 3u); return; }
+      if (e_poll(error_flag)) return;                    // a producer failed: do not wait for progress that will never come
+      if (spins > (1u << 23)) { if (lane0()) atomicExch(error_flag, 3u); return; }
     }
   }
   __device__ void wait_row(int row, int need) { spin_until(progress + row, (unsigned)need, error_flag); }
-  __device__ void publish_row(int row, int done) { e_st_release(progress + row, (unsigned)done); }
+  __device__ void publish_row(int row, int done) { syn::warp_sync(); if (lane0()) e_st_release(progress + row, (unsigned)done); }
   __device__ void wait_substream(int idx) { spin_until(sub_done + idx, 1u, error_flag); }
   __device__ void finish_substream(int idx, int err) {
-    e_st_release(sub_done + idx, 1u);
-    if (err) atomicExch(error_flag, (unsigned)err);
+    syn::warp_sync();
+    if (lane0()) {
+      e_st_release(sub_done + idx, 1u);
+      if (err) atomicExch(error_flag, (unsigned)err);
+    }
   }
   // One of the events sub-stream `target` (batch-wide index) waits for has happened; the last one makes it ready.
   __device__ void notify(int target) {
     if (target < 0) return;
-    __threadfence();                                     // what the target will read (contexts, end state) is published first
-    if (atomicSub(deps + target, 1u) == 1u) { const unsigned s = atomicAdd(qtail, 1u); e_st_release(queue + s, (unsigned)target + 1u); }
+    syn::warp_sync();
+    if (lane0()) {
+      __threadfence();                                   // what the target will read (contexts, end state) is published first
+      if (atomicSub(deps + target, 1u) == 1u) { const unsigned s = atomicAdd(qtail, 1u); e_st_release(queue + s, (unsigned)target + 1u); }
+    }
   }
 };
 
@@ -107,7 +131,7 @@ template <class Cfg> constexpr int entropy_min_blocks() { return B200_ENTROPY_MI
 template <> constexpr int entropy_min_blocks<syn::CfgCommon>() { return B200_ENTROPY_MIN_BLOCKS > 5 ? B200_ENTROPY_MIN_BLOCKS : 5; }
 template <class Cfg>
 __global__ void __launch_bounds__(EWARPS * 32, entropy_min_blocks<Cfg>()) hevc_entropy_kernel(const EntropyBatch b) {
-  __shared__ __align__(8) syn::U2 s_ctx[EWARPS][syn::CTX_COUNT];   // context variables: one state-table entry each
+  __shared__ __align__(8) syn::U2 s_ctx[EWARPS][syn::CTX_COUNT + syn::CTX_SCRATCH];   // context variables: one state-table entry each (+ scratch)
   __shared__ syn::DecoderT<Cfg> s_dec[EWARPS];                    // per-warp decoder state (see run_substream)
   __shared__ DevSync s_sync[EWARPS];                              // per-warp hand-shake pointers (shared: no register holds them across the CTB loop)
   for (int i = threadIdx.x; i < 64; i += blockDim.x) { syn::s_kLps4[i] = syn::d_kLps4[i]; syn::s_kTransLps[i] = syn::d_kTransLps[i]; }
@@ -121,26 +145,31 @@ __global__ void __launch_bounds__(EWARPS * 32, entropy_min_blocks<Cfg>()) hevc_e
   for (int i = threadIdx.x; i < 4; i += blockDim.x) syn::s_kChromaTab[i] = syn::d_kChromaTab[i];
   for (int i = threadIdx.x; i < 4 * 3 * 64; i += blockDim.x) { (&syn::s_kScanX[0][0][0])[i] = (&syn::d_kScanX[0][0][0])[i]; (&syn::s_kScanY[0][0][0])[i] = (&syn::d_kScanY[0][0][0])[i]; }
   __syncthreads();
-  // Lane 0 of every warp decodes: CABAC is serial per sub-stream.  (Several decoders per warp on diverged lanes were
-  // measured 25-70 % slower: the diverged paths of one warp serialise.)
-  if ((threadIdx.x & 31) != 0) return;
+  // Every warp decodes one sub-stream at a time, all 32 lanes on identical data: CABAC is serial per sub-stream, and the
+  // lanes share the per-cell / per-context / per-coefficient work around the bins (b200_hevc_syntax.h).  (Several decoders
+  // per warp on diverged lanes were measured 25-70 % slower: the diverged paths of one warp serialise.)
   const int slot_w = threadIdx.x >> 5;
   const syn::CtxPtr ctx = (syn::CtxPtr)__cvta_generic_to_shared(s_ctx[slot_w]);
   for (;;) {
-    const unsigned slot = atomicAdd(b.qhead, 1u);
+    unsigned slot = 0;
+    if (lane0()) slot = atomicAdd(b.qhead, 1u);
+    slot = __shfl_sync(0xffffffffu, slot, 0);
     if (slot >= (unsigned)b.nsubs) break;
     // the slot is filled when the sub-stream becomes ready (already, for those without prerequisites)
-    unsigned item = e_ld_acquire(b.queue + slot);
+    unsigned item = e_poll(b.queue + slot);
     if (!item) {
       unsigned ns = 500, spins = 0;
       for (;;) {
         __nanosleep(ns); if (ns < 16000) ns <<= 1;
-        if ((item = e_ld_acquire(b.queue + slot)) != 0u) break;
+        if ((item = e_poll(b.queue + slot)) != 0u) break;
         if ((++spins & 31u) != 0) continue;
-        if (e_ld_acquire(b.error_flag)) return;          // a producer failed: its dependants never become ready
-        if (spins > (1u << 22)) { atomicExch(b.error_flag, 3u); return; }
+        if (e_poll(b.error_flag)) return;                // a producer failed: its dependants never become ready
+        if (spins > (1u << 22)) { if (lane0()) atomicExch(b.error_flag, 3u); return; }
       }
     }
+#ifdef B200_ENTROPY_TRACE
+    if (lane0() && item - 1u < (unsigned)TRACE_CAP) { g_trace[item - 1u][0] = e_globaltimer(); g_trace_sm[item - 1u] = e_smid(); }
+#endif
     const syn::Substream& gs = b.subs[item - 1u];
     const EntropyPic& ep = b.pics[gs.pic];
     DevSync& sync = s_sync[slot_w];
@@ -148,8 +177,25 @@ __global__ void __launch_bounds__(EWARPS * 32, entropy_min_blocks<Cfg>()) hevc_e
     sync.queue = b.queue; sync.qtail = b.qtail; sync.deps = b.deps;
     sync.dense_tu = sync.dense_coef = sync.dense_tu_cap = sync.dense_coef_cap = 0; sync.end_bit_position = 0;
     syn::run_substream<Cfg>(s_dec[slot_w], ep.sp, ep.pb, b.subs + ep.sub_base, (int)(item - 1u - ep.sub_base), ctx, sync);
+#ifdef B200_ENTROPY_TRACE
+    if (lane0() && item - 1u < (unsigned)TRACE_CAP) g_trace[item - 1u][1] = e_globaltimer();
+#endif
   }
 }
+
+#ifdef B200_ENTROPY_TRACE
+// n records of {pop ns, end ns, SM} (3 x u64 each) of the last entropy launch; sub-streams past TRACE_CAP are not recorded
+extern "C" int b200_debug_entropy_trace(unsigned long long* out, int n) {
+  if (!out || n < 0 || n > TRACE_CAP) return set_error(B200_E_INVALID, "bad trace request");
+  static unsigned long long t[TRACE_CAP][2]; static unsigned sm[TRACE_CAP];
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess) e = cudaMemcpyFromSymbol(t, g_trace, sizeof t);
+  if (e == cudaSuccess) e = cudaMemcpyFromSymbol(sm, g_trace_sm, sizeof sm);
+  if (e != cudaSuccess) return set_error(B200_E_CUDA, "entropy trace: %s", cudaGetErrorString(e));
+  for (int i = 0; i < n; i++) { out[3 * i] = t[i][0]; out[3 * i + 1] = t[i][1]; out[3 * i + 2] = sm[i]; }
+  return B200_OK;
+}
+#endif
 
 // sums the per-CTB TU / coefficient counts (statistics only: command-stream bytes actually produced)
 __global__ void entropy_stats_kernel(const EntropyBatch b, unsigned long long* out2) {

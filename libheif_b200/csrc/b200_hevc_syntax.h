@@ -5,6 +5,7 @@
 // wavefront (context hand-over after the 2nd CTB of the row above, 9.3.2.2), sequentially on the host.
 // Output = the command stream of b200_hevc_types.h.  No pixel is touched here.
 #pragma once
+#include <cassert>
 #include <cstdint>
 #include <cstring>
 #include "b200_hevc_types.h"
@@ -75,7 +76,8 @@ inline U2 tab_ld64(TabPtr p, int i) { uint64_t v; memcpy(&v, p + 8 * (size_t)i, 
 enum { CTX_SAO_MERGE = 0, CTX_SAO_TYPE = 1, CTX_SPLIT_CU = 2, CTX_PART_MODE = 5, CTX_PREV_INTRA = 6,
        CTX_CHROMA_PRED = 7, CTX_SPLIT_TR = 8, CTX_CBF_LUMA = 11, CTX_CBF_CHROMA = 13, CTX_QP_DELTA = 18,
        CTX_TSKIP = 20, CTX_LAST_X = 22, CTX_LAST_Y = 40, CTX_CSBF = 58, CTX_SIG = 62, CTX_GT1 = 104,
-       CTX_GT2 = 128, CTX_TQ_BYPASS = 134, CTX_COUNT = 135, CTX_STRIDE = 144 };
+       CTX_GT2 = 128, CTX_TQ_BYPASS = 134, CTX_COUNT = 135, CTX_STRIDE = 144,
+       CTX_SCRATCH = 8 };   // device: 8-byte slots behind the context array = the 16 level words of residual_coding's emission
 
 // Tables 9-5 .. 9-37, initType 0 (I slices)
 B200_TABLE(uint8_t, kInitI, [CTX_COUNT], {
@@ -116,6 +118,32 @@ B200_HD inline int pop_count(uint32_t v) { return __popc(v); }
 B200_HD inline int hi_bit(uint32_t v) { return 31 - __builtin_clz(v); }
 B200_HD inline int lo_bit(uint32_t v) { return __builtin_ctz(v); }
 B200_HD inline int pop_count(uint32_t v) { return __builtin_popcount(v); }
+#endif
+
+// Warp-wide decoding on the device: all 32 lanes of a decoder warp run the (serial) syntax decoder on identical data, so
+// every branch outside the lane-parallel sections is warp-uniform and a warp instruction costs one issue slot as before.
+// The per-cell, per-context and per-coefficient work around the bins is split over the lanes in lane-parallel sections:
+//   B200_LANES_BEGIN(); B200_LANE_FOR(k, n) { ... item k ... } B200_LANES_END();
+// On the host the same source is a plain serial loop.  A section's stores (global map cells, shared contexts / scratch)
+// are ordered before anything any lane does after B200_LANES_END.
+#ifdef __CUDACC__
+// volatile: read where it is needed instead of being kept live across the call chain
+__device__ __forceinline__ int lane_id() { unsigned l; asm volatile("mov.u32 %0, %%laneid;" : "=r"(l)); return (int)l; }
+// volatile asm with a memory clobber: also keeps its place among the (volatile asm) context loads and stores
+__device__ __forceinline__ void warp_sync() { asm volatile("bar.warp.sync -1;" ::: "memory"); }
+#endif
+#ifdef B200_SYN_DEVICE
+#ifdef B200_ENTROPY_CHECK_CONVERGENCE     // debug builds: every lane-parallel section is entered by the whole warp
+#define B200_LANES_BEGIN() assert(__activemask() == 0xffffffffu)
+#else
+#define B200_LANES_BEGIN() ((void)0)
+#endif
+#define B200_LANE_FOR(k, n) B200_NOUNROLL for (int k = ::b200::syn::lane_id(); k < (n); k += 32)
+#define B200_LANES_END() ::b200::syn::warp_sync()
+#else
+#define B200_LANES_BEGIN() ((void)0)
+#define B200_LANE_FOR(k, n) B200_NOUNROLL for (int k = 0; k < (n); k++)
+#define B200_LANES_END() ((void)0)
 #endif
 
 // Sequence / picture level parameters the slice data depends on (filled by the host from SPS + PPS).
@@ -279,12 +307,26 @@ struct Cabac {
 
 B200_HDN inline void init_contexts(CtxPtr ctx, int slice_qp) {          // 9.3.2.2
   const int qp = clip3(0, 51, slice_qp);
-  for (int i = 0; i < CTX_COUNT; i++) {
+  B200_LANES_BEGIN();
+  B200_LANE_FOR(i, CTX_COUNT) {
     const int iv = B200_T(kInitI)[i], m = (iv >> 4) * 5 - 45, nn = ((iv & 15) << 3) - 16;
     const int pre = clip3(1, 126, ((m * qp) >> 4) + nn);
     const int mps = pre > 63, st = mps ? pre - 64 : 63 - pre;
     ctx_st(ctx_at(ctx, i), tab_ld64(B200_TADDR(kState), (st << 1) | mps));
   }
+  B200_LANES_END();
+}
+
+// context states from the bytes (pStateIdx << 1 | valMps) another sub-stream stored (WPP hand-over, dependent segment)
+B200_HDN inline void load_contexts(CtxPtr ctx, const uint8_t* st) {
+  B200_LANES_BEGIN();
+  B200_LANE_FOR(i, CTX_COUNT) ctx_st(ctx_at(ctx, i), tab_ld64(B200_TADDR(kState), (int)B200_LD_SHARED(st + i) & 127));
+  B200_LANES_END();
+}
+B200_HDN inline void store_contexts(CtxPtr ctx, uint8_t* st) {
+  B200_LANES_BEGIN();
+  B200_LANE_FOR(i, CTX_COUNT) st[i] = (uint8_t)(ctx_ld(ctx_at(ctx, i)).y >> 24);
+  B200_LANES_END();
 }
 
 enum { SYN_OK = 0, SYN_E_BITSTREAM = 1, SYN_E_OVERFLOW = 2 };
@@ -472,6 +514,40 @@ struct DecoderT {
       if (last_g1 >= 0) g2 = cb_.bin(ctx_at(cx, CTX_GT2 + ctx_set + (c ? 4 : 0)), stream);
       const int nsign = pop_count(sig) - (hidden ? 1 : 0);
       const unsigned signs = cb_.bypass_bits(nsign, stream);
+#ifdef B200_SYN_DEVICE
+      // The serial loop keeps what is serial by nature (the coeff_abs_level_remaining bins, Rice adaptation, the parity sum
+      // of sign hiding) and leaves each absolute level in the warp's scratch words behind its context array; then lane k < 16
+      // emits scan position k: output index (significant positions above it), sign, position, clip, one store.
+      int nsig = 0, sum = 0, rice = 0;
+      const uint32_t lv = ctx_at(cx, CTX_COUNT);
+      B200_NOUNROLL for (unsigned m = sig; m; nsig++) {
+        const int kk = hi_bit(m); m ^= 1u << kk;
+        const int base = 1 + (int)((g1 >> kk) & 1) + (kk == last_g1 ? g2 : 0);
+        int a = base;
+        if (base == ((nsig < 8) ? ((kk == last_g1) ? 3 : 2) : 1)) {
+          int pre = 0; B200_NOUNROLL while (pre < 32 && cb_.bypass(stream)) pre++;
+          if (pre > 20) { err = SYN_E_BITSTREAM; cabac = cb_; const int count = (int)(cn - coef_n); coef_n = cn; return count; }   // far outside the 16-bit range of TransCoeffLevel: corrupt data
+          const int rem = (pre <= 3 ? (pre << rice) : (((1 << (pre - 3)) + 3 - 1) << rice)) + (int)cb_.bypass_bits(pre <= 3 ? rice : pre - 3 + rice, stream);
+          a = base + rem;
+          if (a > 3 * (1 << rice)) rice = imin(rice + 1, 4);
+        }
+        sum += a;
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(lv + 4u * (uint32_t)kk), "r"(a));
+      }
+      if (cn + (uint32_t)nsig > coef_cap) { err = SYN_E_OVERFLOW; cabac = cb_; const int count = (int)(cn - coef_n); coef_n = cn; return count; }
+      B200_LANES_BEGIN();
+      { const int k = lane_id();
+        if (k < 16 && ((sig >> k) & 1u)) {
+          int a; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(a) : "r"(lv + 4u * (uint32_t)k));
+          const int above = pop_count(sig >> k >> 1);     // coefficients decoded (and emitted) before this one
+          const int neg = (hidden && k == first_sig) ? (sum & 1) : (int)((signs >> (nsign - 1 - above)) & 1u);
+          const int p = (int)tab_ld8(spos, k);
+          CoefEntry e; e.pos = (uint16_t)((((ys << 2) + (p >> 2)) << log2n) + (xs << 2) + (p & 3)); e.level = (int16_t)clip3(-32768, 32767, neg ? -a : a);
+          pb.coefs[cn + (uint32_t)above] = e;
+        } }
+      B200_LANES_END();
+      cn += (uint32_t)nsig;
+#else
       int nsig = 0, sum = 0, rice = 0, sidx = nsign;
       B200_NOUNROLL for (unsigned m = sig; m; nsig++) {
         const int kk = hi_bit(m); m ^= 1u << kk;
@@ -493,6 +569,7 @@ struct DecoderT {
         CoefEntry e; e.pos = (uint16_t)((((ys << 2) + (p >> 2)) << log2n) + (xs << 2) + (p & 3)); e.level = (int16_t)clip3(-32768, 32767, v);
         pb.coefs[cn++] = e;
       }
+#endif
     }
     cabac = cb_;
     const int count = (int)(cn - coef_n);                 // coefficients written
@@ -511,10 +588,17 @@ struct DecoderT {
       if ((y0 & 7) == 0 && y0 > 0 && (y0 > ctb_y0 || up_lf)) top = 2;
     }
     // the CTB's flags were cleared in decode_ctb: only the first column / row of 8x8 cells carries an edge.  (QpY of the
-    // cells is written once per coding unit, at its end.)
+    // cells is written once per coding unit, at its end.)  Item k < n8: cell k of the column (the corner takes both flags);
+    // k >= n8: cell k - n8 + 1 of the row -- no two items touch the same cell.
     uint8_t* e = pb.edge8 + by * sp->w8 + bx;
-    if (left) B200_NOUNROLL for (int y = 0; y < n8; y++) e[y * sp->w8] |= left;
-    if (top) B200_NOUNROLL for (int x = 0; x < n8; x++) e[x] |= top;
+    if (!(left | top)) return;
+    B200_LANES_BEGIN();
+    B200_LANE_FOR(k, 2 * n8 - 1) {
+      const bool col = k < n8;
+      const uint8_t v = col ? (uint8_t)(left | (k ? 0 : top)) : top;
+      if (v) e[col ? k * sp->w8 : k - n8 + 1] |= v;
+    }
+    B200_LANES_END();
   }
 
   B200_HDI void transform_unit(const Cu& cu, int x0, int y0, int log2n, int blk, int cbf_l, int cbf_cb, int cbf_cr, int pcb, int pcr) {
@@ -734,12 +818,18 @@ struct DecoderT {
     cabac.start(stream, p);                                             // 9.3.2.5: the arithmetic decoder starts over after the samples
     if (!B200_SPC(cu_qp_delta)) cur_qpy = ss->slice_qp; else derive_qpy(x0, y0);
     const int nofilt = sp->pcm_lf_disabled ? 4 : 0;
-    B200_NOUNROLL for (int yy = 0; yy < n; yy += 4) B200_NOUNROLL for (int xx = 0; xx < n; xx += 4) pb.ipm4[((y0 + yy) >> 2) * sp->w4 + ((x0 + xx) >> 2)] = 1;   // INTRA_DC for its neighbours' mode derivation (8.4.2)
+    { const int l4 = log2cb - 2;                       // INTRA_DC for its neighbours' mode derivation (8.4.2)
+      B200_LANES_BEGIN();
+      B200_LANE_FOR(k, 1 << (2 * l4)) pb.ipm4[((y0 >> 2) + (k >> l4)) * sp->w4 + (x0 >> 2) + (k & ((1 << l4) - 1))] = 1;
+      B200_LANES_END(); }
     mark_tu(x0, y0, log2cb);
-    B200_NOUNROLL for (int yy = 0; yy < n; yy += 8) B200_NOUNROLL for (int xx = 0; xx < n; xx += 8) {
-      const int i8 = ((y0 + yy) >> 3) * sp->w8 + ((x0 + xx) >> 3);
-      pb.cd8[i8] = (uint8_t)depth; pb.qp8[i8] = (int8_t)cur_qpy; pb.edge8[i8] |= (uint8_t)nofilt;
-    }
+    { const int l8 = log2cb - 3;
+      B200_LANES_BEGIN();
+      B200_LANE_FOR(k, 1 << (2 * l8)) {
+        const int i8 = ((y0 >> 3) + (k >> l8)) * sp->w8 + (x0 >> 3) + (k & ((1 << l8) - 1));
+        pb.cd8[i8] = (uint8_t)depth; pb.qp8[i8] = (int8_t)cur_qpy; pb.edge8[i8] |= (uint8_t)nofilt;
+      }
+      B200_LANES_END(); }
     last_cu_qpy = cur_qpy;
     if (cfmt >= 2) {                                   // 4:2:2 / 4:4:4: one command per block, like transform_unit_x
       emit_block(0, x0, y0, log2cb, 1, 0, 1, coef0, (int)nl, 1u << 21);
@@ -776,6 +866,14 @@ struct DecoderT {
     cu.cmode = cu.cmodes[0];
   }
 
+  // the 1 << (2 * l) cells of a square block (l = log2 of its side in cells) whose top-left cell is `m` in a map with `stride`
+  // cells per row: `set` ? v : (cell | v)
+  B200_HDI static void fill_cells(uint8_t* m, int stride, int l, uint8_t v, bool set) {
+    B200_LANES_BEGIN();
+    B200_LANE_FOR(k, 1 << (2 * l)) { uint8_t* p = m + (k >> l) * stride + (k & ((1 << l) - 1)); *p = set ? v : (uint8_t)(*p | v); }
+    B200_LANES_END();
+  }
+
   // -------- 7.3.8.5
   B200_HDI void coding_unit(int x0, int y0, int log2cb, int depth) {
     Cu cu; cu.x0 = x0; cu.y0 = y0; cu.log2cb = log2cb; cu.nxn = 0; cu.cmode = 0;
@@ -783,7 +881,7 @@ struct DecoderT {
     if (B200_SPC(tq_bypass)) {
       cu_bypass = dbin(CTX_TQ_BYPASS);
       // in-loop filters leave the samples of this unit unchanged (8.7.2.5.7 nDp / nDq = 0, 8.7.3 SaoTypeIdx = 0): bit 2 of the 8x8 cells
-      if (cu_bypass) B200_NOUNROLL for (int yy = 0; yy < n; yy += 8) B200_NOUNROLL for (int xx = 0; xx < n; xx += 8) pb.edge8[((y0 + yy) >> 3) * sp->w8 + ((x0 + xx) >> 3)] |= 4;
+      if (cu_bypass) fill_cells(pb.edge8 + (y0 >> 3) * sp->w8 + (x0 >> 3), sp->w8, log2cb - 3, 4, false);
     }
     if (log2cb == B200_SPC(log2_min_cb)) cu.nxn = !dbin(CTX_PART_MODE);
     if (cu.nxn && log2cb == 3 && B200_SPC(log2_min_tb) > 2) { err = SYN_E_BITSTREAM; return; }
@@ -796,17 +894,17 @@ struct DecoderT {
       const int px = x0 + (i & 1) * pbs, py = y0 + (i >> 1) * pbs;
       const int m = luma_mode(px, py, prev[i], mi[i], rem[i]);
       cu.lmode[i] = m;
-      B200_NOUNROLL for (int yy = 0; yy < pbs; yy += 4) B200_NOUNROLL for (int xx = 0; xx < pbs; xx += 4) pb.ipm4[((py + yy) >> 2) * sp->w4 + ((px + xx) >> 2)] = (uint8_t)m;
+      fill_cells(pb.ipm4 + (py >> 2) * sp->w4 + (px >> 2), sp->w4, log2cb - cu.nxn - 2, (uint8_t)m, true);
     }
     if (B200_SPC(chroma) >= 2) chroma_modes_x(cu, np);
     else if (B200_SPC(chroma)) {
       int v = 4; if (dbin(CTX_CHROMA_PRED)) v = (int)dbits(2);
       if (v == 4) cu.cmode = cu.lmode[0]; else { cu.cmode = B200_T(kChromaTab)[v]; if (cu.cmode == cu.lmode[0]) cu.cmode = 34; }
     }
-    B200_NOUNROLL for (int yy = 0; yy < n; yy += 8) B200_NOUNROLL for (int xx = 0; xx < n; xx += 8) pb.cd8[((y0 + yy) >> 3) * sp->w8 + ((x0 + xx) >> 3)] = (uint8_t)depth;
+    fill_cells(pb.cd8 + (y0 >> 3) * sp->w8 + (x0 >> 3), sp->w8, log2cb - 3, (uint8_t)depth, true);
     if (!B200_SPC(cu_qp_delta)) cur_qpy = ss->slice_qp; else derive_qpy(x0, y0);
     if (B200_SPC(chroma) >= 2) transform_tree_x(cu, sp->max_th_depth_intra + cu.nxn); else transform_tree(cu, sp->max_th_depth_intra + cu.nxn);
-    B200_NOUNROLL for (int yy = 0; yy < n; yy += 8) B200_NOUNROLL for (int xx = 0; xx < n; xx += 8) pb.qp8[((y0 + yy) >> 3) * sp->w8 + ((x0 + xx) >> 3)] = (int8_t)cur_qpy;
+    fill_cells(reinterpret_cast<uint8_t*>(pb.qp8) + (y0 >> 3) * sp->w8 + (x0 >> 3), sp->w8, log2cb - 3, (uint8_t)(int8_t)cur_qpy, true);
     last_cu_qpy = cur_qpy;
   }
 
@@ -862,8 +960,10 @@ struct DecoderT {
     if (B200_SPC(sao_enabled)) parse_sao(rx, ry, ci);
     else for (int c = 0; c < 3; c++) { ci.sao[c].type = 0; ci.sao[c].band_or_class = 0; B200_NOUNROLL for (int k = 0; k < 4; k++) ci.sao[c].offset[k] = 0; }
     // 4x4 luma transform units only OR their edge bits: clear this CTB's flags first
-    { const int b0x = rx << (sp->log2ctb - 3), b0y = ry << (sp->log2ctb - 3), nb = 1 << (sp->log2ctb - 3);
-      B200_NOUNROLL for (int y = 0; y < nb && b0y + y < sp->h8; y++) B200_NOUNROLL for (int x = 0; x < nb && b0x + x < sp->w8; x++) pb.edge8[(b0y + y) * sp->w8 + b0x + x] = 0; }
+    { const int l = sp->log2ctb - 3, b0x = rx << l, b0y = ry << l;
+      B200_LANES_BEGIN();
+      B200_LANE_FOR(k, 1 << (2 * l)) { const int y = b0y + (k >> l), x = b0x + (k & ((1 << l) - 1)); if (y < sp->h8 && x < sp->w8) pb.edge8[y * sp->w8 + x] = 0; }
+      B200_LANES_END(); }
     coding_quadtree();
     CtuInfo& ce = pb.ctus[cur_ctb_y * sp->wctb + cur_ctb_x];        // (read again, like the quadtree's state)
     ce.tu_start = ctb_tu0; ce.tu_count = (uint16_t)(tu_n - ctb_tu0);
@@ -891,7 +991,7 @@ B200_HD int run_substream(DecoderT<Cfg>& d, const SeqParams& sp, const PicBuffer
   if (ss.prev >= 0) {                                         // dependent slice segment: continue from the previous segment's end state
     sync.wait_substream(ss.prev);
     const uint8_t* st = pb.end_state + (size_t)ss.prev * CTX_STRIDE;
-    B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) ctx_st(ctx_at(ctx, i), tab_ld64(B200_TADDR(kState), (int)B200_LD_SHARED(st + i) & 127));
+    load_contexts(ctx, st);
     d.last_cu_qpy = (int)(int8_t)B200_LD_SHARED(st + CTX_COUNT); d.first_qg = 0;
   }
   if (ss.init_contexts) init_contexts(ctx, ss.slice_qp);
@@ -901,7 +1001,7 @@ B200_HD int run_substream(DecoderT<Cfg>& d, const SeqParams& sp, const PicBuffer
     const int xn = 1 << sp.log2ctb, yn = (ry0 - 1) << sp.log2ctb;
     bool tr = ry0 > 0 && xn < sp.W && pb.ctu_slice[(ry0 - 1) * sp.wctb + 1] == (uint16_t)ss.slice_idx;
     (void)yn;
-    if (tr) { sync.wait_row(ry0 - 1, 2); const uint8_t* st = pb.wpp_ctx + (size_t)(ry0 - 1) * CTX_STRIDE; B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) ctx_st(ctx_at(ctx, i), tab_ld64(B200_TADDR(kState), (int)B200_LD_SHARED(st + i) & 127)); }
+    if (tr) { sync.wait_row(ry0 - 1, 2); load_contexts(ctx, pb.wpp_ctx + (size_t)(ry0 - 1) * CTX_STRIDE); }
     else if (ss.prev < 0) init_contexts(ctx, ss.slice_qp);
     d.first_qg = 1;
   }
@@ -925,7 +1025,7 @@ B200_HD int run_substream(DecoderT<Cfg>& d, const SeqParams& sp, const PicBuffer
     d.decode_ctb((int)a);
     if (d.err) break;
     rx = d.cur_ctb_x; ry = d.cur_ctb_y;
-    if (B200_SPR(wpp) && rx == 1) { uint8_t* st = d.pb.wpp_ctx + (size_t)ry * CTX_STRIDE; B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) st[i] = (uint8_t)(ctx_ld(ctx_at(d.ctx, i)).y >> 24); }
+    if (B200_SPR(wpp) && rx == 1) store_contexts(d.ctx, d.pb.wpp_ctx + (size_t)ry * CTX_STRIDE);
     const int end = d.cabac.terminate(d.stream);                          // end_of_slice_segment_flag
     const bool last = left == 1;
     if (end != ((last && d.ss->last_of_segment) ? 1 : 0)) { d.err = SYN_E_BITSTREAM; break; }
@@ -935,7 +1035,7 @@ B200_HD int run_substream(DecoderT<Cfg>& d, const SeqParams& sp, const PicBuffer
     if (d.cabac.pos > d.pb.rbsp_size + 64u) { d.err = SYN_E_BITSTREAM; break; }
   }
   // end state for a dependent continuation + dense cursors
-  { uint8_t* st = d.pb.end_state + (size_t)index * CTX_STRIDE; B200_NOUNROLL for (int i = 0; i < CTX_COUNT; i++) st[i] = (uint8_t)(ctx_ld(ctx_at(d.ctx, i)).y >> 24); st[CTX_COUNT] = (uint8_t)(int8_t)d.last_cu_qpy; }
+  { uint8_t* st = d.pb.end_state + (size_t)index * CTX_STRIDE; store_contexts(d.ctx, st); st[CTX_COUNT] = (uint8_t)(int8_t)d.last_cu_qpy; }
   if (B200_SPR(dense)) { sync.dense_tu = d.tu_n; sync.dense_coef = d.coef_n; }
   sync.end_bit_position = d.cabac.bit_position();
   sync.finish_substream(index, d.err);
