@@ -246,6 +246,46 @@ int b200_hevc_encode_intra(const b200_hevc_enc_params* p, const void* y, const v
 void b200_free(void* p);
 
 /* ------------------------------------------------------------------------------------------------
+ * HEVC intra encoder (GPU): n same-sized 8-bit pictures (a grid's tiles, or one image) per call, analysis / reconstruction
+ * and CABAC as sm_90a kernels, parameter sets / slice header / emulation prevention on the host.  Output framing as
+ * b200_hevc_encode_intra: VPS, SPS, PPS and one IDR slice segment, each behind its uint32 BE length.
+ * Coding decisions are deterministic (no LCG): the same input gives the same bytes, alone or in any batch.
+ * Accepted b200_hevc_enc_params: width / height 8..16384 (coded size rounded up to 8, conformance window), log2_ctb_size 5
+ * or 6, qp / init_qp 0..51, wpp = 1 (required), max_transform_hierarchy_depth_intra, strong_intra_smoothing, PPS and slice
+ * Cb / Cr QP offsets, every deblocking field, still_picture, VUI / colour fields.  mode_decision, split_threshold and seed
+ * are ignored.  B200_E_UNSUPPORTED (message names the field): sao, sign_data_hiding, transform_skip, cu_qp_delta,
+ * scaling_lists, pcm, transquant_bypass, tile_cols / tile_rows > 1, slice_ctb_rows, dependent_slice_segments, bit_depth != 8,
+ * chroma_format_idc 2 / 3, wpp = 0.  All validation happens before any CUDA call.
+ * Pictures: b200_planes with width / height = the params', chroma B200_CHROMA_420 (chroma_format_idc 1) or B200_CHROMA_MONO
+ * (0, cb / cr ignored), bit_depth 8.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct b200_gpu_encoder b200_gpu_encoder;
+typedef struct b200_gpu_encode_stats {
+  double analyse_ms, entropy_ms;     /* CUDA events: E1 (analysis + reconstruction), E2 (CABAC) of the last call */
+  double framing_ms, total_ms;       /* host clock: sub-stream D2H + framing; the whole call */
+  uint64_t bytes, ctus, pictures;    /* access-unit bytes, CTBs and pictures of the last call */
+} b200_gpu_encode_stats;
+
+/* Host only, no CUDA: B200_OK if b200_gpu_encode_intra_* would accept these arguments, else the code and message it would
+   return (the encode calls run the same check first). */
+int b200_gpu_encode_check(const b200_hevc_enc_params* p, int n, const b200_planes* pics);
+int b200_gpu_encoder_create(b200_gpu_encoder** enc);      /* on the current CUDA device */
+void b200_gpu_encoder_destroy(b200_gpu_encoder* enc);
+/* device planes; `stream` = cudaStream_t (NULL = default stream); returns when the access units are in host memory */
+int b200_gpu_encode_intra_device(b200_gpu_encoder* enc, const b200_hevc_enc_params* p, int n, const b200_planes* pics, void* stream);
+/* host planes (staged through a page-locked bounce buffer) */
+int b200_gpu_encode_intra_host(b200_gpu_encoder* enc, const b200_hevc_enc_params* p, int n, const b200_planes* pics);
+/* access unit of picture i of the last call (valid until the next call on this encoder) */
+int b200_gpu_encoder_output(b200_gpu_encoder* enc, int i, const uint8_t** data, size_t* size);
+/* picture i of the last call as reconstructed before in-loop filtering, cropped to width x height (host copy): what a decoder
+   holds before deblocking.  cb / cr may be NULL. */
+int b200_gpu_encoder_read_recon(b200_gpu_encoder* enc, int i, void* y, void* cb, void* cr, size_t y_stride, size_t c_stride);
+int b200_gpu_encoder_get_stats(b200_gpu_encoder* enc, b200_gpu_encode_stats* out);
+/* Host only: bytes reserved per CABAC sub-stream (one CTB row) -- the worst case of the syntax; a sub-stream that would need
+   more fails the call instead of writing past it. */
+size_t b200_gpu_encoder_substream_capacity(int width, int log2_ctb_size, int chroma_format_idc);
+
+/* ------------------------------------------------------------------------------------------------
  * HEVC intra decoder: header parsing on the host; CABAC + slice-data syntax, reconstruction, deblocking and SAO as
  * sm_90a kernels (CABAC can be moved to host threads with b200_decoder_set_front_end).
  * Replaces: the libde265 calls of libheif/plugins/decoder_libde265.cc -- de265_new_decoder :181,

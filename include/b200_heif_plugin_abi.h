@@ -117,6 +117,8 @@ extern b200h_plugin_info plugin_info;
 extern b200h_plugin_info b200_encoder_plugin_info;
 const b200h_decoder_plugin* b200_get_decoder_plugin(void);
 const b200h_encoder_plugin* b200_get_encoder_plugin(void);
+/* the GPU encoder's table (id "b200-gpu", priority 60): 8-bit 4:2:0 / monochrome input, log2-ctb-size 5..6, WPP always on */
+const b200h_encoder_plugin* b200_get_gpu_encoder_plugin(void);
 int b200_plugin_bind_libheif(void* dl_handle);
 /* Submission queue of the decoder plugin (concurrent decode_next_image2 calls are decoded as one batch, see b200_plugin.cc):
    out3 = {batches decoded, pictures decoded, largest batch}. */

@@ -9,8 +9,7 @@
 // DST 4x4, transform skip, sign-data hiding, cu_qp_delta, chroma QP offsets, SAO band/edge with merges,
 // deblocking overrides, WPP entry points, multiple slices and dependent slice segments, 8..12 bit,
 // 4:2:0 and 4:0:0.  Syntax follows ITU-T H.265 7.3 / 9.3; the reconstruction loop follows 8.4 / 8.6.
-#include "b200_internal.h"
-#include "b200_hevc_scaling.h"
+#include "b200_hevc_enc_headers.h"
 #include <algorithm>
 #include <vector>
 
@@ -96,18 +95,10 @@ static void init_tables() {
 
 static inline int clip3(int lo, int hi, int v) { return v < lo ? lo : (v > hi ? hi : v); }
 
-// ------------------------------------------------------------------------------------------ bit I/O
-struct BitWriter {
-  std::vector<uint8_t> buf; int nbits = 0; uint8_t cur = 0;
-  void put(unsigned v, int n) { for (int i = n - 1; i >= 0; i--) { cur = (uint8_t)((cur << 1) | ((v >> i) & 1)); if (++nbits == 8) { buf.push_back(cur); cur = 0; nbits = 0; } } }
-  void ue(unsigned v) { unsigned x = v + 1; int len = 0; while ((x >> len) > 1) len++; put(0, len); put(x, len + 1); }
-  void se(int v) { ue(v > 0 ? 2 * v - 1 : -2 * v); }
-  void trailing() { put(1, 1); while (nbits) put(0, 1); }
-  void align_zero() { while (nbits) put(0, 1); }
-};
-
-static void append_nal(std::vector<uint8_t>& out, int type, const std::vector<uint8_t>& rbsp) {
+// ------------------------------------------------------------------------------------------ NAL framing
+void append_nal(std::vector<uint8_t>& out, int type, const std::vector<uint8_t>& rbsp) {
   std::vector<uint8_t> nal;
+  nal.reserve(rbsp.size() + rbsp.size() / 64 + 2);
   nal.push_back((uint8_t)(type << 1)); nal.push_back(1);
   int zeros = 0;
   for (uint8_t b : rbsp) {
@@ -119,10 +110,187 @@ static void append_nal(std::vector<uint8_t>& out, int type, const std::vector<ui
   out.push_back((uint8_t)(n >> 24)); out.push_back((uint8_t)(n >> 16)); out.push_back((uint8_t)(n >> 8)); out.push_back((uint8_t)n);
   out.insert(out.end(), nal.begin(), nal.end());
 }
-static size_t escaped_size(const std::vector<uint8_t>& d) {
+size_t escaped_size(const uint8_t* d, size_t len) {
   size_t n = 0; int zeros = 0;
-  for (uint8_t b : d) { if (zeros >= 2 && b <= 3) { n++; zeros = 0; } n++; zeros = b == 0 ? zeros + 1 : 0; }
+  for (size_t i = 0; i < len; i++) { const uint8_t b = d[i]; if (zeros >= 2 && b <= 3) { n++; zeros = 0; } n++; zeros = b == 0 ? zeros + 1 : 0; }
   return n;
+}
+
+// ------------------------------------------------------------------------------------------ parameter sets, slice header
+static void write_scaling_list_data(BitWriter& b, const SeqHeader& s) {          // 7.3.4
+  for (int sz = 0; sz < 4; sz++) for (int m = 0; m < 6; m += (sz == 3 ? 3 : 1)) {
+    if (s.sl_kind[sz][m] < 2) { b.put(0, 1); b.ue(s.sl_kind[sz][m]); continue; }   // pred_mode_flag = 0: delta 0 = default, 1 = previous matrix
+    b.put(1, 1);
+    int next = 8; const int num = sz == 0 ? 16 : 64;
+    if (sz > 1) { b.se((int)s.sl_lists->dc[sz][m] - 8); next = s.sl_lists->dc[sz][m]; }
+    for (int i = 0; i < num; i++) { int d = (int)s.sl_lists->list[sz][m][i] - next; if (d > 127) d -= 256; if (d < -128) d += 256; b.se(d); next = s.sl_lists->list[sz][m][i]; }
+  }
+}
+
+static void profile_tier_level(BitWriter& b, const SeqHeader& s) {
+  const b200_hevc_enc_params& P = *s.P;
+  const int cfmt = s.cfmt, bd = s.bd, chroma = s.chroma;
+  int profile = cfmt >= 2 ? 4 : (bd == 8 ? (P.still_picture ? 3 : 1) : (bd == 10 && chroma ? 2 : 4));
+  b.put(0, 2); b.put(0, 1); b.put(profile, 5);
+  uint32_t compat = 0;
+  if (profile == 1) compat = (1u << 30) | (1u << 29);       // Main => also Main 10 compatible
+  else if (profile == 2) compat = 1u << 29;
+  else if (profile == 3) compat = (1u << 28) | (1u << 30) | (1u << 29);
+  else compat = 1u << 27;
+  b.put(compat, 32);
+  b.put(1, 1); b.put(0, 1); b.put(0, 1); b.put(1, 1);        // progressive, !interlaced, !non_packed, frame_only
+  if (profile == 4) {                                         // RExt constraint flags: Main 12 / Monochrome 12 family
+    b.put(1, 1);                                              // max_12bit_constraint
+    b.put(bd <= 10, 1); b.put(bd <= 8, 1);                    // max_10bit, max_8bit
+    b.put(cfmt <= 2, 1); b.put(cfmt <= 1, 1); b.put(chroma == 0, 1);   // max_422chroma, max_420chroma, max_monochrome
+    b.put(1, 1); b.put(1, 1); b.put(1, 1);                    // intra, one_picture_only, lower_bit_rate
+    b.put(0, 32); b.put(0, 2);                                // reserved 34 bits
+  } else { b.put(0, 32); b.put(0, 11); }
+  b.put(0, 1);                                                // general_inbld / reserved
+  long px = (long)s.W * s.H;
+  int level = px <= 36864 ? 30 : px <= 122880 ? 60 : px <= 245760 ? 63 : px <= 552960 ? 90 : px <= 983040 ? 93 :
+              px <= 2228224 ? 120 : px <= 8912896 ? 150 : 180;
+  b.put(level, 8);
+}
+
+void write_vps(std::vector<uint8_t>& out, const SeqHeader& s) {
+  BitWriter b;
+  b.put(0, 4); b.put(1, 1); b.put(1, 1); b.put(0, 6); b.put(0, 3); b.put(1, 1); b.put(0xffff, 16);
+  profile_tier_level(b, s);
+  b.put(1, 1);                      // sub_layer_ordering_info_present
+  b.ue(0); b.ue(0); b.ue(0);        // max_dec_pic_buffering_minus1, num_reorder, max_latency
+  b.put(0, 6); b.ue(0);             // max_layer_id, num_layer_sets_minus1
+  b.put(0, 1);                      // timing_info_present
+  b.put(0, 1);                      // extension
+  b.trailing();
+  append_nal(out, 32, b.buf);
+}
+
+void write_sps(std::vector<uint8_t>& out, const SeqHeader& s) {
+  const b200_hevc_enc_params& P = *s.P;
+  BitWriter b;
+  b.put(0, 4); b.put(0, 3); b.put(1, 1);
+  profile_tier_level(b, s);
+  b.ue(0);
+  b.ue(s.cfmt);
+  if (s.cfmt == 3) b.put(0, 1);                                 // separate_colour_plane_flag
+  b.ue(s.W); b.ue(s.H);
+  int cr = (s.W - P.width) >> (s.chroma ? s.sx : 0), cbm = (s.H - P.height) >> (s.chroma ? s.sy : 0);     // conformance window in chroma units
+  if (cr || cbm) { b.put(1, 1); b.ue(0); b.ue(cr); b.ue(0); b.ue(cbm); } else b.put(0, 1);
+  b.ue(s.bd - 8); b.ue(s.bd - 8);
+  b.ue(4);                          // log2_max_pic_order_cnt_lsb_minus4
+  b.put(1, 1); b.ue(0); b.ue(0); b.ue(0);
+  b.ue(0);                          // log2_min_luma_coding_block_size_minus3 (8)
+  b.ue(s.log2ctb - 3);
+  b.ue(s.log2_min_tb - 2); b.ue(s.log2_max_tb - s.log2_min_tb);
+  b.ue(0); b.ue(s.max_th_depth);
+  b.put(s.sl_on ? 1 : 0, 1);        // scaling_list_enabled
+  if (s.sl_on) { b.put(P.scaling_lists == 2 ? 1 : 0, 1); if (P.scaling_lists == 2) write_scaling_list_data(b, s); }
+  b.put(0, 1);                      // amp
+  b.put(P.sao ? 1 : 0, 1);
+  b.put(P.pcm ? 1 : 0, 1);          // pcm_enabled
+  if (P.pcm) {
+    b.put(s.pcm_bd_y - 1, 4); b.put(s.pcm_bd_c - 1, 4);
+    b.ue(0); b.ue(std::min(5, s.log2ctb) - 3);                    // Log2MinIpcmCbSizeY = 3, Log2MaxIpcmCbSizeY = min(CtbLog2SizeY, 5)
+    b.put(P.pcm == 2 ? 1 : 0, 1);                                 // pcm_loop_filter_disabled_flag
+  }
+  b.ue(0);                          // num_short_term_ref_pic_sets
+  b.put(0, 1);                      // long_term_ref_pics_present
+  b.put(0, 1);                      // temporal_mvp
+  b.put(P.strong_intra_smoothing ? 1 : 0, 1);
+  if (P.vui_present) {
+    b.put(1, 1);
+    b.put(0, 1); b.put(0, 1);       // aspect_ratio_info, overscan_info
+    b.put(1, 1);                    // video_signal_type_present
+    b.put(5, 3); b.put(P.full_range ? 1 : 0, 1);
+    if (P.colour_description_present) { b.put(1, 1); b.put(P.colour_primaries, 8); b.put(P.transfer_characteristics, 8); b.put(P.matrix_coefficients, 8); }
+    else b.put(0, 1);
+    b.put(0, 1); b.put(0, 1); b.put(0, 1); b.put(0, 1);   // chroma_loc, neutral_chroma, field_seq, frame_field_info
+    b.put(0, 1); b.put(0, 1); b.put(0, 1);                // default_display_window, timing_info, bitstream_restriction
+  } else b.put(0, 1);
+  b.put(0, 1);                      // sps_extension_present
+  b.trailing();
+  append_nal(out, 33, b.buf);
+}
+
+void write_pps(std::vector<uint8_t>& out, const SeqHeader& s) {
+  const b200_hevc_enc_params& P = *s.P;
+  BitWriter b;
+  b.ue(0); b.ue(0);
+  b.put(P.dependent_slice_segments ? 1 : 0, 1);
+  b.put(0, 1); b.put(0, 3);
+  b.put(P.sign_data_hiding ? 1 : 0, 1);
+  b.put(0, 1);
+  b.ue(0); b.ue(0);
+  b.se(P.init_qp - 26);
+  b.put(0, 1);                      // constrained_intra_pred
+  b.put(P.transform_skip ? 1 : 0, 1);
+  b.put(P.cu_qp_delta ? 1 : 0, 1);
+  if (P.cu_qp_delta) b.ue(s.log2ctb - s.qg_log2);
+  b.se(P.cb_qp_offset); b.se(P.cr_qp_offset);
+  b.put(P.slice_chroma_qp_offsets ? 1 : 0, 1);
+  b.put(0, 1); b.put(0, 1);
+  b.put(P.transquant_bypass ? 1 : 0, 1);   // transquant_bypass_enabled
+  b.put(s.tiles ? 1 : 0, 1);        // tiles_enabled_flag
+  b.put(P.wpp ? 1 : 0, 1);
+  if (s.tiles) {
+    const std::vector<int>& col_bd = *s.col_bd; const std::vector<int>& row_bd = *s.row_bd;
+    b.ue((unsigned)col_bd.size() - 2); b.ue((unsigned)row_bd.size() - 2);
+    b.put(P.tiles_uniform ? 1 : 0, 1);
+    if (!P.tiles_uniform) {
+      for (size_t i = 0; i + 2 < col_bd.size(); i++) b.ue((unsigned)(col_bd[i + 1] - col_bd[i] - 1));
+      for (size_t i = 0; i + 2 < row_bd.size(); i++) b.ue((unsigned)(row_bd[i + 1] - row_bd[i] - 1));
+    }
+    b.put(P.loop_filter_across_tiles ? 1 : 0, 1);
+  }
+  b.put(P.loop_filter_across_slices ? 1 : 0, 1);
+  b.put(1, 1);                      // deblocking_filter_control_present
+  b.put(1, 1);                      // deblocking_filter_override_enabled
+  b.put(P.deblocking_disabled ? 1 : 0, 1);
+  if (!P.deblocking_disabled) { b.se(P.beta_offset_div2); b.se(P.tc_offset_div2); }
+  b.put(P.scaling_lists == 3 ? 1 : 0, 1);   // pps_scaling_list_data_present
+  if (P.scaling_lists == 3) write_scaling_list_data(b, s);
+  b.put(0, 1);                      // lists_modification_present
+  b.ue(0);                          // log2_parallel_merge_level_minus2
+  b.put(0, 1);                      // slice_segment_header_extension_present
+  b.put(0, 1);                      // pps_extension_present
+  b.trailing();
+  append_nal(out, 34, b.buf);
+}
+
+void write_slice_header(BitWriter& b, const SeqHeader& s, int addr0, bool dependent, int slice_qp, const std::vector<size_t>& escaped) {
+  const b200_hevc_enc_params& P = *s.P;
+  const int total = ((s.W + (1 << s.log2ctb) - 1) >> s.log2ctb) * ((s.H + (1 << s.log2ctb) - 1) >> s.log2ctb);
+  bool first = addr0 == 0;
+  b.put(first ? 1 : 0, 1);
+  b.put(0, 1);                                           // no_output_of_prior_pics (IRAP)
+  b.ue(0);
+  if (!first) {
+    if (P.dependent_slice_segments) b.put(dependent ? 1 : 0, 1);
+    int bits = 0; while ((1 << bits) < total) bits++;
+    b.put(addr0, bits);
+  }
+  if (!dependent) {
+    b.ue(2);                                             // slice_type I
+    if (P.sao) { b.put(1, 1); if (s.chroma) b.put(1, 1); }
+    b.se(slice_qp - P.init_qp);
+    if (P.slice_chroma_qp_offsets) { b.se(P.slice_cb_qp_offset); b.se(P.slice_cr_qp_offset); }
+    bool override = P.slice_deblocking_override != 0;
+    b.put(override ? 1 : 0, 1);
+    bool dis = P.deblocking_disabled;
+    if (override) {
+      dis = P.slice_deblocking_disabled != 0;
+      b.put(dis ? 1 : 0, 1);
+      if (!dis) { b.se(P.slice_beta_offset_div2); b.se(P.slice_tc_offset_div2); }
+    }
+    if (P.loop_filter_across_slices && (P.sao || !dis)) b.put(P.slice_loop_filter_across_slices ? 1 : 0, 1);
+  }
+  if (P.wpp || s.tiles) {
+    int ne = (int)escaped.size() - 1;
+    b.ue(ne);
+    if (ne > 0) { b.ue(31); for (int i = 0; i < ne; i++) b.put((unsigned)(escaped[i] - 1), 32); }
+  }
+  b.trailing();                                          // byte_alignment()
 }
 
 // ------------------------------------------------------------------------------------------ CABAC encoder (9.3.4.5)
@@ -289,15 +457,6 @@ class Encoder {
   sl::Lists sl_lists; sl::Factors sl_f; uint8_t sl_kind[4][6] = {}; bool sl_on = false;
   int pcm_bd_y = 8, pcm_bd_c = 8; bool cu_bypass = false;
 
-  void write_scaling_list_data(BitWriter& b) {                    // 7.3.4
-    for (int s = 0; s < 4; s++) for (int m = 0; m < 6; m += (s == 3 ? 3 : 1)) {
-      if (sl_kind[s][m] < 2) { b.put(0, 1); b.ue(sl_kind[s][m]); continue; }       // pred_mode_flag = 0: delta 0 = default, 1 = previous matrix
-      b.put(1, 1);
-      int next = 8; const int num = s == 0 ? 16 : 64;
-      if (s > 1) { b.se((int)sl_lists.dc[s][m] - 8); next = sl_lists.dc[s][m]; }
-      for (int i = 0; i < num; i++) { int d = (int)sl_lists.list[s][m][i] - next; if (d > 127) d -= 256; if (d < -128) d += 256; b.se(d); next = sl_lists.list[s][m][i]; }
-    }
-  }
   int scaling_factor(int c, int log2n, int pos) const {          // m[x][y] of 8.6.4.2 for raster position pos of an n x n block
     if (!sl_on) return 16;
     const int n = 1 << log2n, x = pos & (n - 1), y = pos >> log2n, sid = log2n - 2;
@@ -314,128 +473,13 @@ class Encoder {
   }
 
   // ---------------------------------------------------------------------------- parameter sets
-  void profile_tier_level(BitWriter& b) {
-    int profile = cfmt >= 2 ? 4 : (bd == 8 ? (P.still_picture ? 3 : 1) : (bd == 10 && chroma ? 2 : 4));
-    b.put(0, 2); b.put(0, 1); b.put(profile, 5);
-    uint32_t compat = 0;
-    if (profile == 1) compat = (1u << 30) | (1u << 29);       // Main => also Main 10 compatible
-    else if (profile == 2) compat = 1u << 29;
-    else if (profile == 3) compat = (1u << 28) | (1u << 30) | (1u << 29);
-    else compat = 1u << 27;
-    b.put(compat, 32);
-    b.put(1, 1); b.put(0, 1); b.put(0, 1); b.put(1, 1);        // progressive, !interlaced, !non_packed, frame_only
-    if (profile == 4) {                                         // RExt constraint flags: Main 12 / Monochrome 12 family
-      b.put(1, 1);                                              // max_12bit_constraint
-      b.put(bd <= 10, 1); b.put(bd <= 8, 1);                    // max_10bit, max_8bit
-      b.put(cfmt <= 2, 1); b.put(cfmt <= 1, 1); b.put(chroma == 0, 1);   // max_422chroma, max_420chroma, max_monochrome
-      b.put(1, 1); b.put(1, 1); b.put(1, 1);                    // intra, one_picture_only, lower_bit_rate
-      b.put(0, 32); b.put(0, 2);                                // reserved 34 bits
-    } else { b.put(0, 32); b.put(0, 11); }
-    b.put(0, 1);                                                // general_inbld / reserved
-    long px = (long)W * H;
-    int level = px <= 36864 ? 30 : px <= 122880 ? 60 : px <= 245760 ? 63 : px <= 552960 ? 90 : px <= 983040 ? 93 :
-                px <= 2228224 ? 120 : px <= 8912896 ? 150 : 180;
-    b.put(level, 8);
+  SeqHeader seq_header() const {
+    return SeqHeader{&P, W, H, cfmt, chroma, sx, sy, bd, log2ctb, log2_min_tb, log2_max_tb, max_th_depth, qg_log2, pcm_bd_y, pcm_bd_c,
+                     sl_on, sl_kind, &sl_lists, tiles, &col_bd, &row_bd};
   }
-  void write_vps(std::vector<uint8_t>& out) {
-    BitWriter b;
-    b.put(0, 4); b.put(1, 1); b.put(1, 1); b.put(0, 6); b.put(0, 3); b.put(1, 1); b.put(0xffff, 16);
-    profile_tier_level(b);
-    b.put(1, 1);                      // sub_layer_ordering_info_present
-    b.ue(0); b.ue(0); b.ue(0);        // max_dec_pic_buffering_minus1, num_reorder, max_latency
-    b.put(0, 6); b.ue(0);             // max_layer_id, num_layer_sets_minus1
-    b.put(0, 1);                      // timing_info_present
-    b.put(0, 1);                      // extension
-    b.trailing();
-    append_nal(out, 32, b.buf);
-  }
-  void write_sps(std::vector<uint8_t>& out) {
-    BitWriter b;
-    b.put(0, 4); b.put(0, 3); b.put(1, 1);
-    profile_tier_level(b);
-    b.ue(0);
-    b.ue(cfmt);
-    if (cfmt == 3) b.put(0, 1);                                   // separate_colour_plane_flag
-    b.ue(W); b.ue(H);
-    int cr = (W - P.width) >> (chroma ? sx : 0), cbm = (H - P.height) >> (chroma ? sy : 0);     // conformance window in chroma units
-    if (cr || cbm) { b.put(1, 1); b.ue(0); b.ue(cr); b.ue(0); b.ue(cbm); } else b.put(0, 1);
-    b.ue(bd - 8); b.ue(bd - 8);
-    b.ue(4);                          // log2_max_pic_order_cnt_lsb_minus4
-    b.put(1, 1); b.ue(0); b.ue(0); b.ue(0);
-    b.ue(0);                          // log2_min_luma_coding_block_size_minus3 (8)
-    b.ue(log2ctb - 3);
-    b.ue(log2_min_tb - 2); b.ue(log2_max_tb - log2_min_tb);
-    b.ue(0); b.ue(max_th_depth);
-    b.put(sl_on ? 1 : 0, 1);          // scaling_list_enabled
-    if (sl_on) { b.put(P.scaling_lists == 2 ? 1 : 0, 1); if (P.scaling_lists == 2) write_scaling_list_data(b); }
-    b.put(0, 1);                      // amp
-    b.put(P.sao ? 1 : 0, 1);
-    b.put(P.pcm ? 1 : 0, 1);          // pcm_enabled
-    if (P.pcm) {
-      b.put(pcm_bd_y - 1, 4); b.put(pcm_bd_c - 1, 4);
-      b.ue(0); b.ue(std::min(5, log2ctb) - 3);                      // Log2MinIpcmCbSizeY = 3, Log2MaxIpcmCbSizeY = min(CtbLog2SizeY, 5)
-      b.put(P.pcm == 2 ? 1 : 0, 1);                                 // pcm_loop_filter_disabled_flag
-    }
-    b.ue(0);                          // num_short_term_ref_pic_sets
-    b.put(0, 1);                      // long_term_ref_pics_present
-    b.put(0, 1);                      // temporal_mvp
-    b.put(P.strong_intra_smoothing ? 1 : 0, 1);
-    if (P.vui_present) {
-      b.put(1, 1);
-      b.put(0, 1); b.put(0, 1);       // aspect_ratio_info, overscan_info
-      b.put(1, 1);                    // video_signal_type_present
-      b.put(5, 3); b.put(P.full_range ? 1 : 0, 1);
-      if (P.colour_description_present) { b.put(1, 1); b.put(P.colour_primaries, 8); b.put(P.transfer_characteristics, 8); b.put(P.matrix_coefficients, 8); }
-      else b.put(0, 1);
-      b.put(0, 1); b.put(0, 1); b.put(0, 1); b.put(0, 1);   // chroma_loc, neutral_chroma, field_seq, frame_field_info
-      b.put(0, 1); b.put(0, 1); b.put(0, 1);                // default_display_window, timing_info, bitstream_restriction
-    } else b.put(0, 1);
-    b.put(0, 1);                      // sps_extension_present
-    b.trailing();
-    append_nal(out, 33, b.buf);
-  }
-  void write_pps(std::vector<uint8_t>& out) {
-    BitWriter b;
-    b.ue(0); b.ue(0);
-    b.put(P.dependent_slice_segments ? 1 : 0, 1);
-    b.put(0, 1); b.put(0, 3);
-    b.put(P.sign_data_hiding ? 1 : 0, 1);
-    b.put(0, 1);
-    b.ue(0); b.ue(0);
-    b.se(P.init_qp - 26);
-    b.put(0, 1);                      // constrained_intra_pred
-    b.put(P.transform_skip ? 1 : 0, 1);
-    b.put(P.cu_qp_delta ? 1 : 0, 1);
-    if (P.cu_qp_delta) b.ue(log2ctb - qg_log2);
-    b.se(P.cb_qp_offset); b.se(P.cr_qp_offset);
-    b.put(P.slice_chroma_qp_offsets ? 1 : 0, 1);
-    b.put(0, 1); b.put(0, 1);
-    b.put(P.transquant_bypass ? 1 : 0, 1);   // transquant_bypass_enabled
-    b.put(tiles ? 1 : 0, 1);          // tiles_enabled_flag
-    b.put(P.wpp ? 1 : 0, 1);
-    if (tiles) {
-      b.ue((unsigned)col_bd.size() - 2); b.ue((unsigned)row_bd.size() - 2);
-      b.put(P.tiles_uniform ? 1 : 0, 1);
-      if (!P.tiles_uniform) {
-        for (size_t i = 0; i + 2 < col_bd.size(); i++) b.ue((unsigned)(col_bd[i + 1] - col_bd[i] - 1));
-        for (size_t i = 0; i + 2 < row_bd.size(); i++) b.ue((unsigned)(row_bd[i + 1] - row_bd[i] - 1));
-      }
-      b.put(P.loop_filter_across_tiles ? 1 : 0, 1);
-    }
-    b.put(P.loop_filter_across_slices ? 1 : 0, 1);
-    b.put(1, 1);                      // deblocking_filter_control_present
-    b.put(1, 1);                      // deblocking_filter_override_enabled
-    b.put(P.deblocking_disabled ? 1 : 0, 1);
-    if (!P.deblocking_disabled) { b.se(P.beta_offset_div2); b.se(P.tc_offset_div2); }
-    b.put(P.scaling_lists == 3 ? 1 : 0, 1);   // pps_scaling_list_data_present
-    if (P.scaling_lists == 3) write_scaling_list_data(b);
-    b.put(0, 1);                      // lists_modification_present
-    b.ue(0);                          // log2_parallel_merge_level_minus2
-    b.put(0, 1);                      // slice_segment_header_extension_present
-    b.put(0, 1);                      // pps_extension_present
-    b.trailing();
-    append_nal(out, 34, b.buf);
-  }
+  void write_vps(std::vector<uint8_t>& out) { enc::write_vps(out, seq_header()); }
+  void write_sps(std::vector<uint8_t>& out) { enc::write_sps(out, seq_header()); }
+  void write_pps(std::vector<uint8_t>& out) { enc::write_pps(out, seq_header()); }
 
   // ---------------------------------------------------------------------------- slice segment
   void encode_slice_segment(std::vector<uint8_t>& out, int addr0, int addr1, bool dependent, int slice_addr) {
@@ -484,36 +528,9 @@ class Encoder {
     substreams.push_back(cabac.bw.buf);
     // header
     BitWriter b;
-    bool first = addr0 == 0;
-    b.put(first ? 1 : 0, 1);
-    b.put(0, 1);                                           // no_output_of_prior_pics (IRAP)
-    b.ue(0);
-    if (!first) {
-      if (P.dependent_slice_segments) b.put(dependent ? 1 : 0, 1);
-      int bits = 0; while ((1 << bits) < total) bits++;
-      b.put(addr0, bits);
-    }
-    if (!dependent) {
-      b.ue(2);                                             // slice_type I
-      if (P.sao) { b.put(1, 1); if (chroma) b.put(1, 1); }
-      b.se(slice_qp - P.init_qp);
-      if (P.slice_chroma_qp_offsets) { b.se(P.slice_cb_qp_offset); b.se(P.slice_cr_qp_offset); }
-      bool override = P.slice_deblocking_override != 0;
-      b.put(override ? 1 : 0, 1);
-      bool dis = P.deblocking_disabled;
-      if (override) {
-        dis = P.slice_deblocking_disabled != 0;
-        b.put(dis ? 1 : 0, 1);
-        if (!dis) { b.se(P.slice_beta_offset_div2); b.se(P.slice_tc_offset_div2); }
-      }
-      if (P.loop_filter_across_slices && (P.sao || !dis)) b.put(P.slice_loop_filter_across_slices ? 1 : 0, 1);
-    }
-    if (P.wpp || tiles) {
-      int ne = (int)substreams.size() - 1;
-      b.ue(ne);
-      if (ne > 0) { b.ue(31); for (int i = 0; i < ne; i++) b.put((unsigned)(escaped_size(substreams[i]) - 1), 32); }
-    }
-    b.trailing();                                          // byte_alignment()
+    std::vector<size_t> escaped;
+    for (auto& ss : substreams) escaped.push_back(escaped_size(ss.data(), ss.size()));
+    write_slice_header(b, seq_header(), addr0, dependent, slice_qp, escaped);
     std::vector<uint8_t> rbsp = b.buf;
     for (auto& s : substreams) rbsp.insert(rbsp.end(), s.begin(), s.end());
     append_nal(out, 19 /* IDR_W_RADL */, rbsp);

@@ -1,0 +1,1012 @@
+// b200_hevc_gpu_enc.cu -- HEVC intra encoder on the GPU: N same-sized 8-bit 4:2:0 / 4:0:0 pictures per call.
+//
+//   E1 (analyse + reconstruct), one warp per (picture, CTB row): CU quadtree from the CTB down to 8x8 (NxN at 8x8), decided
+//      bottom-up on J = SATD(prediction residual) + lambda(QP) * estimated mode bits; all 35 luma modes at every PU size, in
+//      closed loop (neighbours from the encoder's own reconstruction); chroma = DM; TU = CU (implicit splits: NxN, > 32);
+//      forward DST 4x4 / DCT 4..32, uniform quantisation with the intra rounding offset 171/512, reconstruction with the
+//      inverse path of 8.6.  Writes the reconstruction (HBM plane: the neighbours of the next row), the luma modes per 4x4,
+//      the CU size / partition per 8x8 and the quantised levels (a coefficient plane: every TB's levels at its position).
+//      Rows trail the row above by two CTBs through per-row progress counters.
+//   E2 (CABAC), one warp per WPP sub-stream (= CTB row): the syntax of 7.3.8 from E1's records, the arithmetic coder of
+//      9.3.4.5, context hand-over after the 2nd CTB of the row above (9.3.2.2), end_of_slice_segment_flag per CTB and
+//      end_of_subset_one_bit + byte alignment per row, into a per-row buffer sized for the worst case.
+//   Framing (host): parameter sets and slice header (b200_hevc_enc_headers.h, shared with the host encoder), entry points
+//      over the escaped sub-stream sizes, emulation prevention, length prefixes.
+//
+// Prediction, transforms and dequantisation are written here rather than taken from the reconstruction kernel
+// (b200_hevc_recon.cu): its predict_tb reconstructs one TB of a known mode inside K1's per-lane padded tile, from a packed
+// descriptor whose neighbour availability is precomputed as index intervals, and residual4_lane / residual_big consume sparse
+// CoefEntry lists.  The mode search needs the predicted sample of any of the 35 modes at any position as a pure function,
+// many modes per block without reconstructing, and dense residual blocks; both files are separate translation units built
+// without relocatable device code.  The tests pin the result bit-exact against that decoder, the C restatement and FFmpeg.
+#include "b200_internal.h"
+#include "b200_staging.h"
+#include "b200_hevc_enc_headers.h"
+#include "b200_hevc_syntax.h"
+#include <algorithm>
+#include <chrono>
+#include <memory>
+#include <vector>
+
+#define GE_LANES 32
+#define GE_SYNC() __syncwarp()
+#define GE_ATOMIC_ADD(p, v) atomicAdd((p), (v))
+#define GE_LD(p) __ldcg(p)          // planes written by other rows' warps (other SMs): bypass the non-coherent L1
+
+namespace b200 {
+namespace genc {
+
+using syn::clip3;
+
+B200_TABLE(int8_t, kDctT, [32], {64, 90, 90, 90, 89, 88, 87, 85, 83, 82, 80, 78, 75, 73, 70, 67,
+                                 64, 61, 57, 54, 50, 46, 43, 38, 36, 31, 25, 22, 18, 13, 9, 4})
+B200_TABLE(int8_t, kDst4, [4][4], {{29, 55, 74, 84}, {74, 74, 0, -74}, {84, -29, -74, 55}, {55, -84, 74, -29}})
+B200_TABLE(int8_t, kAngle, [35], {0, 0, 32, 26, 21, 17, 13, 9, 5, 2, 0, -2, -5, -9, -13, -17, -21, -26, -32,
+                                  -26, -21, -17, -13, -9, -5, -2, 0, 2, 5, 9, 13, 17, 21, 26, 32})
+B200_TABLE(int16_t, kInvAngle, [35], {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, -4096, -1638, -910, -630, -482, -390, -315, -256,
+                                      -315, -390, -482, -630, -910, -1638, -4096, 0, 0, 0, 0, 0, 0, 0, 0, 0})
+B200_TABLE(int32_t, kQuantScale, [6], {26214, 23302, 20560, 18396, 16384, 14564})
+B200_TABLE(uint8_t, kLevelScale, [6], {40, 45, 51, 57, 64, 72})
+B200_TABLE(uint8_t, kLastGroup, [32], {0, 1, 2, 3, 4, 4, 5, 5, 6, 6, 6, 6, 7, 7, 7, 7, 8, 8, 8, 8, 8, 8, 8, 8, 9, 9, 9, 9, 9, 9, 9, 9})
+B200_TABLE(uint8_t, kLastGroupMin, [10], {0, 1, 2, 3, 4, 6, 8, 12, 16, 24})
+
+enum { CU_NXN = 0x80 };
+
+// Worst case of one sub-stream, in bytes per sample of the CTB row, plus a fixed allowance per CTB.  Per coefficient:
+// sig / gt1 / gt2 context bins (at most 6 renormalisation shifts = output bits each, rangeTabLps >= 6) + a sign bypass bin
+// + coeff_abs_level_remaining of a level <= 32767 (at most 32 bypass bins) = 51 bits; 8x8 CUs coded as NxN add per 96
+// samples six TBs of last-position / cbf / csbf bins and the CU header: below 64 bits = 8 bytes per sample in total.
+constexpr int kBytesPerSample = 8, kBytesPerCtb = 64;
+inline size_t substream_capacity(int width, int log2ctb, int cfmt) {
+  const int ctb = 1 << log2ctb, wctb = (((width + 7) & ~7) + ctb - 1) >> log2ctb;
+  const size_t samples = (size_t)ctb * ctb * (cfmt ? 3 : 2) / 2;
+  return (size_t)wctb * (samples * kBytesPerSample + kBytesPerCtb);
+}
+
+struct Pic { const uint8_t* src[3]; size_t stride[3]; };
+
+struct Args {
+  const Pic* pics; int n;
+  int W, H, Wc, Hc, sw, sh;          // coded (multiples of 8) and source sizes (luma)
+  int cfmt, log2ctb, wctb, hctb, max_th_depth, strong, slice_qp, qp[3], lambda16;
+  uint8_t* rec; int16_t* coef; size_t pic_samples;          // per picture: Y (W x H), Cb, Cr (Wc x Hc)
+  uint8_t* ipm4; uint8_t* dec4; size_t map4;                 // per 4x4 luma: intra mode, reconstructed flag
+  uint8_t* cu8; size_t map8;                                 // per 8x8: log2 CU size | CU_NXN
+  unsigned* progress; unsigned* progress2; unsigned* ticket; unsigned* error;   // rows, rows, 2, 1
+  uint8_t* wpp_ctx;                                          // per row: CTX_COUNT context bytes after its 2nd CTB
+  uint8_t* ss; size_t ss_cap; unsigned* ss_len;              // per row sub-stream
+};
+
+// ---------------------------------------------------------------------------------------------------- E1 workspace
+struct Work {
+  int res[1024], tmp[1024], coef[1024];
+  int16_t lev[1024];
+  uint8_t pred[1024];
+  int16_t ref[2][132];               // neighbours (8.4.4.2.2): [0] substituted, [1] filtered
+  int satd[36];
+  int dc, any, acc, mode;
+  uint8_t save[4][4096 + 256];       // per quadtree depth: luma recon + modes of the no-split alternative
+};
+
+struct Ctx2 { const Args& a; int p; int lane; Work& w;
+  __device__ uint8_t* plane(int c) const { return a.rec + (size_t)p * a.pic_samples + (c == 0 ? 0 : (size_t)a.W * a.H + (size_t)(c - 1) * a.Wc * a.Hc); }
+  __device__ int16_t* cplane(int c) const { return a.coef + (size_t)p * a.pic_samples + (c == 0 ? 0 : (size_t)a.W * a.H + (size_t)(c - 1) * a.Wc * a.Hc); }
+  __device__ uint8_t* ipm() const { return a.ipm4 + (size_t)p * a.map4; }
+  __device__ uint8_t* dec() const { return a.dec4 + (size_t)p * a.map4; }
+  __device__ uint8_t* cu() const { return a.cu8 + (size_t)p * a.map8; }
+  __device__ int org(int c, int x, int y) const {                // edge padding of the source to the coded size
+    const int sw = c ? (a.sw + 1) >> 1 : a.sw, sh = c ? (a.sh + 1) >> 1 : a.sh;
+    return a.pics[p].src[c][(size_t)(y < sh ? y : sh - 1) * a.pics[p].stride[c] + (x < sw ? x : sw - 1)];
+  }
+  __device__ bool avail(int x, int y) const {                    // luma position reconstructed already (z-scan availability, one slice)
+    if (x < 0 || y < 0 || x >= a.W || y >= a.H) return false;
+    return GE_LD(dec() + (size_t)(y >> 2) * (a.W >> 2) + (x >> 2)) != 0;
+  }
+};
+
+__device__ inline int dct_coef(int log2n, int k, int x) {        // DCT matrix entry [k][x] of an n x n transform (8.6.4.2)
+  if (k == 0) return 64;
+  int j = ((k << (5 - log2n)) * (2 * x + 1)) & 127, sgn = 1;
+  if (j > 64) j = 128 - j;
+  if (j > 32) { j = 64 - j; sgn = -1; }
+  return sgn * B200_T(kDctT)[j];
+}
+__device__ inline int tmat(bool dst4, int log2n, int k, int x) { return dst4 ? B200_T(kDst4)[k][x] : dct_coef(log2n, k, x); }
+
+// 8.4.2: the three most probable modes of the PU at luma (x, y)
+__device__ inline void mpm_cand(const uint8_t* ipm, int w4, int log2ctb, int x, int y, int cand[3]) {
+  int ca = 1, cb = 1;
+  if (x > 0) ca = GE_LD(ipm + (size_t)(y >> 2) * w4 + ((x - 1) >> 2));
+  if (y > 0 && (y - 1) >= ((y >> log2ctb) << log2ctb)) cb = GE_LD(ipm + (size_t)((y - 1) >> 2) * w4 + (x >> 2));
+  if (ca == cb) {
+    if (ca < 2) { cand[0] = 0; cand[1] = 1; cand[2] = 26; }
+    else { cand[0] = ca; cand[1] = 2 + ((ca + 29) % 32); cand[2] = 2 + ((ca - 2 + 1) % 32); }
+  } else {
+    cand[0] = ca; cand[1] = cb;
+    if (ca != 0 && cb != 0) cand[2] = 0; else if (ca != 1 && cb != 1) cand[2] = 1; else cand[2] = 26;
+  }
+}
+__device__ inline int mode_bits(int mode, const int cand[3]) { return mode == cand[0] ? 2 : (mode == cand[1] || mode == cand[2]) ? 3 : 6; }
+
+// neighbours of the n x n block of component c at (x0, y0): availability, substitution, filtering (8.4.4.2.2 / .3)
+__device__ void gather_refs(Ctx2& e, int c, int x0, int y0, int log2n) {
+  Work& w = e.w;
+  const int n = 1 << log2n, sh = c ? 1 : 0, st = c ? e.a.Wc : e.a.W;
+  const uint8_t* pl = e.plane(c);
+  for (int i = e.lane; i <= 4 * n; i += GE_LANES) {
+    int px, py;
+    if (i < 2 * n) { px = x0 - 1; py = y0 + 2 * n - 1 - i; } else if (i == 2 * n) { px = x0 - 1; py = y0 - 1; } else { px = x0 + (i - 2 * n - 1); py = y0 - 1; }
+    w.ref[0][i] = e.avail(px << sh, py << sh) ? (int16_t)GE_LD(pl + (size_t)py * st + px) : (int16_t)-1;
+  }
+  GE_SYNC();
+  if (e.lane == 0) {
+    int16_t* r = w.ref[0];
+    int first = 0; while (first <= 4 * n && r[first] < 0) first++;
+    if (first > 4 * n) for (int i = 0; i <= 4 * n; i++) r[i] = 128;
+    else {
+      for (int i = 0; i < first; i++) r[i] = r[first];
+      for (int i = first + 1; i <= 4 * n; i++) if (r[i] < 0) r[i] = r[i - 1];
+    }
+    int16_t* f = w.ref[1];
+    if (c == 0 && n != 4) {
+      const int corner = r[2 * n], bl = r[0], tr = r[4 * n];
+      if (e.a.strong && n == 32 && abs(corner + tr - 2 * r[3 * n]) < 8 && abs(corner + bl - 2 * r[n]) < 8) {
+        f[2 * n] = (int16_t)corner; f[0] = (int16_t)bl; f[4 * n] = (int16_t)tr;
+        for (int y = 0; y < 63; y++) f[2 * n - 1 - y] = (int16_t)(((63 - y) * corner + (y + 1) * bl + 32) >> 6);
+        for (int x = 0; x < 63; x++) f[2 * n + 1 + x] = (int16_t)(((63 - x) * corner + (x + 1) * tr + 32) >> 6);
+      } else {
+        f[0] = r[0]; f[4 * n] = r[4 * n];
+        for (int i = 1; i < 4 * n; i++) f[i] = (int16_t)((r[i - 1] + 2 * r[i] + r[i + 1] + 2) >> 2);
+      }
+    }
+    int sum = n; for (int i = 0; i < n; i++) sum += r[2 * n - 1 - i] + r[2 * n + 1 + i];
+    w.dc = sum >> (log2n + 1);
+  }
+  GE_SYNC();
+}
+
+// predicted sample (x, y) of mode `mode` (8.4.4.2.4 .. .6) from the neighbours gathered above
+__device__ inline int pred_px(const Work& w, int c, int log2n, int mode, int x, int y) {
+  const int n = 1 << log2n;
+  bool filt = false;
+  if (c == 0 && mode != 1 && n != 4) {
+    const int dist = min(abs(mode - 26), abs(mode - 10)), thr = n == 8 ? 7 : (n == 16 ? 1 : 0);
+    filt = dist > thr;
+  }
+  const int16_t* ref = w.ref[filt ? 1 : 0];
+#define LEFT(i) ((int)ref[2 * n - 1 - (i)])
+#define TOP(i) ((int)ref[2 * n + 1 + (i)])
+  if (mode == 0) return ((n - 1 - x) * LEFT(y) + (x + 1) * TOP(n) + (n - 1 - y) * TOP(x) + (y + 1) * LEFT(n) + n) >> (log2n + 1);
+  if (mode == 1) {
+    const int dc = w.dc;
+    if (c == 0 && n < 32) {
+      if (x == 0 && y == 0) return (LEFT(0) + 2 * dc + TOP(0) + 2) >> 2;
+      if (y == 0) return (TOP(x) + 3 * dc + 2) >> 2;
+      if (x == 0) return (LEFT(y) + 3 * dc + 2) >> 2;
+    }
+    return dc;
+  }
+  const int ang = B200_T(kAngle)[mode], ia = B200_T(kInvAngle)[mode];
+  if (mode >= 18) {
+    if (mode == 26 && c == 0 && n < 32 && x == 0) return clip3(0, 255, TOP(0) + ((LEFT(y) - LEFT(-1)) >> 1));
+    const int idx = ((y + 1) * ang) >> 5, f = ((y + 1) * ang) & 31, k1 = x + idx + 1, k2 = k1 + 1;
+    const int r1 = k1 >= 0 ? TOP(k1 - 1) : LEFT(-1 + ((k1 * ia + 128) >> 8));
+    if (!f) return r1;
+    const int r2 = k2 >= 0 ? TOP(k2 - 1) : LEFT(-1 + ((k2 * ia + 128) >> 8));
+    return ((32 - f) * r1 + f * r2 + 16) >> 5;
+  }
+  if (mode == 10 && c == 0 && n < 32 && y == 0) return clip3(0, 255, LEFT(0) + ((TOP(x) - TOP(-1)) >> 1));
+  const int idx = ((x + 1) * ang) >> 5, f = ((x + 1) * ang) & 31, k1 = y + idx + 1, k2 = k1 + 1;
+  const int r1 = k1 >= 0 ? LEFT(k1 - 1) : TOP(-1 + ((k1 * ia + 128) >> 8));
+  if (!f) return r1;
+  const int r2 = k2 >= 0 ? LEFT(k2 - 1) : TOP(-1 + ((k2 * ia + 128) >> 8));
+  return ((32 - f) * r1 + f * r2 + 16) >> 5;
+#undef LEFT
+#undef TOP
+}
+
+__device__ inline int satd4(const int d[16]) {                   // 4x4 Hadamard
+  int m[16], s = 0;
+  for (int i = 0; i < 4; i++) {
+    const int a0 = d[i * 4] + d[i * 4 + 3], a1 = d[i * 4 + 1] + d[i * 4 + 2], a2 = d[i * 4 + 1] - d[i * 4 + 2], a3 = d[i * 4] - d[i * 4 + 3];
+    m[i * 4] = a0 + a1; m[i * 4 + 2] = a0 - a1; m[i * 4 + 1] = a3 + a2; m[i * 4 + 3] = a3 - a2;
+  }
+  for (int i = 0; i < 4; i++) {
+    const int a0 = m[i] + m[12 + i], a1 = m[4 + i] + m[8 + i], a2 = m[4 + i] - m[8 + i], a3 = m[i] - m[12 + i];
+    s += abs(a0 + a1) + abs(a0 - a1) + abs(a3 + a2) + abs(a3 - a2);
+  }
+  return (s + 1) >> 1;
+}
+
+// best luma mode of the n x n PU at (x0, y0) on SATD + lambda * mode bits; returns the mode, *cost = its J (x16)
+__device__ int search_mode(Ctx2& e, int x0, int y0, int log2n, long long* cost) {
+  Work& w = e.w;
+  const int n = 1 << log2n, nsb = (n * n) >> 4;
+  gather_refs(e, 0, x0, y0, log2n);
+  for (int i = e.lane; i < 35; i += GE_LANES) w.satd[i] = 0;
+  GE_SYNC();
+  for (int it = e.lane; it < 35 * nsb; it += GE_LANES) {
+    const int mode = it % 35, sb = it / 35, bx = (sb % (n >> 2)) << 2, by = (sb / (n >> 2)) << 2;
+    int d[16];
+    for (int k = 0; k < 16; k++) d[k] = e.org(0, x0 + bx + (k & 3), y0 + by + (k >> 2)) - pred_px(w, 0, log2n, mode, bx + (k & 3), by + (k >> 2));
+    GE_ATOMIC_ADD(&w.satd[mode], satd4(d));
+  }
+  GE_SYNC();
+  if (e.lane == 0) {
+    int cand[3]; mpm_cand(e.ipm(), e.a.W >> 2, e.a.log2ctb, x0, y0, cand);
+    long long best = -1; int bm = 0;
+    for (int m = 0; m < 35; m++) {
+      const long long j = ((long long)w.satd[m] << 4) + (long long)e.a.lambda16 * mode_bits(m, cand);
+      if (best < 0 || j < best) { best = j; bm = m; }
+    }
+    w.mode = bm; w.satd[35] = (int)best;                      // J x 16 of a 32x32 PU stays far below 2^31
+  }
+  GE_SYNC();
+  *cost = w.satd[35];
+  return w.mode;
+}
+
+// Predict, transform, quantise, reconstruct one TB of component c (component coordinates).  `final`: store the levels in the
+// coefficient plane.  Returns the SATD of the prediction residual (luma only, else 0).
+__device__ int code_tb(Ctx2& e, int c, int x0, int y0, int log2n, int mode, bool final) {
+  Work& w = e.w;
+  const int n = 1 << log2n, nn = n * n, st = c ? e.a.Wc : e.a.W, qp = e.a.qp[c];
+  const bool dst4 = c == 0 && log2n == 2;
+  gather_refs(e, c, x0, y0, log2n);
+  if (e.lane == 0) { w.any = 0; w.acc = 0; }
+  for (int i = e.lane; i < nn; i += GE_LANES) {
+    const int x = i & (n - 1), y = i >> log2n, pv = pred_px(w, c, log2n, mode, x, y);
+    w.pred[i] = (uint8_t)pv; w.res[i] = e.org(c, x0 + x, y0 + y) - pv;
+  }
+  GE_SYNC();
+  if (c == 0) {
+    for (int sb = e.lane; sb < (nn >> 4); sb += GE_LANES) {
+      const int bx = (sb % (n >> 2)) << 2, by = (sb / (n >> 2)) << 2;
+      int d[16]; for (int k = 0; k < 16; k++) d[k] = w.res[(by + (k >> 2)) * n + bx + (k & 3)];
+      GE_ATOMIC_ADD(&w.acc, satd4(d));
+    }
+  }
+  // forward transform: columns then rows (shifts log2n - 1 and log2n + 6 at 8 bit)
+  const int s1 = log2n - 1, s2 = log2n + 6;
+  for (int i = e.lane; i < nn; i += GE_LANES) {
+    const int k = i >> log2n, x = i & (n - 1);
+    int s = 0; for (int y = 0; y < n; y++) s += tmat(dst4, log2n, k, y) * w.res[y * n + x];
+    w.tmp[i] = (s + (1 << (s1 - 1))) >> s1;
+  }
+  GE_SYNC();
+  const int qbits = 14 + qp / 6 + (7 - log2n), qs = B200_T(kQuantScale)[qp % 6];
+  const long long add = 171LL << (qbits - 9);
+  for (int i = e.lane; i < nn; i += GE_LANES) {
+    const int y = i >> log2n, k = i & (n - 1);
+    int s = 0; for (int x = 0; x < n; x++) s += tmat(dst4, log2n, k, x) * w.tmp[y * n + x];
+    const int cf = (s + (1 << (s2 - 1))) >> s2;
+    int l = (int)(((long long)abs(cf) * qs + add) >> qbits);
+    l = min(l, 32767);
+    w.lev[i] = (int16_t)(cf < 0 ? -l : l);
+    if (l) w.any = 1;
+  }
+  GE_SYNC();
+  if (final) { int16_t* cp = e.cplane(c); for (int i = e.lane; i < nn; i += GE_LANES) cp[(size_t)(y0 + (i >> log2n)) * st + x0 + (i & (n - 1))] = w.lev[i]; }
+  uint8_t* rp = e.plane(c);
+  if (w.any) {
+    const int bs = log2n + 3, scale = B200_T(kLevelScale)[qp % 6] << (qp / 6);
+    for (int i = e.lane; i < nn; i += GE_LANES) {
+      const long long t = ((long long)w.lev[i] * 16 * scale + (1LL << (bs - 1))) >> bs;
+      w.coef[i] = (int)(t < -32768 ? -32768 : (t > 32767 ? 32767 : t));
+    }
+    GE_SYNC();
+    for (int i = e.lane; i < nn; i += GE_LANES) {       // tmp[y][x] = sum_k d[k][x] M[k][y]
+      const int y = i >> log2n, x = i & (n - 1);
+      int s = 0; for (int k = 0; k < n; k++) s += w.coef[k * n + x] * tmat(dst4, log2n, k, y);
+      w.tmp[i] = clip3(-32768, 32767, (s + 64) >> 7);
+    }
+    GE_SYNC();
+    for (int i = e.lane; i < nn; i += GE_LANES) {
+      const int y = i >> log2n, x = i & (n - 1);
+      int s = 0; for (int k = 0; k < n; k++) s += w.tmp[y * n + k] * tmat(dst4, log2n, k, x);
+      rp[(size_t)(y0 + y) * st + x0 + x] = (uint8_t)clip3(0, 255, w.pred[i] + ((s + (1 << 11)) >> 12));
+    }
+  } else {
+    for (int i = e.lane; i < nn; i += GE_LANES) rp[(size_t)(y0 + (i >> log2n)) * st + x0 + (i & (n - 1))] = w.pred[i];
+  }
+  if (c == 0) {
+    const int n4 = n >> 2; uint8_t* d = e.dec();
+    for (int i = e.lane; i < n4 * n4; i += GE_LANES) d[(size_t)((y0 >> 2) + i / n4) * (e.a.W >> 2) + (x0 >> 2) + i % n4] = 1;
+  }
+  GE_SYNC();
+  return w.acc;
+}
+
+__device__ void set_modes(Ctx2& e, int x0, int y0, int n, int mode) {
+  const int n4 = n >> 2; uint8_t* m = e.ipm();
+  for (int i = e.lane; i < n4 * n4; i += GE_LANES) m[(size_t)((y0 >> 2) + i / n4) * (e.a.W >> 2) + (x0 >> 2) + i % n4] = (uint8_t)mode;
+  GE_SYNC();
+}
+__device__ void set_cu(Ctx2& e, int x0, int y0, int n, int v) {
+  const int n8 = n >> 3; uint8_t* m = e.cu();
+  for (int i = e.lane; i < n8 * n8; i += GE_LANES) m[(size_t)((y0 >> 3) + i / n8) * (e.a.W >> 3) + (x0 >> 3) + i % n8] = (uint8_t)v;
+  GE_SYNC();
+}
+// save / restore / invalidate the luma reconstruction and modes of an n x n region (decision pass)
+__device__ void region(Ctx2& e, int x0, int y0, int n, uint8_t* buf, int op /* 0 save, 1 restore, 2 mark not reconstructed */) {
+  const int W = e.a.W, n4 = n >> 2; uint8_t* pl = e.plane(0); uint8_t* m = e.ipm(); uint8_t* d = e.dec();
+  for (int i = e.lane; i < n * n; i += GE_LANES) {
+    uint8_t* p = pl + (size_t)(y0 + i / n) * W + x0 + i % n;
+    if (op == 0) buf[i] = *p; else if (op == 1) *p = buf[i];
+  }
+  for (int i = e.lane; i < n4 * n4; i += GE_LANES) {
+    const size_t k = (size_t)((y0 >> 2) + i / n4) * (W >> 2) + (x0 >> 2) + i % n4;
+    if (op == 0) buf[n * n + i] = m[k]; else if (op == 1) m[k] = buf[n * n + i]; else d[k] = 0;
+  }
+  GE_SYNC();
+}
+
+// luma of one CU, closed loop; returns J x 16
+__device__ long long eval_cu(Ctx2& e, int x0, int y0, int log2cb, bool nxn) {
+  long long j = 0, jm;
+  if (nxn) {
+    for (int k = 0; k < 4; k++) {
+      const int px = x0 + (k & 1) * 4, py = y0 + (k >> 1) * 4;
+      const int m = search_mode(e, px, py, 2, &jm);
+      set_modes(e, px, py, 4, m);
+      code_tb(e, 0, px, py, 2, m, false);
+      j += jm;
+    }
+    return j + e.a.lambda16;                                  // part_mode bin
+  }
+  const int lg = log2cb < 5 ? log2cb : 5;
+  const int m = search_mode(e, x0, y0, lg, &jm);              // a 64x64 CU: chosen on its first 32x32 block
+  set_modes(e, x0, y0, 1 << log2cb, m);
+  if (log2cb < 6) { code_tb(e, 0, x0, y0, log2cb, m, false); return jm; }
+  j = jm - ((long long)e.w.satd[m] << 4);
+  for (int k = 0; k < 4; k++) j += (long long)code_tb(e, 0, x0 + (k & 1) * 32, y0 + (k >> 1) * 32, 5, m, false) << 4;
+  return j;
+}
+
+// decision pass: bottom-up quadtree, leaves the chosen luma reconstruction / modes / CU sizes; returns J x 16
+// (The quadtree walks are templates on the block size: no run-time recursion, so the stack size is known at compile time.)
+template <int L>
+__device__ long long decide(Ctx2& e, int x0, int y0, int depth) {
+  const int n = 1 << L, log2cb = L;
+  if (x0 + n > e.a.W || y0 + n > e.a.H) {                     // crosses the picture border: split implied
+    long long j = 0;
+    if constexpr (L > 3)
+      for (int k = 0; k < 4; k++) { const int x1 = x0 + (k & 1) * (n >> 1), y1 = y0 + (k >> 1) * (n >> 1); if (x1 < e.a.W && y1 < e.a.H) j += decide<L - 1>(e, x1, y1, depth + 1); }
+    return j;
+  }
+  const long long j0 = eval_cu(e, x0, y0, log2cb, false);
+  uint8_t* buf = e.w.save[depth];
+  region(e, x0, y0, n, buf, 0);
+  region(e, x0, y0, n, buf, 2);
+  long long j1;
+  if constexpr (L == 3) j1 = eval_cu(e, x0, y0, 3, true);
+  else {
+    j1 = e.a.lambda16;                                         // split_cu_flag
+    for (int k = 0; k < 4; k++) j1 += decide<L - 1>(e, x0 + (k & 1) * (n >> 1), y0 + (k >> 1) * (n >> 1), depth + 1);
+  }
+  if (j0 <= j1) { region(e, x0, y0, n, buf, 1); set_cu(e, x0, y0, n, log2cb); return j0; }
+  if (log2cb == 3) set_cu(e, x0, y0, 8, 3 | CU_NXN);
+  return j1;
+}
+
+// final pass: the chosen CUs again, luma and chroma in decoding order, levels into the coefficient plane
+template <int L>
+__device__ void finalize(Ctx2& e, int x0, int y0) {
+  if (x0 >= e.a.W || y0 >= e.a.H) return;
+  const int n = 1 << L, W = e.a.W, log2cb = L;
+  const int cell = GE_LD(e.cu() + (size_t)(y0 >> 3) * (W >> 3) + (x0 >> 3));
+  if constexpr (L > 3)
+    if ((cell & 7) < log2cb) { for (int k = 0; k < 4; k++) finalize<L - 1>(e, x0 + (k & 1) * (n >> 1), y0 + (k >> 1) * (n >> 1)); return; }
+  const int mode = GE_LD(e.ipm() + (size_t)(y0 >> 2) * (W >> 2) + (x0 >> 2));
+  const bool chroma = e.a.cfmt != 0;
+  if (cell & CU_NXN) {
+    for (int k = 0; k < 4; k++) {
+      const int px = x0 + (k & 1) * 4, py = y0 + (k >> 1) * 4;
+      code_tb(e, 0, px, py, 2, GE_LD(e.ipm() + (size_t)(py >> 2) * (W >> 2) + (px >> 2)), true);
+    }
+    if (chroma) { code_tb(e, 1, x0 >> 1, y0 >> 1, 2, mode, true); code_tb(e, 2, x0 >> 1, y0 >> 1, 2, mode, true); }
+    return;
+  }
+  const int lt = log2cb < 5 ? log2cb : 5, nt = 1 << lt;
+  for (int k = 0; k < (log2cb == 6 ? 4 : 1); k++) {
+    const int tx = x0 + (k & 1) * nt, ty = y0 + (k >> 1) * nt;
+    code_tb(e, 0, tx, ty, lt, mode, true);
+    if (chroma) { code_tb(e, 1, tx >> 1, ty >> 1, lt - 1, mode, true); code_tb(e, 2, tx >> 1, ty >> 1, lt - 1, mode, true); }
+  }
+}
+
+__device__ inline unsigned ld_relaxed(const unsigned* p) {
+  unsigned v; asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v;
+}
+// lane 0 polls with back-off (relaxed loads), then one fence orders the reads that follow (DESIGN 4 (i) / (iii))
+__device__ inline void wait_for(const unsigned* p, unsigned v, int lane) {
+  if (lane == 0) {
+    unsigned ns = 64;
+    while (ld_relaxed(p) < v) { __nanosleep(ns); if (ns < 4096) ns <<= 1; }
+    __threadfence();
+  }
+  __syncwarp();
+}
+__device__ inline void publish(unsigned* p, unsigned v, int lane) {
+  __syncwarp();
+  if (lane == 0) { __threadfence(); atomicExch(p, v); }
+}
+
+__device__ void e1_row(const Args& a, Work& w, int p, int ry, int lane) {
+  Ctx2 e{a, p, lane, w};
+  const size_t row = (size_t)p * a.hctb + ry;
+  for (int rx = 0; rx < a.wctb; rx++) {
+    if (ry > 0) wait_for(a.progress + row - 1, (unsigned)min(rx + 2, a.wctb), lane);
+    const int x0 = rx << a.log2ctb, y0 = ry << a.log2ctb;
+    if (a.log2ctb == 6) decide<6>(e, x0, y0, 0); else decide<5>(e, x0, y0, 0);
+    {                                                          // the final pass sees the CTB's blocks appear in decoding order again
+      const int w4 = min(1 << a.log2ctb, a.W - x0) >> 2, h4 = min(1 << a.log2ctb, a.H - y0) >> 2;
+      for (int i = lane; i < w4 * h4; i += GE_LANES) e.dec()[(size_t)((y0 >> 2) + i / w4) * (a.W >> 2) + (x0 >> 2) + i % w4] = 0;
+      GE_SYNC();
+    }
+    if (a.log2ctb == 6) finalize<6>(e, x0, y0); else finalize<5>(e, x0, y0);
+    publish(a.progress + row, (unsigned)(rx + 1), lane);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------- E2
+struct Cabac {                                                // 9.3.4.5 (arithmetic encoder with outstanding bits)
+  uint8_t* out; size_t cap, pos; unsigned cur; int nbits;
+  unsigned low, range; int outstanding; bool first, overflow;
+  uint8_t* ctx;                                               // CTX_COUNT entries: pStateIdx << 1 | valMps
+  __device__ void put1(unsigned b) {
+    cur = (cur << 1) | b;
+    if (++nbits == 8) { if (pos < cap) out[pos++] = (uint8_t)cur; else overflow = true; cur = 0; nbits = 0; }
+  }
+  __device__ void put_bit(unsigned b) {
+    if (first) first = false; else put1(b);
+    while (outstanding > 0) { put1(1 - b); outstanding--; }
+  }
+  __device__ void renorm() {
+    while (range < 256) {
+      if (low < 256) put_bit(0);
+      else if (low >= 512) { low -= 512; put_bit(1); }
+      else { low -= 256; outstanding++; }
+      range <<= 1; low <<= 1;
+    }
+  }
+  __device__ void bin(int ci, int b) {
+    const unsigned s = ctx[ci], state = s >> 1, mps = s & 1;
+    const unsigned lps = (syn::B200_T(kLps4)[state] >> (8 * ((range >> 6) & 3))) & 0xff;
+    range -= lps;
+    if ((unsigned)b != mps) {
+      low += range; range = lps;
+      ctx[ci] = (uint8_t)((syn::B200_T(kTransLps)[state] << 1) | (state == 0 ? 1 - mps : mps));
+    } else if (state < 62) ctx[ci] = (uint8_t)(((state + 1) << 1) | mps);
+    renorm();
+  }
+  __device__ void bypass(int b) {
+    low <<= 1;
+    if (b) low += range;
+    if (low >= 1024) { put_bit(1); low -= 1024; }
+    else if (low < 512) put_bit(0);
+    else { low -= 512; outstanding++; }
+  }
+  __device__ void bypass_bits(unsigned v, int n) { for (int i = n - 1; i >= 0; i--) bypass((v >> i) & 1); }
+  __device__ void terminate(int b) {
+    range -= 2;
+    if (b) {
+      low += range; range = 2; renorm(); put_bit((low >> 9) & 1);
+      put1((((low >> 7) & 3) | 1) >> 1); put1(1);
+      while (nbits) put1(0);
+    } else renorm();
+  }
+};
+
+__device__ inline void init_ctx(uint8_t* ctx, int qp) {
+  for (int i = 0; i < syn::CTX_COUNT; i++) {
+    const int iv = syn::B200_T(kInitI)[i], m = (iv >> 4) * 5 - 45, nn = ((iv & 15) << 3) - 16;
+    const int pre = clip3(1, 126, ((m * qp) >> 4) + nn), mps = pre > 63;
+    ctx[i] = (uint8_t)(((mps ? pre - 64 : 63 - pre) << 1) | mps);
+  }
+}
+
+struct Writer {
+  const Args& a; int p; Cabac& cb;
+  __device__ int cu_at(int x, int y) const { return a.cu8[(size_t)p * a.map8 + (size_t)(y >> 3) * (a.W >> 3) + (x >> 3)]; }
+  __device__ const int16_t* cplane(int c) const { return a.coef + (size_t)p * a.pic_samples + (c == 0 ? 0 : (size_t)a.W * a.H + (size_t)(c - 1) * a.Wc * a.Hc); }
+  __device__ bool nonzero(int c, int x0, int y0, int n) const {
+    const int st = c ? a.Wc : a.W; const int16_t* pl = cplane(c);
+    for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) if (pl[(size_t)(y0 + y) * st + x0 + x]) return true;
+    return false;
+  }
+
+  __device__ void residual(int c, int x0, int y0, int log2n, int scan) {     // 7.3.8.11
+    using namespace syn;
+    const int n = 1 << log2n, l2sb = log2n - 2, st = c ? a.Wc : a.W;
+    const int16_t* pl = cplane(c) + (size_t)y0 * st + x0;
+    const uint8_t *sbx = B200_T(kScanX)[l2sb][scan], *sby = B200_T(kScanY)[l2sb][scan], *px = B200_T(kScanX)[2][scan], *py = B200_T(kScanY)[2][scan];
+#define LEV(xx, yy) ((int)pl[(size_t)(yy) * st + (xx)])
+    int last_sb = -1, last_pos = -1;
+    for (int i = (1 << (2 * l2sb)) - 1; i >= 0 && last_sb < 0; i--) for (int k = 15; k >= 0; k--)
+      if (LEV((sbx[i] << 2) + px[k], (sby[i] << 2) + py[k])) { last_sb = i; last_pos = k; break; }
+    int lx = (sbx[last_sb] << 2) + px[last_pos], ly = (sby[last_sb] << 2) + py[last_pos];
+    if (scan == 2) { const int t = lx; lx = ly; ly = t; }
+    const uint8_t* group = B200_T(kLastGroup);
+    const uint8_t* min_in_group = B200_T(kLastGroupMin);
+    const int cmax = (log2n << 1) - 1;
+    int off, shift;
+    if (c == 0) { off = 3 * (log2n - 2) + ((log2n - 1) >> 2); shift = (log2n + 1) >> 2; } else { off = 15; shift = log2n - 2; }
+    const int gx = group[lx], gy = group[ly];
+    for (int k = 0; k < gx; k++) cb.bin(CTX_LAST_X + off + (k >> shift), 1);
+    if (gx < cmax) cb.bin(CTX_LAST_X + off + (gx >> shift), 0);
+    for (int k = 0; k < gy; k++) cb.bin(CTX_LAST_Y + off + (k >> shift), 1);
+    if (gy < cmax) cb.bin(CTX_LAST_Y + off + (gy >> shift), 0);
+    if (gx > 3) cb.bypass_bits(lx - min_in_group[gx], (gx >> 1) - 1);
+    if (gy > 3) cb.bypass_bits(ly - min_in_group[gy], (gy >> 1) - 1);
+    uint64_t csbf = 0;                                        // coded_sub_block_flag, bit ys * 8 + xs
+#define CSBF(xx, yy) ((int)((csbf >> ((yy) * 8 + (xx))) & 1))
+    int carry = 1; bool first_done = false;
+    for (int i = last_sb; i >= 0; i--) {
+      const int xs = sbx[i], ys = sby[i];
+      int v[16]; bool coded = false;
+      for (int k = 0; k < 16; k++) { v[k] = LEV((xs << 2) + px[k], (ys << 2) + py[k]); coded |= v[k] != 0; }
+      bool infer_dc = false;
+      if (i < last_sb && i > 0) {
+        int cs = 0;
+        if (xs + 1 < (1 << l2sb)) cs |= CSBF(xs + 1, ys);
+        if (ys + 1 < (1 << l2sb)) cs |= CSBF(xs, ys + 1);
+        cb.bin(CTX_CSBF + (cs ? 1 : 0) + (c ? 2 : 0), coded);
+        infer_dc = true;
+      } else coded = true;
+      if (coded) csbf |= 1ull << (ys * 8 + xs);
+      if (!coded) continue;
+      int prev = 0;
+      if (xs + 1 < (1 << l2sb)) prev |= CSBF(xs + 1, ys);
+      if (ys + 1 < (1 << l2sb)) prev |= CSBF(xs, ys + 1) << 1;
+      const int start = i == last_sb ? last_pos - 1 : 15;
+      for (int k = start; k >= 0; k--) {
+        const int xc = (xs << 2) + px[k], yc = (ys << 2) + py[k];
+        if (k > 0 || !infer_dc) {
+          int sc;
+          if (log2n == 2) sc = B200_T(kSigMap4)[(yc << 2) + xc];
+          else if (xc + yc == 0) sc = 0;
+          else {
+            const int xp = xc & 3, yp = yc & 3;
+            if (prev == 0) sc = (xp + yp == 0) ? 2 : (xp + yp < 3) ? 1 : 0;
+            else if (prev == 1) sc = yp == 0 ? 2 : (yp == 1 ? 1 : 0);
+            else if (prev == 2) sc = xp == 0 ? 2 : (xp == 1 ? 1 : 0);
+            else sc = 2;
+            if (c == 0) { if (xs || ys) sc += 3; sc += log2n == 3 ? (scan == 0 ? 9 : 15) : 21; }
+            else sc += log2n == 3 ? 9 : 12;
+          }
+          cb.bin(CTX_SIG + (c == 0 ? sc : 27 + sc), v[k] != 0);
+          if (v[k]) infer_dc = false;
+        }
+      }
+      int ng1 = 0, last_g1 = -1, g1ctx = 1;
+      int ctx_set = (i == 0 || c > 0) ? 0 : 2;
+      if (first_done && carry == 0) ctx_set++;
+      first_done = true;
+      bool any = false;
+      for (int k = 15; k >= 0; k--) if (v[k]) {
+        any = true;
+        if (ng1 < 8) {
+          const int g = abs(v[k]) > 1;
+          cb.bin(CTX_GT1 + ctx_set * 4 + min(3, g1ctx) + (c ? 16 : 0), g);
+          ng1++;
+          if (g) { g1ctx = 0; if (last_g1 < 0) last_g1 = k; } else if (g1ctx > 0) g1ctx++;
+        }
+      }
+      if (any) carry = g1ctx;
+      if (last_g1 >= 0) cb.bin(CTX_GT2 + ctx_set + (c ? 4 : 0), abs(v[last_g1]) > 2);
+      for (int k = 15; k >= 0; k--) if (v[k]) cb.bypass(v[k] < 0);
+      int nsig = 0, rice = 0, cnt1 = 0;
+      for (int k = 15; k >= 0; k--) if (v[k]) {
+        const int av = abs(v[k]);
+        const int g1 = cnt1 < 8 ? (av > 1) : 0; if (cnt1 < 8) cnt1++;
+        const int g2 = (k == last_g1) ? (av > 2) : 0;
+        const int base = 1 + g1 + g2;
+        if (base == ((nsig < 8) ? ((k == last_g1) ? 3 : 2) : 1)) {
+          const int rem = av - base;
+          if ((rem >> rice) <= 3) { const int pre = rem >> rice; for (int t = 0; t < pre; t++) cb.bypass(1); cb.bypass(0); cb.bypass_bits(rem & ((1 << rice) - 1), rice); }
+          else {
+            const int q = (rem >> rice) - 2; int kk = 0; while ((q >> (kk + 1)) > 0) kk++;
+            for (int t = 0; t < kk + 3; t++) cb.bypass(1);
+            cb.bypass(0);
+            cb.bypass_bits(rem - (((1 << kk) + 2) << rice), kk + rice);
+          }
+          if (av > 3 * (1 << rice)) rice = min(rice + 1, 4);
+        }
+        nsig++;
+      }
+    }
+#undef LEV
+#undef CSBF
+  }
+
+  __device__ static int scan_of(int mode) { return (mode >= 6 && mode <= 14) ? 2 : (mode >= 22 && mode <= 30) ? 1 : 0; }
+
+  // transform tree (7.3.8.8 / 7.3.8.10): TU = CU apart from the implied splits
+  template <int L>
+  __device__ void tree(int x0, int y0, int depth, int blk, bool nxn, int max_depth, const int lmode[4], int cmode, bool pcb, bool pcr, int cux, int cuy) {
+    using namespace syn;
+    const int log2n = L;
+    const bool chroma = a.cfmt != 0;
+    const bool can_split = log2n <= 5 && log2n > 2 && depth < max_depth && !(nxn && depth == 0);
+    const bool split = !can_split && (log2n > 5 || (nxn && depth == 0));
+    if (can_split) cb.bin(CTX_SPLIT_TR + 5 - log2n, 0);
+    bool ccb = false, ccr = false;
+    if (chroma) {
+      if (log2n > 2) {
+        const int nc = 1 << (log2n - 1);
+        if (depth == 0 || pcb) { ccb = nonzero(1, x0 >> 1, y0 >> 1, nc); cb.bin(CTX_CBF_CHROMA + depth, ccb); }
+        if (depth == 0 || pcr) { ccr = nonzero(2, x0 >> 1, y0 >> 1, nc); cb.bin(CTX_CBF_CHROMA + depth, ccr); }
+      } else { ccb = pcb; ccr = pcr; }
+    }
+    if constexpr (L > 2)
+      if (split) {
+        const int h = 1 << (log2n - 1);
+        for (int k = 0; k < 4; k++) tree<L - 1>(x0 + (k & 1) * h, y0 + (k >> 1) * h, depth + 1, k, nxn, max_depth, lmode, cmode, ccb, ccr, cux, cuy);
+        return;
+      }
+    const int pu = nxn ? ((y0 > cuy) ? 2 : 0) + ((x0 > cux) ? 1 : 0) : 0;
+    const bool cbf_l = nonzero(0, x0, y0, 1 << log2n);
+    cb.bin(CTX_CBF_LUMA + (depth == 0 ? 1 : 0), cbf_l);
+    if (cbf_l) residual(0, x0, y0, log2n, log2n <= 3 ? scan_of(lmode[pu]) : 0);
+    if (chroma) {
+      if (log2n > 2) {
+        if (ccb) residual(1, x0 >> 1, y0 >> 1, log2n - 1, log2n - 1 == 2 ? scan_of(cmode) : 0);
+        if (ccr) residual(2, x0 >> 1, y0 >> 1, log2n - 1, log2n - 1 == 2 ? scan_of(cmode) : 0);
+      } else if (blk == 3) {
+        if (pcb) residual(1, cux >> 1, cuy >> 1, 2, scan_of(cmode));
+        if (pcr) residual(2, cux >> 1, cuy >> 1, 2, scan_of(cmode));
+      }
+    }
+  }
+
+  template <int L>
+  __device__ void quadtree(int x0, int y0, int depth) {
+    using namespace syn;
+    const int n = 1 << L, W = a.W, H = a.H, log2cb = L;
+    const int cell = cu_at(x0, y0);
+    bool split;
+    if (x0 + n <= W && y0 + n <= H && log2cb > 3) {
+      split = (cell & 7) < log2cb;
+      int inc = 0;
+      if (x0 > 0 && a.log2ctb - (cu_at(x0 - 1, y0) & 7) > depth) inc++;
+      if (y0 > 0 && a.log2ctb - (cu_at(x0, y0 - 1) & 7) > depth) inc++;
+      cb.bin(CTX_SPLIT_CU + inc, split);
+    } else split = log2cb > 3;
+    if constexpr (L > 3)
+      if (split) {
+        const int h = n >> 1;
+        for (int k = 0; k < 4; k++) { const int x1 = x0 + (k & 1) * h, y1 = y0 + (k >> 1) * h; if (x1 < W && y1 < H) quadtree<L - 1>(x1, y1, depth + 1); }
+        return;
+      }
+    // coding_unit (7.3.8.5)
+    const bool nxn = log2cb == 3 && (cell & CU_NXN);
+    if (log2cb == 3) cb.bin(CTX_PART_MODE, !nxn);
+    const int np = nxn ? 4 : 1, pb = nxn ? n / 2 : n;
+    const uint8_t* ipm = a.ipm4 + (size_t)p * a.map4;
+    int lmode[4] = {0, 0, 0, 0}, prev[4], idx[4], rem[4];
+    for (int i = 0; i < np; i++) {
+      const int px = x0 + (i & 1) * pb, py = y0 + (i >> 1) * pb;
+      int cand[3]; mpm_cand(ipm, W >> 2, a.log2ctb, px, py, cand);
+      const int mode = ipm[(size_t)(py >> 2) * (W >> 2) + (px >> 2)];
+      lmode[i] = mode; prev[i] = 0; idx[i] = 0; rem[i] = 0;
+      for (int k = 0; k < 3; k++) if (cand[k] == mode) { prev[i] = 1; idx[i] = k; }
+      if (!prev[i]) {
+        int s0 = cand[0], s1 = cand[1], s2 = cand[2], t;
+        if (s0 > s1) { t = s0; s0 = s1; s1 = t; }
+        if (s1 > s2) { t = s1; s1 = s2; s2 = t; }
+        if (s0 > s1) { t = s0; s0 = s1; s1 = t; }
+        int r = mode; if (r > s2) r--; if (r > s1) r--; if (r > s0) r--;
+        rem[i] = r;
+      }
+    }
+    for (int i = 0; i < np; i++) cb.bin(CTX_PREV_INTRA, prev[i]);
+    for (int i = 0; i < np; i++) {
+      if (prev[i]) { cb.bypass(idx[i] > 0); if (idx[i] > 0) cb.bypass(idx[i] > 1); }
+      else cb.bypass_bits(rem[i], 5);
+    }
+    if (a.cfmt) cb.bin(CTX_CHROMA_PRED, 0);                    // intra_chroma_pred_mode = 4 (DM)
+    tree<L>(x0, y0, 0, 0, nxn, a.max_th_depth + (nxn ? 1 : 0), lmode, lmode[0], false, false, x0, y0);
+  }
+};
+
+__device__ void e2_row(const Args& a, uint8_t* ctx, int p, int ry, int lane) {
+  const size_t row = (size_t)p * a.hctb + ry;
+  if (lane == 0) {
+    Cabac cb{a.ss + row * a.ss_cap, a.ss_cap, 0, 0, 0, 0, 510, 0, true, false, ctx};
+    Writer wr{a, p, cb};
+    if (ry > 0 && a.wctb >= 2) {
+      const uint8_t* src = a.wpp_ctx + (row - 1) * syn::CTX_COUNT;
+      for (int i = 0; i < syn::CTX_COUNT; i++) ctx[i] = GE_LD(src + i);
+    } else init_ctx(ctx, a.slice_qp);
+    for (int rx = 0; rx < a.wctb; rx++) {
+      if (a.log2ctb == 6) wr.quadtree<6>(rx << a.log2ctb, ry << a.log2ctb, 0); else wr.quadtree<5>(rx << a.log2ctb, ry << a.log2ctb, 0);
+      if (rx == 1) {
+        uint8_t* dst = a.wpp_ctx + row * syn::CTX_COUNT;
+        for (int i = 0; i < syn::CTX_COUNT; i++) dst[i] = ctx[i];
+        __threadfence(); atomicExch(a.progress2 + row, 1u);
+      }
+      const bool last = ry == a.hctb - 1 && rx == a.wctb - 1;
+      cb.terminate(last ? 1 : 0);                              // end_of_slice_segment_flag
+      if (!last && rx == a.wctb - 1) cb.terminate(1);          // end_of_subset_one_bit + byte_alignment()
+    }
+    a.ss_len[row] = (unsigned)cb.pos;
+    if (cb.overflow) atomicOr(a.error, 1u);
+  }
+}
+
+__global__ void __launch_bounds__(32) e1_kernel(Args a) {
+  __shared__ Work w;
+  __shared__ unsigned t;
+  if (threadIdx.x == 0) t = atomicAdd(a.ticket, 1u);
+  __syncwarp();
+  const unsigned row = t;
+  __syncwarp();
+  e1_row(a, w, (int)(row / a.hctb), (int)(row % a.hctb), threadIdx.x);
+}
+
+__global__ void __launch_bounds__(32) e2_kernel(Args a) {
+  __shared__ uint8_t ctx[syn::CTX_COUNT];
+  __shared__ unsigned t;
+  if (threadIdx.x == 0) t = atomicAdd(a.ticket + 1, 1u);
+  __syncwarp();
+  const unsigned row = t;
+  const int p = (int)(row / a.hctb), ry = (int)(row % a.hctb);
+  if (ry > 0 && a.wctb >= 2) wait_for(a.progress2 + row - 1, 1u, threadIdx.x);
+  e2_row(a, ctx, p, ry, threadIdx.x);
+}
+
+// gathers the sub-streams of all rows into one packed buffer (offsets from the host's prefix sum)
+__global__ void pack_kernel(const uint8_t* ss, size_t cap, const unsigned* len, const unsigned long long* off, uint8_t* out) {
+  const size_t row = blockIdx.x;
+  const uint8_t* s = ss + row * cap; uint8_t* d = out + off[row];
+  for (unsigned i = threadIdx.x; i < len[row]; i += blockDim.x) d[i] = s[i];
+}
+
+}  // namespace genc
+}  // namespace b200
+
+// ---------------------------------------------------------------------------------------------------- host side
+struct b200_gpu_encoder {
+  b200::Pool pool{std::max(1, std::min(16, (int)std::thread::hardware_concurrency()))};
+  b200::Bounce bounce;
+  b200::Stream stream;
+  b200::Event ev[3];
+  b200::DevBuf<uint8_t> src, rec, ipm4, dec4, cu8, wpp_ctx, ss, packed;
+  b200::DevBuf<int16_t> coef;
+  b200::DevBuf<unsigned> sync, ss_len;
+  b200::DevBuf<unsigned long long> off;
+  b200::DevBuf<b200::genc::Pic> pics;
+  std::vector<std::vector<uint8_t>> out;
+  b200_hevc_enc_params params{};
+  int n = 0, W = 0, H = 0, cfmt = 1;
+  b200_gpu_encode_stats stats{};
+  bool ready = false;
+};
+
+namespace b200 {
+namespace genc {
+
+int validate(const b200_hevc_enc_params* p, int n, const b200_planes* pics) {
+  if (!p || !pics) return set_error(B200_E_INVALID, "null argument");
+  if (n <= 0) return set_error(B200_E_INVALID, "picture count %d", n);
+  if (p->width < 8 || p->height < 8 || p->width > 16384 || p->height > 16384) return set_error(B200_E_INVALID, "size %dx%d", p->width, p->height);
+  if (p->bit_depth != 8) return set_error(B200_E_UNSUPPORTED, "bit_depth %d: the GPU encoder codes 8-bit pictures", p->bit_depth);
+  if (p->chroma_format_idc != 0 && p->chroma_format_idc != 1) return set_error(B200_E_UNSUPPORTED, "chroma_format_idc %d: 4:2:0 and 4:0:0 only", p->chroma_format_idc);
+  if (p->log2_ctb_size != 5 && p->log2_ctb_size != 6) return set_error(B200_E_UNSUPPORTED, "log2_ctb_size %d: 5 or 6", p->log2_ctb_size);
+  if (p->qp < 0 || p->qp > 51 || p->init_qp < 0 || p->init_qp > 51) return set_error(B200_E_INVALID, "qp %d / init_qp %d", p->qp, p->init_qp);
+  if (p->max_transform_hierarchy_depth_intra < 0 || p->max_transform_hierarchy_depth_intra > 4) return set_error(B200_E_INVALID, "max_transform_hierarchy_depth_intra %d", p->max_transform_hierarchy_depth_intra);
+  if (abs(p->cb_qp_offset) > 12 || abs(p->cr_qp_offset) > 12 || abs(p->slice_cb_qp_offset) > 12 || abs(p->slice_cr_qp_offset) > 12 ||
+      abs(p->cb_qp_offset + p->slice_cb_qp_offset) > 12 || abs(p->cr_qp_offset + p->slice_cr_qp_offset) > 12)
+    return set_error(B200_E_INVALID, "chroma QP offsets");
+  if (abs(p->beta_offset_div2) > 6 || abs(p->tc_offset_div2) > 6 || abs(p->slice_beta_offset_div2) > 6 || abs(p->slice_tc_offset_div2) > 6)
+    return set_error(B200_E_INVALID, "deblocking offsets");
+  static const struct { const char* name; int off; } refused[] = {
+    {"sao", offsetof(b200_hevc_enc_params, sao)}, {"sign_data_hiding", offsetof(b200_hevc_enc_params, sign_data_hiding)},
+    {"transform_skip", offsetof(b200_hevc_enc_params, transform_skip)}, {"cu_qp_delta", offsetof(b200_hevc_enc_params, cu_qp_delta)},
+    {"scaling_lists", offsetof(b200_hevc_enc_params, scaling_lists)}, {"pcm", offsetof(b200_hevc_enc_params, pcm)},
+    {"transquant_bypass", offsetof(b200_hevc_enc_params, transquant_bypass)}, {"slice_ctb_rows", offsetof(b200_hevc_enc_params, slice_ctb_rows)},
+    {"dependent_slice_segments", offsetof(b200_hevc_enc_params, dependent_slice_segments)}};
+  for (const auto& r : refused)
+    if (*(const int*)((const char*)p + r.off)) return set_error(B200_E_UNSUPPORTED, "%s: not supported by the GPU encoder", r.name);
+  if (p->tile_cols > 1 || p->tile_rows > 1) return set_error(B200_E_UNSUPPORTED, "tile_cols / tile_rows: tiles are not supported by the GPU encoder");
+  if (!p->wpp) return set_error(B200_E_UNSUPPORTED, "wpp = 0: the GPU encoder codes one WPP sub-stream per CTB row");
+  const int want_chroma = p->chroma_format_idc ? B200_CHROMA_420 : B200_CHROMA_MONO;
+  for (int i = 0; i < n; i++) {
+    const b200_planes& q = pics[i];
+    if (!q.y || (p->chroma_format_idc && (!q.cb || !q.cr))) return set_error(B200_E_INVALID, "picture %d: missing plane", i);
+    if (q.width != p->width || q.height != p->height) return set_error(B200_E_INVALID, "picture %d: %dx%d, the call codes %dx%d", i, q.width, q.height, p->width, p->height);
+    if (q.chroma != want_chroma) return set_error(B200_E_INVALID, "picture %d: chroma %d, the call codes chroma_format_idc %d", i, q.chroma, p->chroma_format_idc);
+    if (q.bit_depth != 8) return set_error(B200_E_UNSUPPORTED, "picture %d: bit depth %d", i, q.bit_depth);
+    if (q.y_stride < (size_t)q.width || (p->chroma_format_idc && q.c_stride < (size_t)((q.width + 1) >> 1))) return set_error(B200_E_INVALID, "picture %d: stride", i);
+  }
+  return B200_OK;
+}
+
+// SATD-domain Lagrangian: lambda = sqrt(0.57 * 2^((QP - 12) / 3)), in 1/16 units
+inline int lambda16(int qp) { return (int)(16.0 * std::sqrt(0.57 * std::pow(2.0, (qp - 12) / 3.0)) + 0.5); }
+
+inline int chroma_qp(int qpy, int off) {                      // 8.6.1, ChromaArrayType 1, 8 bit
+  static const uint8_t tab[14] = {29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37};
+  const int qpi = clip3(0, 57, qpy + off);
+  return qpi < 30 ? qpi : (qpi >= 43 ? qpi - 6 : tab[qpi - 30]);
+}
+
+int encode(b200_gpu_encoder* e, const b200_hevc_enc_params* p, int n, const Pic* host_pics, cudaStream_t s) {
+  using clk = std::chrono::steady_clock;
+  const auto t0 = clk::now();
+  e->ready = false;
+  const int W = (p->width + 7) & ~7, H = (p->height + 7) & ~7, cfmt = p->chroma_format_idc, log2ctb = p->log2_ctb_size;
+  const int Wc = cfmt ? W / 2 : 0, Hc = cfmt ? H / 2 : 0, ctb = 1 << log2ctb;
+  const int wctb = (W + ctb - 1) >> log2ctb, hctb = (H + ctb - 1) >> log2ctb;
+  const size_t rows = (size_t)n * hctb, pic_samples = (size_t)W * H + 2 * (size_t)Wc * Hc;
+  const size_t map4 = (size_t)(W / 4) * (H / 4), map8 = (size_t)(W / 8) * (H / 8);
+  const size_t cap = substream_capacity(p->width, log2ctb, cfmt);
+  int rc;
+  if ((rc = e->rec.reserve(n * pic_samples, false)) || (rc = e->coef.reserve(n * pic_samples, false)) || (rc = e->ipm4.reserve(n * map4, false)) ||
+      (rc = e->dec4.reserve(n * map4, false)) || (rc = e->cu8.reserve(n * map8, false)) || (rc = e->wpp_ctx.reserve(rows * syn::CTX_COUNT, false)) ||
+      (rc = e->ss.reserve(rows * cap, false)) || (rc = e->sync.reserve(2 * rows + 3, false)) || (rc = e->ss_len.reserve(rows)) ||
+      (rc = e->off.reserve(rows)) || (rc = e->pics.reserve(n)))
+    return rc;
+  for (int i = 0; i < n; i++) e->pics.h[i] = host_pics[i];
+  B200_CUDA_CHECK(cudaMemcpyAsync(e->pics.d, e->pics.h, n * sizeof(Pic), cudaMemcpyHostToDevice, s));
+  B200_CUDA_CHECK(cudaMemsetAsync(e->dec4.d, 0, n * map4, s));
+  B200_CUDA_CHECK(cudaMemsetAsync(e->sync.d, 0, (2 * rows + 3) * sizeof(unsigned), s));
+  Args a{};
+  a.pics = e->pics.d; a.n = n; a.W = W; a.H = H; a.Wc = Wc; a.Hc = Hc; a.sw = p->width; a.sh = p->height;
+  a.cfmt = cfmt; a.log2ctb = log2ctb; a.wctb = wctb; a.hctb = hctb; a.max_th_depth = p->max_transform_hierarchy_depth_intra;
+  a.strong = p->strong_intra_smoothing != 0; a.slice_qp = p->qp;
+  a.qp[0] = p->qp; a.qp[1] = chroma_qp(p->qp, p->cb_qp_offset + p->slice_cb_qp_offset * (p->slice_chroma_qp_offsets != 0));
+  a.qp[2] = chroma_qp(p->qp, p->cr_qp_offset + p->slice_cr_qp_offset * (p->slice_chroma_qp_offsets != 0));
+  a.lambda16 = lambda16(p->qp);
+  a.rec = e->rec.d; a.coef = e->coef.d; a.pic_samples = pic_samples; a.ipm4 = e->ipm4.d; a.dec4 = e->dec4.d; a.map4 = map4;
+  a.cu8 = e->cu8.d; a.map8 = map8;
+  a.progress = e->sync.d; a.progress2 = e->sync.d + rows; a.ticket = e->sync.d + 2 * rows; a.error = e->sync.d + 2 * rows + 2;
+  a.wpp_ctx = e->wpp_ctx.d; a.ss = e->ss.d; a.ss_cap = cap; a.ss_len = e->ss_len.d;
+  B200_CUDA_CHECK(cudaEventRecord(e->ev[0], s));
+  e1_kernel<<<(unsigned)rows, 32, 0, s>>>(a);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(e->ev[1], s));
+  e2_kernel<<<(unsigned)rows, 32, 0, s>>>(a);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaEventRecord(e->ev[2], s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(e->ss_len.h, e->ss_len.d, rows * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  unsigned err = 0;
+  B200_CUDA_CHECK(cudaMemcpyAsync(&err, a.error, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  const auto t1 = clk::now();
+  if (err) return set_error(B200_E_LIMIT, "a sub-stream exceeded its worst-case buffer of %zu bytes", cap);
+  size_t total = 0;
+  for (size_t r = 0; r < rows; r++) { e->off.h[r] = total; total += e->ss_len.h[r]; }
+  if ((rc = e->packed.reserve(total + 1))) return rc;
+  B200_CUDA_CHECK(cudaMemcpyAsync(e->off.d, e->off.h, rows * sizeof(unsigned long long), cudaMemcpyHostToDevice, s));
+  pack_kernel<<<(unsigned)rows, 256, 0, s>>>(e->ss.d, cap, e->ss_len.d, e->off.d, e->packed.d);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpyAsync(e->packed.h, e->packed.d, total, cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaStreamSynchronize(s));
+  // framing: one access unit per picture
+  const std::vector<int> none;
+  const enc::SeqHeader sh{p, W, H, cfmt, cfmt ? 1 : 0, 1, 1, 8, log2ctb, 2, std::min(5, log2ctb), p->max_transform_hierarchy_depth_intra, log2ctb, 8, 8,
+                          false, nullptr, nullptr, false, &none, &none};
+  std::vector<uint8_t> ps;
+  enc::write_vps(ps, sh); enc::write_sps(ps, sh); enc::write_pps(ps, sh);
+  e->out.resize(n);
+  e->pool.parallel_for(n, [&](int i) {
+    std::vector<size_t> esc(hctb);
+    const uint8_t* base = e->packed.h + e->off.h[(size_t)i * hctb];
+    size_t bytes = 0;
+    for (int r = 0; r < hctb; r++) {
+      const size_t row = (size_t)i * hctb + r;
+      esc[r] = enc::escaped_size(e->packed.h + e->off.h[row], e->ss_len.h[row]);
+      bytes += e->ss_len.h[row];
+    }
+    enc::BitWriter b;
+    enc::write_slice_header(b, sh, 0, false, p->qp, esc);
+    b.buf.insert(b.buf.end(), base, base + bytes);
+    std::vector<uint8_t>& o = e->out[i];
+    o.assign(ps.begin(), ps.end());
+    enc::append_nal(o, 19 /* IDR_W_RADL */, b.buf);
+  });
+  const auto t2 = clk::now();
+  float ms1 = 0, ms2 = 0;
+  cudaEventElapsedTime(&ms1, e->ev[0], e->ev[1]);
+  cudaEventElapsedTime(&ms2, e->ev[1], e->ev[2]);
+  b200_gpu_encode_stats& st = e->stats;
+  st.analyse_ms = ms1; st.entropy_ms = ms2;
+  st.framing_ms = std::chrono::duration<double, std::milli>(t2 - t1).count();
+  st.total_ms = std::chrono::duration<double, std::milli>(t2 - t0).count();
+  st.bytes = 0; for (auto& o : e->out) st.bytes += o.size();
+  st.ctus = (uint64_t)rows * wctb; st.pictures = (uint64_t)n;
+  e->params = *p; e->n = n; e->W = W; e->H = H; e->cfmt = cfmt; e->ready = true;
+  return B200_OK;
+}
+
+}  // namespace genc
+}  // namespace b200
+
+extern "C" {
+
+int b200_gpu_encoder_create(b200_gpu_encoder** enc) {
+  using namespace b200;
+  if (!enc) return set_error(B200_E_INVALID, "null argument");
+  std::unique_ptr<b200_gpu_encoder> e(new b200_gpu_encoder());
+  B200_CUDA_CHECK(cudaStreamCreateWithFlags(&e->stream.h, cudaStreamNonBlocking));
+  for (auto& ev : e->ev) B200_CUDA_CHECK(cudaEventCreate(&ev.h));
+  *enc = e.release();
+  return B200_OK;
+}
+
+void b200_gpu_encoder_destroy(b200_gpu_encoder* enc) { delete enc; }
+
+int b200_gpu_encode_check(const b200_hevc_enc_params* p, int n, const b200_planes* pics) { return b200::genc::validate(p, n, pics); }
+
+size_t b200_gpu_encoder_substream_capacity(int width, int log2_ctb_size, int chroma_format_idc) {
+  return b200::genc::substream_capacity(width, log2_ctb_size, chroma_format_idc);
+}
+
+int b200_gpu_encode_intra_device(b200_gpu_encoder* enc, const b200_hevc_enc_params* p, int n, const b200_planes* pics, void* stream) {
+  using namespace b200;
+  if (!enc) return set_error(B200_E_INVALID, "null encoder");
+  if (int rc = genc::validate(p, n, pics)) return rc;
+  std::vector<genc::Pic> hp(n);
+  for (int i = 0; i < n; i++) {
+    hp[i].src[0] = (const uint8_t*)pics[i].y; hp[i].src[1] = (const uint8_t*)pics[i].cb; hp[i].src[2] = (const uint8_t*)pics[i].cr;
+    hp[i].stride[0] = pics[i].y_stride; hp[i].stride[1] = hp[i].stride[2] = pics[i].c_stride;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  return genc::encode(enc, p, n, hp.data(), s);
+}
+
+int b200_gpu_encode_intra_host(b200_gpu_encoder* enc, const b200_hevc_enc_params* p, int n, const b200_planes* pics) {
+  using namespace b200;
+  if (!enc) return set_error(B200_E_INVALID, "null encoder");
+  if (int rc = genc::validate(p, n, pics)) return rc;
+  const int w = p->width, h = p->height, cw = (w + 1) >> 1, ch = (h + 1) >> 1, cfmt = p->chroma_format_idc;
+  const size_t per = (size_t)w * h + (cfmt ? 2 * (size_t)cw * ch : 0);
+  if (int rc = enc->src.reserve(n * per, false)) return rc;
+  std::vector<genc::Pic> hp(n);
+  for (int i = 0; i < n; i++) {
+    uint8_t* d = enc->src.d + i * per;
+    hp[i].src[0] = d; hp[i].stride[0] = w;
+    if (int rc = enc->bounce.upload(d, w, pics[i].y, pics[i].y_stride, w, h, enc->stream, enc->pool)) return rc;
+    if (cfmt) {
+      hp[i].src[1] = d + (size_t)w * h; hp[i].src[2] = d + (size_t)w * h + (size_t)cw * ch; hp[i].stride[1] = hp[i].stride[2] = cw;
+      if (int rc = enc->bounce.upload((void*)hp[i].src[1], cw, pics[i].cb, pics[i].c_stride, cw, ch, enc->stream, enc->pool)) return rc;
+      if (int rc = enc->bounce.upload((void*)hp[i].src[2], cw, pics[i].cr, pics[i].c_stride, cw, ch, enc->stream, enc->pool)) return rc;
+    }
+  }
+  return genc::encode(enc, p, n, hp.data(), enc->stream);
+}
+
+int b200_gpu_encoder_output(b200_gpu_encoder* enc, int i, const uint8_t** data, size_t* size) {
+  using namespace b200;
+  if (!enc || !data || !size) return set_error(B200_E_INVALID, "null argument");
+  if (!enc->ready || i < 0 || i >= enc->n) return set_error(B200_E_INVALID, "no picture %d in the last call", i);
+  *data = enc->out[i].data(); *size = enc->out[i].size();
+  return B200_OK;
+}
+
+int b200_gpu_encoder_read_recon(b200_gpu_encoder* enc, int i, void* y, void* cb, void* cr, size_t y_stride, size_t c_stride) {
+  using namespace b200;
+  if (!enc || !y) return set_error(B200_E_INVALID, "null argument");
+  if (!enc->ready || i < 0 || i >= enc->n) return set_error(B200_E_INVALID, "no picture %d in the last call", i);
+  const int w = enc->params.width, h = enc->params.height, W = enc->W, H = enc->H;
+  const size_t ps = (size_t)W * H + (enc->cfmt ? 2 * (size_t)(W / 2) * (H / 2) : 0);
+  const uint8_t* base = enc->rec.d + i * ps;
+  B200_CUDA_CHECK(cudaMemcpy2D(y, y_stride, base, W, w, h, cudaMemcpyDeviceToHost));
+  if (enc->cfmt && cb && cr) {
+    const int cw = (w + 1) >> 1, ch = (h + 1) >> 1;
+    B200_CUDA_CHECK(cudaMemcpy2D(cb, c_stride, base + (size_t)W * H, W / 2, cw, ch, cudaMemcpyDeviceToHost));
+    B200_CUDA_CHECK(cudaMemcpy2D(cr, c_stride, base + (size_t)W * H + (size_t)(W / 2) * (H / 2), W / 2, cw, ch, cudaMemcpyDeviceToHost));
+  }
+  return B200_OK;
+}
+
+int b200_gpu_encoder_get_stats(b200_gpu_encoder* enc, b200_gpu_encode_stats* out) {
+  using namespace b200;
+  if (!enc || !out) return set_error(B200_E_INVALID, "null argument");
+  *out = enc->stats;
+  return B200_OK;
+}
+
+}  // extern "C"

@@ -1,4 +1,5 @@
-"""Host HEVC-intra encoder wrapper (b200_hevc_encode_intra) and the synthetic source images of SURVEY.md 8(d)."""
+"""HEVC-intra encoders: the host encoder (b200_hevc_encode_intra), the GPU encoder (GpuEncoder, b200_gpu_encoder_*), and the
+synthetic source images of SURVEY.md 8(d)."""
 import ctypes as C
 
 import numpy as np
@@ -57,6 +58,111 @@ def encode_intra(y, cb=None, cr=None, **kw) -> bytes:
     data = bytes(C.cast(out, C.POINTER(C.c_uint8 * n.value)).contents)
     l.b200_free(out)
     return data
+
+
+class GpuEncodeStats(C.Structure):
+    _fields_ = [("analyse_ms", C.c_double), ("entropy_ms", C.c_double), ("framing_ms", C.c_double), ("total_ms", C.c_double),
+                ("bytes", C.c_uint64), ("ctus", C.c_uint64), ("pictures", C.c_uint64)]
+
+
+# What the GPU encoder codes (b200_heif.h): no SAO, sign hiding or cu_qp_delta, one WPP sub-stream per CTB row.
+GPU_DEFAULTS = dict(sao=0, sign_data_hiding=0, cu_qp_delta=0, wpp=1)
+
+
+def gpu_params(width, height, chroma, **kw) -> EncParams:
+    """b200_hevc_enc_params for b200_gpu_encode_intra_*: the library defaults with GPU_DEFAULTS, then `kw`."""
+    return default_params(width=width, height=height, **{"chroma_format_idc": 1 if chroma else 0, **GPU_DEFAULTS, **kw})
+
+
+def substream_capacity(width, log2_ctb_size, chroma=True) -> int:
+    l = _lib.lib()
+    l.b200_gpu_encoder_substream_capacity.restype = C.c_size_t
+    l.b200_gpu_encoder_substream_capacity.argtypes = [C.c_int, C.c_int, C.c_int]
+    return int(l.b200_gpu_encoder_substream_capacity(width, log2_ctb_size, 1 if chroma else 0))
+
+
+class GpuEncoder:
+    """HEVC intra encoder on the GPU (b200_gpu_encoder_*): N same-sized 8-bit 4:2:0 or 4:0:0 pictures per call.
+
+    encode(pictures, **params) takes a list of (y, cb, cr) tuples -- numpy uint8 host planes or uint8 CUDA tensors,
+    cb = cr = None for monochrome -- and returns one access unit (length-prefixed NALs) per picture."""
+
+    def __init__(self):
+        l = self._l = _lib.lib()
+        l.b200_gpu_encoder_create.argtypes = [C.POINTER(C.c_void_p)]
+        l.b200_gpu_encoder_destroy.argtypes = [C.c_void_p]
+        l.b200_gpu_encoder_destroy.restype = None
+        for f in (l.b200_gpu_encode_intra_device, l.b200_gpu_encode_intra_host):
+            f.argtypes = [C.c_void_p, C.POINTER(EncParams), C.c_int, C.POINTER(_lib.Planes)] + ([C.c_void_p] if f is l.b200_gpu_encode_intra_device else [])
+        l.b200_gpu_encoder_output.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)]
+        l.b200_gpu_encoder_read_recon.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]
+        l.b200_gpu_encoder_get_stats.argtypes = [C.c_void_p, C.POINTER(GpuEncodeStats)]
+        self._h = C.c_void_p()
+        _lib.check(l.b200_gpu_encoder_create(C.byref(self._h)))
+        self._shape = None
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._l.b200_gpu_encoder_destroy(self._h)
+            self._h = C.c_void_p()
+
+    __del__ = close
+
+    def encode(self, pictures, **params):
+        pictures = list(pictures)
+        if not pictures:
+            raise ValueError("no pictures")
+        y0 = pictures[0][0]
+        h, w = int(y0.shape[0]), int(y0.shape[1])
+        chroma = pictures[0][1] is not None
+        p = gpu_params(w, h, chroma, **params)
+        device = hasattr(y0, "is_cuda") and y0.is_cuda
+        keep = []
+        planes = (_lib.Planes * len(pictures))()
+        for i, (y, cb, cr) in enumerate(pictures):
+            q = planes[i]
+            q.height, q.width = int(y.shape[0]), int(y.shape[1])
+            q.chroma = 1 if cb is not None else 0
+            q.bit_depth = 8
+            arrs = [y, cb, cr] if cb is not None else [y]
+            if device:
+                arrs = [a.contiguous() for a in arrs]
+                ptrs, strides = [a.data_ptr() for a in arrs], [a.stride(0) for a in arrs]
+            else:
+                arrs = [np.ascontiguousarray(a, dtype=np.uint8) for a in arrs]
+                ptrs, strides = [a.ctypes.data for a in arrs], [a.strides[0] for a in arrs]
+            keep += arrs
+            q.y, q.y_stride = ptrs[0], strides[0]
+            if cb is not None:
+                q.cb, q.cr, q.c_stride = ptrs[1], ptrs[2], strides[1]
+        if device:
+            import torch
+            stream = torch.cuda.current_stream(y0.device).cuda_stream
+            _lib.check(self._l.b200_gpu_encode_intra_device(self._h, C.byref(p), len(pictures), planes, stream))
+        else:
+            _lib.check(self._l.b200_gpu_encode_intra_host(self._h, C.byref(p), len(pictures), planes))
+        self._shape = (w, h, chroma)
+        out = []
+        for i in range(len(pictures)):
+            d, n = C.POINTER(C.c_uint8)(), C.c_size_t()
+            _lib.check(self._l.b200_gpu_encoder_output(self._h, i, C.byref(d), C.byref(n)))
+            out.append(C.string_at(d, n.value))
+        return out
+
+    def recon(self, i):
+        """Picture i of the last call as reconstructed before in-loop filtering: [y, cb, cr] (uint8; [y] for 4:0:0)."""
+        w, h, chroma = self._shape
+        y = np.empty((h, w), np.uint8)
+        cb = np.empty(((h + 1) // 2, (w + 1) // 2), np.uint8) if chroma else None
+        cr = np.empty_like(cb) if chroma else None
+        _lib.check(self._l.b200_gpu_encoder_read_recon(self._h, i, y.ctypes.data, cb.ctypes.data if chroma else None,
+                                                       cr.ctypes.data if chroma else None, w, (w + 1) // 2 if chroma else 0))
+        return [y, cb, cr] if chroma else [y]
+
+    def stats(self) -> GpuEncodeStats:
+        s = GpuEncodeStats()
+        _lib.check(self._l.b200_gpu_encoder_get_stats(self._h, C.byref(s)))
+        return s
 
 
 def synthetic_image(seed: int, width: int, height: int, bit_depth: int = 8, chroma=True):
