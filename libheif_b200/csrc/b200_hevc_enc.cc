@@ -9,6 +9,10 @@
 // DST 4x4, transform skip, sign-data hiding, cu_qp_delta, chroma QP offsets, SAO band/edge with merges,
 // deblocking overrides, WPP entry points, multiple slices and dependent slice segments, 8..12 bit,
 // 4:2:0 and 4:0:0.  Syntax follows ITU-T H.265 7.3 / 9.3; the reconstruction loop follows 8.4 / 8.6.
+// The arithmetic coder, residual_coding(), intra mode signalling and the constant tables are the ones the GPU encoder
+// uses too (b200_hevc_enc_cabac.h); the parameter sets and slice header come from b200_hevc_enc_headers.h.
+#define B200_SYNTAX_HOST_ONLY 1   // this translation unit uses the shared encoder / syntax code on the host only
+#include "b200_hevc_enc_cabac.h"
 #include "b200_hevc_enc_headers.h"
 #include <algorithm>
 #include <vector>
@@ -16,84 +20,18 @@
 namespace b200 {
 namespace enc {
 
+using namespace syn;
+
 // ------------------------------------------------------------------------------------------ tables
-enum { CTX_SAO_MERGE = 0, CTX_SAO_TYPE = 1, CTX_SPLIT_CU = 2, CTX_PART_MODE = 5, CTX_PREV_INTRA = 6,
-       CTX_CHROMA_PRED = 7, CTX_SPLIT_TR = 8, CTX_CBF_LUMA = 11, CTX_CBF_CHROMA = 13, CTX_QP_DELTA = 18,
-       CTX_TSKIP = 20, CTX_LAST_X = 22, CTX_LAST_Y = 40, CTX_CSBF = 58, CTX_SIG = 62, CTX_GT1 = 104,
-       CTX_GT2 = 128, CTX_TQ_BYPASS = 134, CTX_COUNT = 135 };
-
-static const uint8_t kCtxInitI[CTX_COUNT] = {
-  153, 200, 139, 141, 157, 184, 184, 63, 153, 138, 138, 111, 141, 94, 138, 182, 154, 154, 154, 154, 139, 139,
-  110, 110, 124, 125, 140, 153, 125, 127, 140, 109, 111, 143, 127, 111, 79, 108, 123, 63,
-  110, 110, 124, 125, 140, 153, 125, 127, 140, 109, 111, 143, 127, 111, 79, 108, 123, 63,
-  91, 171, 134, 141,
-  111, 111, 125, 110, 110, 94, 124, 108, 124, 107, 125, 141, 179, 153, 125, 107, 125, 141, 179, 153, 125,
-  107, 125, 141, 179, 153, 125, 140, 139, 182, 182, 152, 136, 152, 136, 153, 136, 139, 111, 136, 139, 111,
-  140, 92, 137, 138, 140, 152, 138, 139, 153, 74, 149, 92, 139, 107, 122, 152, 140, 179, 166, 182, 140, 227, 122, 197,
-  138, 153, 136, 167, 152, 152,
-  154};                                        // cu_transquant_bypass_flag (Table 9-8)
-
-static const uint8_t kRangeLps[64][4] = {
-  {128,176,208,240},{128,167,197,227},{128,158,187,216},{123,150,178,205},{116,142,169,195},{111,135,160,185},
-  {105,128,152,175},{100,122,144,166},{95,116,137,158},{90,110,130,150},{85,104,123,142},{81,99,117,135},
-  {77,94,111,128},{73,89,105,122},{69,85,100,116},{66,80,95,110},{62,76,90,104},{59,72,86,99},{56,69,81,94},
-  {53,65,77,89},{51,62,73,85},{48,59,69,80},{46,56,66,76},{43,53,63,72},{41,50,59,69},{39,48,56,65},
-  {37,45,54,62},{35,43,51,59},{33,41,48,56},{32,39,46,53},{30,37,43,50},{29,35,41,48},{27,33,39,45},
-  {26,31,37,43},{24,30,35,41},{23,28,33,39},{22,27,32,37},{21,26,30,35},{20,24,29,33},{19,23,27,31},
-  {18,22,26,30},{17,21,25,28},{16,20,23,27},{15,19,22,25},{14,18,21,24},{14,17,20,23},{13,16,19,22},
-  {12,15,18,21},{12,14,17,20},{11,14,16,19},{11,13,15,18},{10,12,15,17},{10,12,14,16},{9,11,13,15},
-  {9,11,12,14},{8,10,12,14},{8,9,11,13},{7,9,11,12},{7,9,10,12},{7,8,10,11},{6,8,9,11},{6,7,9,10},
-  {6,7,8,9},{2,2,2,2}};
-static const uint8_t kTransLps[64] = {0,0,1,2,2,4,4,5,6,7,8,9,9,11,11,12,13,13,15,15,16,16,18,18,19,19,21,21,22,22,23,24,
-  24,25,26,26,27,27,28,29,29,30,30,30,31,32,32,33,33,33,34,34,35,35,35,36,36,36,37,37,37,38,38,63};
-
-static const int8_t kDctT[32] = {64, 90, 90, 90, 89, 88, 87, 85, 83, 82, 80, 78, 75, 73, 70, 67,
-                                 64, 61, 57, 54, 50, 46, 43, 38, 36, 31, 25, 22, 18, 13, 9, 4};
-static const int8_t kDst4[4][4] = {{29, 55, 74, 84}, {74, 74, 0, -74}, {84, -29, -74, 55}, {55, -84, 74, -29}};
-static const int8_t kAngle[35] = {0, 0, 32, 26, 21, 17, 13, 9, 5, 2, 0, -2, -5, -9, -13, -17, -21, -26, -32,
-                                  -26, -21, -17, -13, -9, -5, -2, 0, 2, 5, 9, 13, 17, 21, 26, 32};
-static const int16_t kInvAngle[35] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, -4096, -1638, -910, -630, -482, -390, -315, -256,
-                                      -315, -390, -482, -630, -910, -1638, -4096, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-static const uint8_t kSigCtxMap4[16] = {0, 1, 4, 5, 2, 3, 4, 5, 6, 6, 8, 8, 7, 7, 8, 8};
-static const uint8_t kQpcTab[14] = {29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37};
-static const uint8_t kLevelScale[6] = {40, 45, 51, 57, 64, 72};
-static const int kQuantScale[6] = {26214, 23302, 20560, 18396, 16384, 14564};
-
 static int16_t g_mat[4][32][32];       // [log2n-2][k][n] DCT matrices
-static uint8_t g_scan_x[4][3][64], g_scan_y[4][3][64];
 static bool g_tables_ready = false;
 
 static void init_tables() {
   if (g_tables_ready) return;
-  for (int l = 2; l <= 5; l++) {
-    int n = 1 << l;
-    for (int k = 0; k < n; k++) for (int x = 0; x < n; x++) {
-      int v;
-      if (k == 0) v = 64;
-      else {
-        int j = ((k << (5 - l)) * (2 * x + 1)) & 127, sgn = 1;
-        if (j > 64) j = 128 - j;
-        if (j > 32) { j = 64 - j; sgn = -1; }
-        v = sgn * kDctT[j];
-      }
-      g_mat[l - 2][k][x] = (int16_t)v;
-    }
-  }
-  for (int l = 0; l <= 3; l++) {
-    int n = 1 << l, i = 0, x = 0, y = 0;
-    bool stop = false;
-    while (!stop) {
-      while (y >= 0) { if (x < n && y < n) { g_scan_x[l][0][i] = (uint8_t)x; g_scan_y[l][0][i] = (uint8_t)y; i++; } y--; x++; }
-      y = x; x = 0;
-      if (i >= n * n) stop = true;
-    }
-    i = 0; for (y = 0; y < n; y++) for (x = 0; x < n; x++) { g_scan_x[l][1][i] = (uint8_t)x; g_scan_y[l][1][i] = (uint8_t)y; i++; }
-    i = 0; for (x = 0; x < n; x++) for (y = 0; y < n; y++) { g_scan_x[l][2][i] = (uint8_t)x; g_scan_y[l][2][i] = (uint8_t)y; i++; }
-  }
+  for (int l = 2; l <= 5; l++)
+    for (int k = 0; k < (1 << l); k++) for (int x = 0; x < (1 << l); x++) g_mat[l - 2][k][x] = (int16_t)dct_coef(l, k, x);
   g_tables_ready = true;
 }
-
-static inline int clip3(int lo, int hi, int v) { return v < lo ? lo : (v > hi ? hi : v); }
 
 // ------------------------------------------------------------------------------------------ NAL framing
 void append_nal(std::vector<uint8_t>& out, int type, const std::vector<uint8_t>& rbsp) {
@@ -293,55 +231,6 @@ void write_slice_header(BitWriter& b, const SeqHeader& s, int addr0, bool depend
   b.trailing();                                          // byte_alignment()
 }
 
-// ------------------------------------------------------------------------------------------ CABAC encoder (9.3.4.5)
-struct Ctx { uint8_t state, mps; };
-struct Cabac {
-  BitWriter bw; unsigned low = 0, range = 510; int outstanding = 0; bool first = true;
-  void reset() { bw = BitWriter(); low = 0; range = 510; outstanding = 0; first = true; }
-  void put_bit(unsigned b) {
-    if (first) first = false; else bw.put(b, 1);
-    while (outstanding > 0) { bw.put(1 - b, 1); outstanding--; }
-  }
-  void renorm() {
-    while (range < 256) {
-      if (low < 256) put_bit(0);
-      else if (low >= 512) { low -= 512; put_bit(1); }
-      else { low -= 256; outstanding++; }
-      range <<= 1; low <<= 1;
-    }
-  }
-  void bin(Ctx& c, int b) {
-    unsigned lps = kRangeLps[c.state][(range >> 6) & 3];
-    range -= lps;
-    if (b != c.mps) { low += range; range = lps; if (c.state == 0) c.mps = 1 - c.mps; c.state = kTransLps[c.state]; }
-    else if (c.state < 62) c.state++;
-    renorm();
-  }
-  void bypass(int b) {
-    low <<= 1;
-    if (b) low += range;
-    if (low >= 1024) { put_bit(1); low -= 1024; }
-    else if (low < 512) put_bit(0);
-    else { low -= 512; outstanding++; }
-  }
-  void bypass_bits(unsigned v, int n) { for (int i = n - 1; i >= 0; i--) bypass((v >> i) & 1); }
-  void restart() { low = 0; range = 510; outstanding = 0; first = true; }     // 9.3.2.5 after pcm_sample(): same bit writer, fresh interval
-  void terminate(int b) {
-    range -= 2;
-    if (b) { low += range; range = 2; renorm(); put_bit((low >> 9) & 1); bw.put(((low >> 7) & 3) | 1, 2); bw.align_zero(); }
-    else renorm();
-  }
-};
-
-static void init_contexts(Ctx* ctx, int slice_qp) {
-  int qp = clip3(0, 51, slice_qp);
-  for (int i = 0; i < CTX_COUNT; i++) {
-    int iv = kCtxInitI[i], m = (iv >> 4) * 5 - 45, n = ((iv & 15) << 3) - 16;
-    int pre = clip3(1, 126, ((m * qp) >> 4) + n);
-    ctx[i].mps = pre > 63; ctx[i].state = (uint8_t)(ctx[i].mps ? pre - 64 : 63 - pre);
-  }
-}
-
 struct Lcg { uint32_t s; uint32_t next() { s = s * 1664525u + 1013904223u; return s >> 8; } int range(int n) { return (int)(next() % (uint32_t)n); } };
 
 struct SaoParams { int type[3], band_pos[3], eo_class[3], abs[3][4], sign[3][4]; int merge_left, merge_up; };
@@ -446,7 +335,8 @@ class Encoder {
   std::vector<uint16_t> org[3], rec[3];
   std::vector<uint16_t> slice_of4; std::vector<uint8_t> ipm4, cd4; std::vector<int8_t> qp4;
   Lcg rng;
-  Cabac cabac; Ctx ctx[CTX_COUNT], ctx_wpp[CTX_COUNT];
+  uint8_t ctx[CTX_COUNT], ctx_wpp[CTX_COUNT];          // context states, pStateIdx << 1 | valMps
+  CabacWriter<BitWriter> cabac{BitWriter(), ctx};
   std::vector<SaoParams> sao;
   int slice_idx = 0, slice_addr_rs = 0, slice_qp = 26;
   int region_idx = 0;                                  // counts (slice, tile) regions: availability = same region
@@ -500,7 +390,7 @@ class Encoder {
     if (sao.empty()) sao.resize((size_t)total);
     // slice data: one CABAC sub-stream per CTB row when WPP is on, one per tile when tiles are on
     std::vector<std::vector<uint8_t>> substreams;
-    cabac.reset();
+    cabac = {BitWriter(), ctx};
     size_t next_start = 1;
     for (size_t k = 0; k < order.size(); k++) {
       const int a = order[k];
@@ -522,10 +412,10 @@ class Encoder {
       const bool tile_end = tiles && next_start < starts.size() && (int)k + 1 == starts[next_start];
       if (!end && ((P.wpp && (a + 1) % wctb == 0) || tile_end)) {
         cabac.terminate(1);                                // end_of_subset_one_bit (+ byte_alignment)
-        substreams.push_back(cabac.bw.buf); cabac.reset();
+        substreams.push_back(cabac.bits.buf); cabac = {BitWriter(), ctx};
       }
     }
-    substreams.push_back(cabac.bw.buf);
+    substreams.push_back(cabac.bits.buf);
     // header
     BitWriter b;
     std::vector<size_t> escaped;
@@ -561,14 +451,14 @@ class Encoder {
   void write_sao(int rx, int ry) {
     int addr = ry * wctb + rx;
     const SaoParams& s = sao[addr];
-    if (rx > 0 && ctb_region[(size_t)addr - 1] == region_idx) cabac.bin(ctx[CTX_SAO_MERGE], s.merge_left);
+    if (rx > 0 && ctb_region[(size_t)addr - 1] == region_idx) cabac.bin(CTX_SAO_MERGE, s.merge_left);
     if (s.merge_left) return;
-    if (ry > 0 && ctb_region[(size_t)(addr - wctb)] == region_idx) cabac.bin(ctx[CTX_SAO_MERGE], s.merge_up);
+    if (ry > 0 && ctb_region[(size_t)(addr - wctb)] == region_idx) cabac.bin(CTX_SAO_MERGE, s.merge_up);
     if (s.merge_up) return;
     int cmax = (1 << (std::min(bd, 10) - 5)) - 1;
     for (int c = 0; c < (chroma ? 3 : 1); c++) {
       if (c < 2) {
-        cabac.bin(ctx[CTX_SAO_TYPE], s.type[c] != 0);
+        cabac.bin(CTX_SAO_TYPE, s.type[c] != 0);
         if (s.type[c]) cabac.bypass(s.type[c] == 2);
       }
       if (!s.type[c]) continue;
@@ -631,7 +521,7 @@ class Encoder {
         for (int y = 1; y < n; y++) dst[y * n] = (uint16_t)((LEFT(y) + 3 * dc + 2) >> 2);
       }
     } else {
-      int ang = kAngle[mode], ia = kInvAngle[mode];
+      int ang = B200_T(kAngle)[mode], ia = B200_T(kInvAngle)[mode];
       int rbuf[98]; int* r = rbuf + 32;
       if (mode >= 18) {
         for (int x = 0; x <= n; x++) r[x] = TOP(x - 1);
@@ -663,12 +553,12 @@ class Encoder {
     int s1 = log2n + bd - 9, s2 = log2n + 6;
     for (int k = 0; k < n; k++) for (int x = 0; x < n; x++) {        // columns: tmp[k][x] = sum_y M[k][y] res[y][x]
       long e = 0;
-      for (int y = 0; y < n; y++) e += (dst4 ? kDst4[k][y] : g_mat[log2n - 2][k][y]) * res[y * n + x];
+      for (int y = 0; y < n; y++) e += (dst4 ? B200_T(kDst4)[k][y] : g_mat[log2n - 2][k][y]) * res[y * n + x];
       tmp[k * n + x] = (int)((e + (s1 > 0 ? (1 << (s1 - 1)) : 0)) >> s1);
     }
     for (int k = 0; k < n; k++) for (int y = 0; y < n; y++) {        // rows
       long e = 0;
-      for (int x = 0; x < n; x++) e += (dst4 ? kDst4[k][x] : g_mat[log2n - 2][k][x]) * tmp[y * n + x];
+      for (int x = 0; x < n; x++) e += (dst4 ? B200_T(kDst4)[k][x] : g_mat[log2n - 2][k][x]) * tmp[y * n + x];
       coef[y * n + k] = (int)((e + (1 << (s2 - 1))) >> s2);
     }
   }
@@ -678,19 +568,14 @@ class Encoder {
     int tmp[1024];
     for (int x = 0; x < n; x++) for (int y = 0; y < n; y++) {
       int e = 0;
-      for (int k = 0; k < n; k++) e += d[k * n + x] * (dst4 ? kDst4[k][y] : g_mat[log2n - 2][k][y]);
+      for (int k = 0; k < n; k++) e += d[k * n + x] * (dst4 ? B200_T(kDst4)[k][y] : g_mat[log2n - 2][k][y]);
       tmp[y * n + x] = clip3(-32768, 32767, (e + 64) >> 7);
     }
     for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) {
       int e = 0;
-      for (int k = 0; k < n; k++) e += tmp[y * n + k] * (dst4 ? kDst4[k][x] : g_mat[log2n - 2][k][x]);
+      for (int k = 0; k < n; k++) e += tmp[y * n + k] * (dst4 ? B200_T(kDst4)[k][x] : g_mat[log2n - 2][k][x]);
       res[y * n + x] = (e + (1 << (bs - 1))) >> bs;
     }
-  }
-  int chroma_qp(int qpy, int off) const {
-    int qbd = 6 * (bd - 8), qpi = clip3(-qbd, 57, qpy + off);
-    int qpc = cfmt != 1 ? std::min(qpi, 51) : (qpi < 30 ? qpi : (qpi >= 43 ? qpi - 6 : kQpcTab[qpi - 30]));      // Table 8-10 only for ChromaArrayType == 1
-    return qpc + qbd;
   }
 
   // ---------------------------------------------------------------------------- QP (8.6.1)
@@ -710,24 +595,25 @@ class Encoder {
     bool any = false;
     for (int i = 0; i < n * n; i++) {
       long a = std::labs((long)coef[i]);
-      int l = (int)((a * kQuantScale[qp % 6] + add) >> qbits);
+      int l = (int)((a * B200_T(kQuantScale)[qp % 6] + add) >> qbits);
       l = std::min(l, 32767);
       lev[i] = (int16_t)(coef[i] < 0 ? -l : l);
       any |= l != 0;
     }
     if (any && P.sign_data_hiding && !cu_bypass) {
-      int l2sb = log2n - 2;
+      const int l2sb = log2n - 2;
+      const uint8_t *sbx = B200_T(kScanX)[l2sb][scan], *sby = B200_T(kScanY)[l2sb][scan], *px = B200_T(kScanX)[2][scan], *py = B200_T(kScanY)[2][scan];
       for (int i = 0; i < (1 << (2 * l2sb)); i++) {
-        int xs = g_scan_x[l2sb][scan][i], ys = g_scan_y[l2sb][scan][i];
+        int xs = sbx[i], ys = sby[i];
         int first = 16, last = -1, sum = 0;
         for (int k = 0; k < 16; k++) {
-          int v = lev[((ys << 2) + g_scan_y[2][scan][k]) * n + (xs << 2) + g_scan_x[2][scan][k]];
+          int v = lev[((ys << 2) + py[k]) * n + (xs << 2) + px[k]];
           if (v) { if (first == 16) first = k; last = k; sum += std::abs(v); }
         }
         if (last - first > 3) {
-          int16_t& f = lev[((ys << 2) + g_scan_y[2][scan][first]) * n + (xs << 2) + g_scan_x[2][scan][first]];
+          int16_t& f = lev[((ys << 2) + py[first]) * n + (xs << 2) + px[first]];
           if ((sum & 1) != (f < 0 ? 1 : 0)) {               // parity must equal the sign of the first coefficient
-            int16_t& t = lev[((ys << 2) + g_scan_y[2][scan][last]) * n + (xs << 2) + g_scan_x[2][scan][last]];
+            int16_t& t = lev[((ys << 2) + py[last]) * n + (xs << 2) + px[last]];
             t = (int16_t)(t < 0 ? t - 1 : t + 1);
           }
         }
@@ -736,118 +622,20 @@ class Encoder {
     return any;
   }
 
-  void write_residual(const int16_t* lev, int log2n, int c, int scan, bool tskip) {
-    const int n = 1 << log2n, l2sb = log2n - 2;
-    if (P.transform_skip && log2n == 2 && !cu_bypass) cabac.bin(ctx[CTX_TSKIP + (c ? 1 : 0)], tskip);
-    const uint8_t *sbx = g_scan_x[l2sb][scan], *sby = g_scan_y[l2sb][scan], *px = g_scan_x[2][scan], *py = g_scan_y[2][scan];
-    int last_sb = -1, last_pos = -1;
-    for (int i = (1 << (2 * l2sb)) - 1; i >= 0 && last_sb < 0; i--) for (int k = 15; k >= 0; k--)
-      if (lev[((sby[i] << 2) + py[k]) * n + (sbx[i] << 2) + px[k]]) { last_sb = i; last_pos = k; break; }
-    int lx = (sbx[last_sb] << 2) + px[last_pos], ly = (sby[last_sb] << 2) + py[last_pos];
-    if (scan == 2) std::swap(lx, ly);
-    static const uint8_t group[32] = {0, 1, 2, 3, 4, 4, 5, 5, 6, 6, 6, 6, 7, 7, 7, 7, 8, 8, 8, 8, 8, 8, 8, 8, 9, 9, 9, 9, 9, 9, 9, 9};
-    static const uint8_t min_in_group[10] = {0, 1, 2, 3, 4, 6, 8, 12, 16, 24};
-    int cmax = (log2n << 1) - 1, off, shift;
-    if (c == 0) { off = 3 * (log2n - 2) + ((log2n - 1) >> 2); shift = (log2n + 1) >> 2; } else { off = 15; shift = log2n - 2; }
-    int gx = group[lx], gy = group[ly];
-    for (int k = 0; k < gx; k++) cabac.bin(ctx[CTX_LAST_X + off + (k >> shift)], 1);
-    if (gx < cmax) cabac.bin(ctx[CTX_LAST_X + off + (gx >> shift)], 0);
-    for (int k = 0; k < gy; k++) cabac.bin(ctx[CTX_LAST_Y + off + (k >> shift)], 1);
-    if (gy < cmax) cabac.bin(ctx[CTX_LAST_Y + off + (gy >> shift)], 0);
-    if (gx > 3) cabac.bypass_bits(lx - min_in_group[gx], (gx >> 1) - 1);
-    if (gy > 3) cabac.bypass_bits(ly - min_in_group[gy], (gy >> 1) - 1);
-    uint8_t csbf[8][8]; memset(csbf, 0, sizeof csbf);
-    int carry = 1; bool first_done = false;
-    for (int i = last_sb; i >= 0; i--) {
-      int xs = sbx[i], ys = sby[i];
-      int16_t v[16]; bool coded = false;
-      for (int k = 0; k < 16; k++) { v[k] = lev[((ys << 2) + py[k]) * n + (xs << 2) + px[k]]; coded |= v[k] != 0; }
-      bool infer_dc = false;
-      if (i < last_sb && i > 0) {
-        int cs = 0;
-        if (xs + 1 < (1 << l2sb)) cs |= csbf[ys][xs + 1];
-        if (ys + 1 < (1 << l2sb)) cs |= csbf[ys + 1][xs];
-        cabac.bin(ctx[CTX_CSBF + (cs ? 1 : 0) + (c ? 2 : 0)], coded);
-        infer_dc = true;
-      } else coded = true;
-      csbf[ys][xs] = coded;
-      if (!coded) continue;
-      int prev = 0;
-      if (xs + 1 < (1 << l2sb)) prev |= csbf[ys][xs + 1];
-      if (ys + 1 < (1 << l2sb)) prev |= csbf[ys + 1][xs] << 1;
-      int start = i == last_sb ? last_pos - 1 : 15;
-      for (int k = start; k >= 0; k--) {
-        int xc = (xs << 2) + px[k], yc = (ys << 2) + py[k];
-        if (k > 0 || !infer_dc) {
-          int sc;
-          if (log2n == 2) sc = kSigCtxMap4[(yc << 2) + xc];
-          else if (xc + yc == 0) sc = 0;
-          else {
-            int xp = xc & 3, yp = yc & 3;
-            if (prev == 0) sc = (xp + yp == 0) ? 2 : (xp + yp < 3) ? 1 : 0;
-            else if (prev == 1) sc = yp == 0 ? 2 : (yp == 1 ? 1 : 0);
-            else if (prev == 2) sc = xp == 0 ? 2 : (xp == 1 ? 1 : 0);
-            else sc = 2;
-            if (c == 0) { if (xs || ys) sc += 3; sc += log2n == 3 ? (scan == 0 ? 9 : 15) : 21; }
-            else sc += log2n == 3 ? 9 : 12;
-          }
-          cabac.bin(ctx[CTX_SIG + (c == 0 ? sc : 27 + sc)], v[k] != 0);
-          if (v[k]) infer_dc = false;
-        }
-      }
-      int first_sig = 16, last_sig = -1, ng1 = 0, last_g1 = -1, g1ctx = 1;
-      int ctx_set = (i == 0 || c > 0) ? 0 : 2;
-      if (first_done && carry == 0) ctx_set++;
-      first_done = true;
-      bool any = false;
-      for (int k = 15; k >= 0; k--) if (v[k]) {
-        any = true;
-        if (ng1 < 8) {
-          int g = std::abs(v[k]) > 1;
-          cabac.bin(ctx[CTX_GT1 + ctx_set * 4 + std::min(3, g1ctx) + (c ? 16 : 0)], g);
-          ng1++;
-          if (g) { g1ctx = 0; if (last_g1 < 0) last_g1 = k; } else if (g1ctx > 0) g1ctx++;
-        }
-        if (last_sig < 0) last_sig = k;
-        first_sig = k;
-      }
-      if (any) carry = g1ctx;
-      bool hidden = P.sign_data_hiding && !cu_bypass && (last_sig - first_sig > 3);
-      if (last_g1 >= 0) cabac.bin(ctx[CTX_GT2 + ctx_set + (c ? 4 : 0)], std::abs(v[last_g1]) > 2);
-      for (int k = 15; k >= 0; k--) if (v[k] && (!hidden || k != first_sig)) cabac.bypass(v[k] < 0);
-      int nsig = 0, rice = 0, cnt1 = 0;
-      for (int k = 15; k >= 0; k--) if (v[k]) {
-        int a = std::abs(v[k]);
-        int g1 = cnt1 < 8 ? (a > 1) : 0; if (cnt1 < 8) cnt1++;
-        int g2 = (k == last_g1) ? (a > 2) : 0;
-        int base = 1 + g1 + g2;
-        if (base == ((nsig < 8) ? ((k == last_g1) ? 3 : 2) : 1)) {
-          int rem = a - base;
-          if ((rem >> rice) <= 3) { int pre = rem >> rice; for (int t = 0; t < pre; t++) cabac.bypass(1); cabac.bypass(0); cabac.bypass_bits(rem & ((1 << rice) - 1), rice); }
-          else {
-            int q = (rem >> rice) - 2, kk = 0; while ((q >> (kk + 1)) > 0) kk++;
-            int pre = kk + 3;
-            for (int t = 0; t < pre; t++) cabac.bypass(1); cabac.bypass(0);
-            cabac.bypass_bits(rem - (((1 << kk) + 2) << rice), kk + rice);
-          }
-          if (a > 3 * (1 << rice)) rice = std::min(rice + 1, 4);
-        }
-        nsig++;
-      }
-    }
-  }
-
   // one transform block: predict, transform, quantise, (write), reconstruct. Returns cbf.
   struct TbResult { bool cbf; int16_t lev[1024]; int scan; bool tskip; };
+  void write_residual(const TbResult& t, int log2n, int c) {
+    residual_coding(cabac, t.lev, 1 << log2n, log2n, c, t.scan, P.transform_skip && !cu_bypass, t.tskip, P.sign_data_hiding && !cu_bypass);
+  }
   void code_tb(int c, int x0, int y0, int log2n, int mode, TbResult& r) {
     const int n = 1 << log2n, st = stride_of(c);
     uint16_t pred[1024]; int res[1024], coef[1024];
     predict(c, x0, y0, log2n, mode, pred);
     for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) res[y * n + x] = (int)org[c][(size_t)(y0 + y) * st + x0 + x] - pred[y * n + x];
     bool dst4 = c == 0 && log2n == 2;
+    r.scan = log2n == 2 || (log2n == 3 && (c == 0 || cfmt == 3)) ? scan_idx(mode) : 0;
     if (cu_bypass) {                                  // cu_transquant_bypass_flag: the residual is coded as is (8.6.2), lossless
-      r.tskip = false; r.scan = 0;
-      if (log2n == 2 || (log2n == 3 && (c == 0 || cfmt == 3))) { if (mode >= 6 && mode <= 14) r.scan = 2; else if (mode >= 22 && mode <= 30) r.scan = 1; }
+      r.tskip = false;
       r.cbf = false;
       for (int i = 0; i < n * n; i++) { r.lev[i] = (int16_t)res[i]; r.cbf |= res[i] != 0; }
       uint16_t* rq = rec[c].data();
@@ -855,16 +643,14 @@ class Encoder {
       return;
     }
     r.tskip = P.transform_skip && log2n == 2 && rng.range(4) == 0;
-    r.scan = 0;
-    if (log2n == 2 || (log2n == 3 && (c == 0 || cfmt == 3))) { if (mode >= 6 && mode <= 14) r.scan = 2; else if (mode >= 22 && mode <= 30) r.scan = 1; }
     forward(res, coef, log2n, dst4, r.tskip);
-    int qp = c == 0 ? qg_target_qp + 6 * (bd - 8) : chroma_qp(qg_target_qp, (c == 1 ? P.cb_qp_offset : P.cr_qp_offset) + (P.slice_chroma_qp_offsets ? (c == 1 ? P.slice_cb_qp_offset : P.slice_cr_qp_offset) : 0));
+    int qp = c == 0 ? qg_target_qp + 6 * (bd - 8) : chroma_qp(qg_target_qp + (c == 1 ? P.cb_qp_offset : P.cr_qp_offset) + (P.slice_chroma_qp_offsets ? (c == 1 ? P.slice_cb_qp_offset : P.slice_cr_qp_offset) : 0), cfmt, bd);
     r.cbf = quantise(coef, r.lev, log2n, qp, r.scan);
     // NOTE: the QP used here (qg_target_qp) is only valid if a cu_qp_delta can still be sent (or already
     // was); the caller re-runs with the predicted QP when neither holds.
     uint16_t* rp = rec[c].data();
     if (r.cbf) {
-      int16_t d[1024]; int bs = bd + log2n - 5, scale = kLevelScale[qp % 6] << (qp / 6);
+      int16_t d[1024]; int bs = bd + log2n - 5, scale = B200_T(kLevelScale)[qp % 6] << (qp / 6);
       for (int i = 0; i < n * n; i++) { long t = ((long)r.lev[i] * scaling_factor(c, log2n, i) * scale + (1L << (bs - 1))) >> bs; d[i] = (int16_t)(t < -32768 ? -32768 : (t > 32767 ? 32767 : t)); }
       inverse(d, res, log2n, dst4, r.tskip);
       int maxv = (1 << bd) - 1;
@@ -932,36 +718,36 @@ class Encoder {
   void write_tree(const Cu& cu, int me, const bool parent_cb[2], const bool parent_cr[2], int max_depth) {
     const Node& nd = nodes[me];
     bool can_split = nd.log2n <= log2_max_tb && nd.log2n > log2_min_tb && nd.depth < max_depth && !(cu.nxn && nd.depth == 0);
-    if (can_split) cabac.bin(ctx[CTX_SPLIT_TR + 5 - nd.log2n], nd.split);
+    if (can_split) cabac.bin(CTX_SPLIT_TR + 5 - nd.log2n, nd.split);
     bool cb[2] = {false, false}, cr[2] = {false, false};
     if (chroma) {
       if (nd.log2n > 2 || cfmt == 3) {
         const bool two = cfmt == 2 && (!nd.split || nd.log2n == 3);
-        if (nd.depth == 0 || parent_cb[0]) { cb[0] = nd.cbf_cb[0]; cabac.bin(ctx[CTX_CBF_CHROMA + nd.depth], cb[0]); if (two) { cb[1] = nd.cbf_cb[1]; cabac.bin(ctx[CTX_CBF_CHROMA + nd.depth], cb[1]); } }
-        if (nd.depth == 0 || parent_cr[0]) { cr[0] = nd.cbf_cr[0]; cabac.bin(ctx[CTX_CBF_CHROMA + nd.depth], cr[0]); if (two) { cr[1] = nd.cbf_cr[1]; cabac.bin(ctx[CTX_CBF_CHROMA + nd.depth], cr[1]); } }
+        if (nd.depth == 0 || parent_cb[0]) { cb[0] = nd.cbf_cb[0]; cabac.bin(CTX_CBF_CHROMA + nd.depth, cb[0]); if (two) { cb[1] = nd.cbf_cb[1]; cabac.bin(CTX_CBF_CHROMA + nd.depth, cb[1]); } }
+        if (nd.depth == 0 || parent_cr[0]) { cr[0] = nd.cbf_cr[0]; cabac.bin(CTX_CBF_CHROMA + nd.depth, cr[0]); if (two) { cr[1] = nd.cbf_cr[1]; cabac.bin(CTX_CBF_CHROMA + nd.depth, cr[1]); } }
       } else { cb[0] = parent_cb[0]; cb[1] = parent_cb[1]; cr[0] = parent_cr[0]; cr[1] = parent_cr[1]; }
     }
     if (nd.split) { for (int k = 0; k < 4; k++) write_tree(cu, nd.child[k], cb, cr, max_depth); return; }
-    cabac.bin(ctx[CTX_CBF_LUMA + (nd.depth == 0 ? 1 : 0)], nd.cbf_l);
+    cabac.bin(CTX_CBF_LUMA + (nd.depth == 0 ? 1 : 0), nd.cbf_l);
     bool cbf_chroma = chroma && (cb[0] || cb[1] || cr[0] || cr[1]);
     if ((nd.cbf_l || cbf_chroma) && P.cu_qp_delta && !is_qp_delta_coded) {
       int v = cu_qp_delta_val, a = std::abs(v);
-      for (int k = 0; k < std::min(a, 5); k++) cabac.bin(ctx[CTX_QP_DELTA + (k ? 1 : 0)], 1);
-      if (a < 5) cabac.bin(ctx[CTX_QP_DELTA + (a ? 1 : 0)], 0);
+      for (int k = 0; k < std::min(a, 5); k++) cabac.bin(CTX_QP_DELTA + (k ? 1 : 0), 1);
+      if (a < 5) cabac.bin(CTX_QP_DELTA + (a ? 1 : 0), 0);
       else { int rem = a - 5, k = 0; while (rem >= (1 << k)) { cabac.bypass(1); rem -= 1 << k; k++; } cabac.bypass(0); cabac.bypass_bits(rem, k); }
       if (a) cabac.bypass(v < 0);
       is_qp_delta_coded = 1;
     }
-    if (nd.cbf_l) write_residual(nd.l->lev, nd.log2n, 0, nd.l->scan, nd.l->tskip);
+    if (nd.cbf_l) write_residual(*nd.l, nd.log2n, 0);
     if (chroma) {
       const int nb = cfmt == 2 ? 2 : 1;
       if (nd.log2n > 2 || cfmt == 3) {
         const int lc = cfmt == 3 ? nd.log2n : nd.log2n - 1;
-        for (int t = 0; t < nb; t++) if (cb[t]) write_residual(nd.cb[t]->lev, lc, 1, nd.cb[t]->scan, nd.cb[t]->tskip);
-        for (int t = 0; t < nb; t++) if (cr[t]) write_residual(nd.cr[t]->lev, lc, 2, nd.cr[t]->scan, nd.cr[t]->tskip);
+        for (int t = 0; t < nb; t++) if (cb[t]) write_residual(*nd.cb[t], lc, 1);
+        for (int t = 0; t < nb; t++) if (cr[t]) write_residual(*nd.cr[t], lc, 2);
       } else if (nd.blk == 3) {
-        for (int t = 0; t < nb; t++) if (parent_cb[t]) write_residual(nd.cb[t]->lev, 2, 1, nd.cb[t]->scan, nd.cb[t]->tskip);
-        for (int t = 0; t < nb; t++) if (parent_cr[t]) write_residual(nd.cr[t]->lev, 2, 2, nd.cr[t]->scan, nd.cr[t]->tskip);
+        for (int t = 0; t < nb; t++) if (parent_cb[t]) write_residual(*nd.cb[t], 2, 1);
+        for (int t = 0; t < nb; t++) if (parent_cr[t]) write_residual(*nd.cr[t], 2, 2);
       }
     }
   }
@@ -971,13 +757,7 @@ class Encoder {
     int ca = 1, cb = 1;
     if (avail(x - 1, y)) ca = ipm4[(size_t)(y >> 2) * w4 + ((x - 1) >> 2)];
     if (avail(x, y - 1) && (y - 1) >= ((y >> log2ctb) << log2ctb)) cb = ipm4[(size_t)((y - 1) >> 2) * w4 + (x >> 2)];
-    if (ca == cb) {
-      if (ca < 2) { cand[0] = 0; cand[1] = 1; cand[2] = 26; }
-      else { cand[0] = ca; cand[1] = 2 + ((ca + 29) % 32); cand[2] = 2 + ((ca - 2 + 1) % 32); }
-    } else {
-      cand[0] = ca; cand[1] = cb;
-      if (ca != 0 && cb != 0) cand[2] = 0; else if (ca != 1 && cb != 1) cand[2] = 1; else cand[2] = 26;
-    }
+    mpm_candidates(ca, cb, cand);
   }
 
   int choose_mode(int x0, int y0, int log2n, const int cand[3]) {
@@ -1002,8 +782,8 @@ class Encoder {
     Cu cu{}; cu.x0 = x0; cu.y0 = y0; cu.log2cb = log2cb;
     const int n = 1 << log2cb;
     cu_bypass = false;
-    if (P.transquant_bypass) { cu_bypass = P.transquant_bypass == 2 || rng.range(4) == 0; cabac.bin(ctx[CTX_TQ_BYPASS], cu_bypass); }
-    if (log2cb == 3) { cu.nxn = rng.range(3) == 0; cabac.bin(ctx[CTX_PART_MODE], !cu.nxn); }
+    if (P.transquant_bypass) { cu_bypass = P.transquant_bypass == 2 || rng.range(4) == 0; cabac.bin(CTX_TQ_BYPASS, cu_bypass); }
+    if (log2cb == 3) { cu.nxn = rng.range(3) == 0; cabac.bin(CTX_PART_MODE, !cu.nxn); }
     if (P.pcm && !cu.nxn && log2cb <= std::min(5, log2ctb)) {
       const bool pcm = rng.range(6) == 0;
       cabac.terminate(pcm ? 1 : 0);                   // pcm_flag (terminate bin); value 1: flush, stop bit, pcm_alignment_zero_bits
@@ -1014,7 +794,7 @@ class Encoder {
           for (int y = 0; y < (n >> shy); y++) for (int x = 0; x < (n >> shx); x++) {
             const size_t idx = (size_t)((y0 >> shy) + y) * st + (x0 >> shx) + x;
             const unsigned v = org[c][idx] >> (bd - pbd);
-            cabac.bw.put(v, pbd);                     // pcm_sample_luma / pcm_sample_chroma
+            cabac.bits.put(v, pbd);                     // pcm_sample_luma / pcm_sample_chroma
             rq[idx] = (uint16_t)(v << (bd - pbd));
           }
         }
@@ -1032,39 +812,28 @@ class Encoder {
       }
     }
     int np = cu.nxn ? 4 : 1, pb = cu.nxn ? n / 2 : n;
-    int prev[4], mpm_idx[4], rem[4];
+    int code[4];
     for (int i = 0; i < np; i++) {
       int px = x0 + (i & 1) * pb, py = y0 + (i >> 1) * pb, cand[3];
       mpm(px, py, cand);
       int mode = choose_mode(px, py, cu.nxn ? 2 : log2cb, cand);
       cu.lmode[i] = mode;
-      prev[i] = 0; mpm_idx[i] = 0; rem[i] = 0;
-      for (int k = 0; k < 3; k++) if (cand[k] == mode) { prev[i] = 1; mpm_idx[i] = k; }
-      if (!prev[i]) {
-        int s[3] = {cand[0], cand[1], cand[2]}; std::sort(s, s + 3);
-        int r = mode; for (int k = 2; k >= 0; k--) if (r > s[k]) r--;
-        rem[i] = r;
-      }
+      code[i] = mpm_code(mode, cand);
       for (int yy = 0; yy < pb; yy += 4) for (int xx = 0; xx < pb; xx += 4) {
         size_t idx = (size_t)((py + yy) >> 2) * w4 + ((px + xx) >> 2);
         ipm4[idx] = (uint8_t)mode; slice_of4[idx] = (uint16_t)(region_idx + 1);
       }
     }
-    for (int i = 0; i < np; i++) cabac.bin(ctx[CTX_PREV_INTRA], prev[i]);
-    for (int i = 0; i < np; i++) {
-      if (prev[i]) { cabac.bypass(mpm_idx[i] > 0); if (mpm_idx[i] > 0) cabac.bypass(mpm_idx[i] > 1); }
-      else cabac.bypass_bits(rem[i], 5);
-    }
+    write_luma_modes(cabac, np, code);
     if (chroma) {
       // intra_chroma_pred_mode: one per prediction unit in 4:4:4, else one per coding unit (7.3.8.5); 8.4.3 + Table 8-3 for 4:2:2
-      static const uint8_t tab[4] = {0, 26, 10, 1};
       static const uint8_t k422[35] = {0, 1, 2, 2, 2, 2, 3, 5, 7, 8, 10, 12, 13, 15, 17, 18, 19, 20, 21, 22, 23, 23, 24, 24, 25, 25, 26, 27, 27, 28, 28, 29, 29, 30, 31};
       for (int i = 0; i < (cfmt == 3 ? np : 1); i++) {
         int v = rng.range(8); if (v > 4) v = 4;
-        int m = (v < 4 && tab[v] == cu.lmode[i]) ? 34 : (v == 4 ? cu.lmode[i] : tab[v]);
+        int m = (v < 4 && B200_T(kChromaTab)[v] == cu.lmode[i]) ? 34 : (v == 4 ? cu.lmode[i] : B200_T(kChromaTab)[v]);
         if (cfmt == 2) m = k422[m];
         cu.cmode[i] = m;
-        cabac.bin(ctx[CTX_CHROMA_PRED], v != 4);
+        cabac.bin(CTX_CHROMA_PRED, v != 4);
         if (v != 4) cabac.bypass_bits(v, 2);
       }
     }
@@ -1114,7 +883,7 @@ class Encoder {
       int inc = 0;
       if (avail(x0 - 1, y0) && cd4[(size_t)(y0 >> 2) * w4 + ((x0 - 1) >> 2)] > depth) inc++;
       if (avail(x0, y0 - 1) && cd4[(size_t)((y0 - 1) >> 2) * w4 + (x0 >> 2)] > depth) inc++;
-      cabac.bin(ctx[CTX_SPLIT_CU + inc], split);
+      cabac.bin(CTX_SPLIT_CU + inc, split);
     } else split = log2cb > 3;
     if (P.cu_qp_delta && log2cb >= qg_log2) {
       is_qp_delta_coded = 0; cu_qp_delta_val = 0;

@@ -12,6 +12,7 @@ namespace enc {
 
 struct BitWriter {
   std::vector<uint8_t> buf; int nbits = 0; uint8_t cur = 0;
+  void put1(unsigned b) { put(b, 1); }
   void put(unsigned v, int n) { for (int i = n - 1; i >= 0; i--) { cur = (uint8_t)((cur << 1) | ((v >> i) & 1)); if (++nbits == 8) { buf.push_back(cur); cur = 0; nbits = 0; } } }
   void ue(unsigned v) { unsigned x = v + 1; int len = 0; while ((x >> len) > 1) len++; put(0, len); put(x, len + 1); }
   void se(int v) { ue(v > 0 ? 2 * v - 1 : -2 * v); }

@@ -7,9 +7,10 @@
 //      inverse path of 8.6.  Writes the reconstruction (HBM plane: the neighbours of the next row), the luma modes per 4x4,
 //      the CU size / partition per 8x8 and the quantised levels (a coefficient plane: every TB's levels at its position).
 //      Rows trail the row above by two CTBs through per-row progress counters.
-//   E2 (CABAC), one warp per WPP sub-stream (= CTB row): the syntax of 7.3.8 from E1's records, the arithmetic coder of
-//      9.3.4.5, context hand-over after the 2nd CTB of the row above (9.3.2.2), end_of_slice_segment_flag per CTB and
-//      end_of_subset_one_bit + byte alignment per row, into a per-row buffer sized for the worst case.
+//   E2 (CABAC), one warp per WPP sub-stream (= CTB row): the syntax of 7.3.8 from E1's records, context hand-over after
+//      the 2nd CTB of the row above (9.3.2.2), end_of_slice_segment_flag per CTB and end_of_subset_one_bit + byte
+//      alignment per row, into a per-row buffer sized for the worst case.  The arithmetic coder, residual_coding(), the
+//      intra mode signalling and the constant tables are the host encoder's (b200_hevc_enc_cabac.h).
 //   Framing (host): parameter sets and slice header (b200_hevc_enc_headers.h, shared with the host encoder), entry points
 //      over the escaped sub-stream sizes, emulation prevention, length prefixes.
 //
@@ -22,7 +23,7 @@
 #include "b200_internal.h"
 #include "b200_staging.h"
 #include "b200_hevc_enc_headers.h"
-#include "b200_hevc_syntax.h"
+#include "b200_hevc_enc_cabac.h"
 #include <algorithm>
 #include <chrono>
 #include <memory>
@@ -37,18 +38,6 @@ namespace b200 {
 namespace genc {
 
 using syn::clip3;
-
-B200_TABLE(int8_t, kDctT, [32], {64, 90, 90, 90, 89, 88, 87, 85, 83, 82, 80, 78, 75, 73, 70, 67,
-                                 64, 61, 57, 54, 50, 46, 43, 38, 36, 31, 25, 22, 18, 13, 9, 4})
-B200_TABLE(int8_t, kDst4, [4][4], {{29, 55, 74, 84}, {74, 74, 0, -74}, {84, -29, -74, 55}, {55, -84, 74, -29}})
-B200_TABLE(int8_t, kAngle, [35], {0, 0, 32, 26, 21, 17, 13, 9, 5, 2, 0, -2, -5, -9, -13, -17, -21, -26, -32,
-                                  -26, -21, -17, -13, -9, -5, -2, 0, 2, 5, 9, 13, 17, 21, 26, 32})
-B200_TABLE(int16_t, kInvAngle, [35], {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, -4096, -1638, -910, -630, -482, -390, -315, -256,
-                                      -315, -390, -482, -630, -910, -1638, -4096, 0, 0, 0, 0, 0, 0, 0, 0, 0})
-B200_TABLE(int32_t, kQuantScale, [6], {26214, 23302, 20560, 18396, 16384, 14564})
-B200_TABLE(uint8_t, kLevelScale, [6], {40, 45, 51, 57, 64, 72})
-B200_TABLE(uint8_t, kLastGroup, [32], {0, 1, 2, 3, 4, 4, 5, 5, 6, 6, 6, 6, 7, 7, 7, 7, 8, 8, 8, 8, 8, 8, 8, 8, 9, 9, 9, 9, 9, 9, 9, 9})
-B200_TABLE(uint8_t, kLastGroupMin, [10], {0, 1, 2, 3, 4, 6, 8, 12, 16, 24})
 
 enum { CU_NXN = 0x80 };
 
@@ -104,27 +93,14 @@ struct Ctx2 { const Args& a; int p; int lane; Work& w;
   }
 };
 
-__device__ inline int dct_coef(int log2n, int k, int x) {        // DCT matrix entry [k][x] of an n x n transform (8.6.4.2)
-  if (k == 0) return 64;
-  int j = ((k << (5 - log2n)) * (2 * x + 1)) & 127, sgn = 1;
-  if (j > 64) j = 128 - j;
-  if (j > 32) { j = 64 - j; sgn = -1; }
-  return sgn * B200_T(kDctT)[j];
-}
-__device__ inline int tmat(bool dst4, int log2n, int k, int x) { return dst4 ? B200_T(kDst4)[k][x] : dct_coef(log2n, k, x); }
+__device__ inline int tmat(bool dst4, int log2n, int k, int x) { return dst4 ? enc::B200_T(kDst4)[k][x] : enc::dct_coef(log2n, k, x); }
 
 // 8.4.2: the three most probable modes of the PU at luma (x, y)
 __device__ inline void mpm_cand(const uint8_t* ipm, int w4, int log2ctb, int x, int y, int cand[3]) {
   int ca = 1, cb = 1;
   if (x > 0) ca = GE_LD(ipm + (size_t)(y >> 2) * w4 + ((x - 1) >> 2));
   if (y > 0 && (y - 1) >= ((y >> log2ctb) << log2ctb)) cb = GE_LD(ipm + (size_t)((y - 1) >> 2) * w4 + (x >> 2));
-  if (ca == cb) {
-    if (ca < 2) { cand[0] = 0; cand[1] = 1; cand[2] = 26; }
-    else { cand[0] = ca; cand[1] = 2 + ((ca + 29) % 32); cand[2] = 2 + ((ca - 2 + 1) % 32); }
-  } else {
-    cand[0] = ca; cand[1] = cb;
-    if (ca != 0 && cb != 0) cand[2] = 0; else if (ca != 1 && cb != 1) cand[2] = 1; else cand[2] = 26;
-  }
+  enc::mpm_candidates(ca, cb, cand);
 }
 __device__ inline int mode_bits(int mode, const int cand[3]) { return mode == cand[0] ? 2 : (mode == cand[1] || mode == cand[2]) ? 3 : 6; }
 
@@ -186,7 +162,7 @@ __device__ inline int pred_px(const Work& w, int c, int log2n, int mode, int x, 
     }
     return dc;
   }
-  const int ang = B200_T(kAngle)[mode], ia = B200_T(kInvAngle)[mode];
+  const int ang = enc::B200_T(kAngle)[mode], ia = enc::B200_T(kInvAngle)[mode];
   if (mode >= 18) {
     if (mode == 26 && c == 0 && n < 32 && x == 0) return clip3(0, 255, TOP(0) + ((LEFT(y) - LEFT(-1)) >> 1));
     const int idx = ((y + 1) * ang) >> 5, f = ((y + 1) * ang) & 31, k1 = x + idx + 1, k2 = k1 + 1;
@@ -274,7 +250,7 @@ __device__ int code_tb(Ctx2& e, int c, int x0, int y0, int log2n, int mode, bool
     w.tmp[i] = (s + (1 << (s1 - 1))) >> s1;
   }
   GE_SYNC();
-  const int qbits = 14 + qp / 6 + (7 - log2n), qs = B200_T(kQuantScale)[qp % 6];
+  const int qbits = 14 + qp / 6 + (7 - log2n), qs = enc::B200_T(kQuantScale)[qp % 6];
   const long long add = 171LL << (qbits - 9);
   for (int i = e.lane; i < nn; i += GE_LANES) {
     const int y = i >> log2n, k = i & (n - 1);
@@ -289,7 +265,7 @@ __device__ int code_tb(Ctx2& e, int c, int x0, int y0, int log2n, int mode, bool
   if (final) { int16_t* cp = e.cplane(c); for (int i = e.lane; i < nn; i += GE_LANES) cp[(size_t)(y0 + (i >> log2n)) * st + x0 + (i & (n - 1))] = w.lev[i]; }
   uint8_t* rp = e.plane(c);
   if (w.any) {
-    const int bs = log2n + 3, scale = B200_T(kLevelScale)[qp % 6] << (qp / 6);
+    const int bs = log2n + 3, scale = enc::B200_T(kLevelScale)[qp % 6] << (qp / 6);
     for (int i = e.lane; i < nn; i += GE_LANES) {
       const long long t = ((long long)w.lev[i] * 16 * scale + (1LL << (bs - 1))) >> bs;
       w.coef[i] = (int)(t < -32768 ? -32768 : (t > 32767 ? 32767 : t));
@@ -450,61 +426,17 @@ __device__ void e1_row(const Args& a, Work& w, int p, int ry, int lane) {
 }
 
 // ---------------------------------------------------------------------------------------------------- E2
-struct Cabac {                                                // 9.3.4.5 (arithmetic encoder with outstanding bits)
-  uint8_t* out; size_t cap, pos; unsigned cur; int nbits;
-  unsigned low, range; int outstanding; bool first, overflow;
-  uint8_t* ctx;                                               // CTX_COUNT entries: pStateIdx << 1 | valMps
-  __device__ void put1(unsigned b) {
+// E2's bit sink: the row's buffer of `cap` bytes; a sub-stream that would pass it sets `overflow` instead of writing
+struct RowSink {
+  uint8_t* out; size_t cap, pos; unsigned cur; int nbits; bool overflow;
+  B200_HD void put1(unsigned b) {
     cur = (cur << 1) | b;
     if (++nbits == 8) { if (pos < cap) out[pos++] = (uint8_t)cur; else overflow = true; cur = 0; nbits = 0; }
   }
-  __device__ void put_bit(unsigned b) {
-    if (first) first = false; else put1(b);
-    while (outstanding > 0) { put1(1 - b); outstanding--; }
-  }
-  __device__ void renorm() {
-    while (range < 256) {
-      if (low < 256) put_bit(0);
-      else if (low >= 512) { low -= 512; put_bit(1); }
-      else { low -= 256; outstanding++; }
-      range <<= 1; low <<= 1;
-    }
-  }
-  __device__ void bin(int ci, int b) {
-    const unsigned s = ctx[ci], state = s >> 1, mps = s & 1;
-    const unsigned lps = (syn::B200_T(kLps4)[state] >> (8 * ((range >> 6) & 3))) & 0xff;
-    range -= lps;
-    if ((unsigned)b != mps) {
-      low += range; range = lps;
-      ctx[ci] = (uint8_t)((syn::B200_T(kTransLps)[state] << 1) | (state == 0 ? 1 - mps : mps));
-    } else if (state < 62) ctx[ci] = (uint8_t)(((state + 1) << 1) | mps);
-    renorm();
-  }
-  __device__ void bypass(int b) {
-    low <<= 1;
-    if (b) low += range;
-    if (low >= 1024) { put_bit(1); low -= 1024; }
-    else if (low < 512) put_bit(0);
-    else { low -= 512; outstanding++; }
-  }
-  __device__ void bypass_bits(unsigned v, int n) { for (int i = n - 1; i >= 0; i--) bypass((v >> i) & 1); }
-  __device__ void terminate(int b) {
-    range -= 2;
-    if (b) {
-      low += range; range = 2; renorm(); put_bit((low >> 9) & 1);
-      put1((((low >> 7) & 3) | 1) >> 1); put1(1);
-      while (nbits) put1(0);
-    } else renorm();
-  }
+  B200_HD void put(unsigned v, int n) { for (int i = n - 1; i >= 0; i--) put1((v >> i) & 1); }
+  B200_HD void align_zero() { while (nbits) put1(0); }
 };
-
-__device__ inline void init_ctx(uint8_t* ctx, int qp) {
-  for (int i = 0; i < syn::CTX_COUNT; i++) {
-    const int iv = syn::B200_T(kInitI)[i], m = (iv >> 4) * 5 - 45, nn = ((iv & 15) << 3) - 16;
-    const int pre = clip3(1, 126, ((m * qp) >> 4) + nn), mps = pre > 63;
-    ctx[i] = (uint8_t)(((mps ? pre - 64 : 63 - pre) << 1) | mps);
-  }
-}
+using Cabac = enc::CabacWriter<RowSink>;
 
 struct Writer {
   const Args& a; int p; Cabac& cb;
@@ -516,111 +448,10 @@ struct Writer {
     return false;
   }
 
-  __device__ void residual(int c, int x0, int y0, int log2n, int scan) {     // 7.3.8.11
-    using namespace syn;
-    const int n = 1 << log2n, l2sb = log2n - 2, st = c ? a.Wc : a.W;
-    const int16_t* pl = cplane(c) + (size_t)y0 * st + x0;
-    const uint8_t *sbx = B200_T(kScanX)[l2sb][scan], *sby = B200_T(kScanY)[l2sb][scan], *px = B200_T(kScanX)[2][scan], *py = B200_T(kScanY)[2][scan];
-#define LEV(xx, yy) ((int)pl[(size_t)(yy) * st + (xx)])
-    int last_sb = -1, last_pos = -1;
-    for (int i = (1 << (2 * l2sb)) - 1; i >= 0 && last_sb < 0; i--) for (int k = 15; k >= 0; k--)
-      if (LEV((sbx[i] << 2) + px[k], (sby[i] << 2) + py[k])) { last_sb = i; last_pos = k; break; }
-    int lx = (sbx[last_sb] << 2) + px[last_pos], ly = (sby[last_sb] << 2) + py[last_pos];
-    if (scan == 2) { const int t = lx; lx = ly; ly = t; }
-    const uint8_t* group = B200_T(kLastGroup);
-    const uint8_t* min_in_group = B200_T(kLastGroupMin);
-    const int cmax = (log2n << 1) - 1;
-    int off, shift;
-    if (c == 0) { off = 3 * (log2n - 2) + ((log2n - 1) >> 2); shift = (log2n + 1) >> 2; } else { off = 15; shift = log2n - 2; }
-    const int gx = group[lx], gy = group[ly];
-    for (int k = 0; k < gx; k++) cb.bin(CTX_LAST_X + off + (k >> shift), 1);
-    if (gx < cmax) cb.bin(CTX_LAST_X + off + (gx >> shift), 0);
-    for (int k = 0; k < gy; k++) cb.bin(CTX_LAST_Y + off + (k >> shift), 1);
-    if (gy < cmax) cb.bin(CTX_LAST_Y + off + (gy >> shift), 0);
-    if (gx > 3) cb.bypass_bits(lx - min_in_group[gx], (gx >> 1) - 1);
-    if (gy > 3) cb.bypass_bits(ly - min_in_group[gy], (gy >> 1) - 1);
-    uint64_t csbf = 0;                                        // coded_sub_block_flag, bit ys * 8 + xs
-#define CSBF(xx, yy) ((int)((csbf >> ((yy) * 8 + (xx))) & 1))
-    int carry = 1; bool first_done = false;
-    for (int i = last_sb; i >= 0; i--) {
-      const int xs = sbx[i], ys = sby[i];
-      int v[16]; bool coded = false;
-      for (int k = 0; k < 16; k++) { v[k] = LEV((xs << 2) + px[k], (ys << 2) + py[k]); coded |= v[k] != 0; }
-      bool infer_dc = false;
-      if (i < last_sb && i > 0) {
-        int cs = 0;
-        if (xs + 1 < (1 << l2sb)) cs |= CSBF(xs + 1, ys);
-        if (ys + 1 < (1 << l2sb)) cs |= CSBF(xs, ys + 1);
-        cb.bin(CTX_CSBF + (cs ? 1 : 0) + (c ? 2 : 0), coded);
-        infer_dc = true;
-      } else coded = true;
-      if (coded) csbf |= 1ull << (ys * 8 + xs);
-      if (!coded) continue;
-      int prev = 0;
-      if (xs + 1 < (1 << l2sb)) prev |= CSBF(xs + 1, ys);
-      if (ys + 1 < (1 << l2sb)) prev |= CSBF(xs, ys + 1) << 1;
-      const int start = i == last_sb ? last_pos - 1 : 15;
-      for (int k = start; k >= 0; k--) {
-        const int xc = (xs << 2) + px[k], yc = (ys << 2) + py[k];
-        if (k > 0 || !infer_dc) {
-          int sc;
-          if (log2n == 2) sc = B200_T(kSigMap4)[(yc << 2) + xc];
-          else if (xc + yc == 0) sc = 0;
-          else {
-            const int xp = xc & 3, yp = yc & 3;
-            if (prev == 0) sc = (xp + yp == 0) ? 2 : (xp + yp < 3) ? 1 : 0;
-            else if (prev == 1) sc = yp == 0 ? 2 : (yp == 1 ? 1 : 0);
-            else if (prev == 2) sc = xp == 0 ? 2 : (xp == 1 ? 1 : 0);
-            else sc = 2;
-            if (c == 0) { if (xs || ys) sc += 3; sc += log2n == 3 ? (scan == 0 ? 9 : 15) : 21; }
-            else sc += log2n == 3 ? 9 : 12;
-          }
-          cb.bin(CTX_SIG + (c == 0 ? sc : 27 + sc), v[k] != 0);
-          if (v[k]) infer_dc = false;
-        }
-      }
-      int ng1 = 0, last_g1 = -1, g1ctx = 1;
-      int ctx_set = (i == 0 || c > 0) ? 0 : 2;
-      if (first_done && carry == 0) ctx_set++;
-      first_done = true;
-      bool any = false;
-      for (int k = 15; k >= 0; k--) if (v[k]) {
-        any = true;
-        if (ng1 < 8) {
-          const int g = abs(v[k]) > 1;
-          cb.bin(CTX_GT1 + ctx_set * 4 + min(3, g1ctx) + (c ? 16 : 0), g);
-          ng1++;
-          if (g) { g1ctx = 0; if (last_g1 < 0) last_g1 = k; } else if (g1ctx > 0) g1ctx++;
-        }
-      }
-      if (any) carry = g1ctx;
-      if (last_g1 >= 0) cb.bin(CTX_GT2 + ctx_set + (c ? 4 : 0), abs(v[last_g1]) > 2);
-      for (int k = 15; k >= 0; k--) if (v[k]) cb.bypass(v[k] < 0);
-      int nsig = 0, rice = 0, cnt1 = 0;
-      for (int k = 15; k >= 0; k--) if (v[k]) {
-        const int av = abs(v[k]);
-        const int g1 = cnt1 < 8 ? (av > 1) : 0; if (cnt1 < 8) cnt1++;
-        const int g2 = (k == last_g1) ? (av > 2) : 0;
-        const int base = 1 + g1 + g2;
-        if (base == ((nsig < 8) ? ((k == last_g1) ? 3 : 2) : 1)) {
-          const int rem = av - base;
-          if ((rem >> rice) <= 3) { const int pre = rem >> rice; for (int t = 0; t < pre; t++) cb.bypass(1); cb.bypass(0); cb.bypass_bits(rem & ((1 << rice) - 1), rice); }
-          else {
-            const int q = (rem >> rice) - 2; int kk = 0; while ((q >> (kk + 1)) > 0) kk++;
-            for (int t = 0; t < kk + 3; t++) cb.bypass(1);
-            cb.bypass(0);
-            cb.bypass_bits(rem - (((1 << kk) + 2) << rice), kk + rice);
-          }
-          if (av > 3 * (1 << rice)) rice = min(rice + 1, 4);
-        }
-        nsig++;
-      }
-    }
-#undef LEV
-#undef CSBF
+  __device__ void residual(int c, int x0, int y0, int log2n, int scan) {
+    const int st = c ? a.Wc : a.W;
+    enc::residual_coding(cb, cplane(c) + (size_t)y0 * st + x0, st, log2n, c, scan, false, false, false);
   }
-
-  __device__ static int scan_of(int mode) { return (mode >= 6 && mode <= 14) ? 2 : (mode >= 22 && mode <= 30) ? 1 : 0; }
 
   // transform tree (7.3.8.8 / 7.3.8.10): TU = CU apart from the implied splits
   template <int L>
@@ -648,14 +479,14 @@ struct Writer {
     const int pu = nxn ? ((y0 > cuy) ? 2 : 0) + ((x0 > cux) ? 1 : 0) : 0;
     const bool cbf_l = nonzero(0, x0, y0, 1 << log2n);
     cb.bin(CTX_CBF_LUMA + (depth == 0 ? 1 : 0), cbf_l);
-    if (cbf_l) residual(0, x0, y0, log2n, log2n <= 3 ? scan_of(lmode[pu]) : 0);
+    if (cbf_l) residual(0, x0, y0, log2n, log2n <= 3 ? enc::scan_idx(lmode[pu]) : 0);
     if (chroma) {
       if (log2n > 2) {
-        if (ccb) residual(1, x0 >> 1, y0 >> 1, log2n - 1, log2n - 1 == 2 ? scan_of(cmode) : 0);
-        if (ccr) residual(2, x0 >> 1, y0 >> 1, log2n - 1, log2n - 1 == 2 ? scan_of(cmode) : 0);
+        if (ccb) residual(1, x0 >> 1, y0 >> 1, log2n - 1, log2n - 1 == 2 ? enc::scan_idx(cmode) : 0);
+        if (ccr) residual(2, x0 >> 1, y0 >> 1, log2n - 1, log2n - 1 == 2 ? enc::scan_idx(cmode) : 0);
       } else if (blk == 3) {
-        if (pcb) residual(1, cux >> 1, cuy >> 1, 2, scan_of(cmode));
-        if (pcr) residual(2, cux >> 1, cuy >> 1, 2, scan_of(cmode));
+        if (pcb) residual(1, cux >> 1, cuy >> 1, 2, enc::scan_idx(cmode));
+        if (pcr) residual(2, cux >> 1, cuy >> 1, 2, enc::scan_idx(cmode));
       }
     }
   }
@@ -684,27 +515,14 @@ struct Writer {
     if (log2cb == 3) cb.bin(CTX_PART_MODE, !nxn);
     const int np = nxn ? 4 : 1, pb = nxn ? n / 2 : n;
     const uint8_t* ipm = a.ipm4 + (size_t)p * a.map4;
-    int lmode[4] = {0, 0, 0, 0}, prev[4], idx[4], rem[4];
+    int lmode[4] = {0, 0, 0, 0}, code[4];
     for (int i = 0; i < np; i++) {
       const int px = x0 + (i & 1) * pb, py = y0 + (i >> 1) * pb;
       int cand[3]; mpm_cand(ipm, W >> 2, a.log2ctb, px, py, cand);
       const int mode = ipm[(size_t)(py >> 2) * (W >> 2) + (px >> 2)];
-      lmode[i] = mode; prev[i] = 0; idx[i] = 0; rem[i] = 0;
-      for (int k = 0; k < 3; k++) if (cand[k] == mode) { prev[i] = 1; idx[i] = k; }
-      if (!prev[i]) {
-        int s0 = cand[0], s1 = cand[1], s2 = cand[2], t;
-        if (s0 > s1) { t = s0; s0 = s1; s1 = t; }
-        if (s1 > s2) { t = s1; s1 = s2; s2 = t; }
-        if (s0 > s1) { t = s0; s0 = s1; s1 = t; }
-        int r = mode; if (r > s2) r--; if (r > s1) r--; if (r > s0) r--;
-        rem[i] = r;
-      }
+      lmode[i] = mode; code[i] = enc::mpm_code(mode, cand);
     }
-    for (int i = 0; i < np; i++) cb.bin(CTX_PREV_INTRA, prev[i]);
-    for (int i = 0; i < np; i++) {
-      if (prev[i]) { cb.bypass(idx[i] > 0); if (idx[i] > 0) cb.bypass(idx[i] > 1); }
-      else cb.bypass_bits(rem[i], 5);
-    }
+    enc::write_luma_modes(cb, np, code);
     if (a.cfmt) cb.bin(CTX_CHROMA_PRED, 0);                    // intra_chroma_pred_mode = 4 (DM)
     tree<L>(x0, y0, 0, 0, nxn, a.max_th_depth + (nxn ? 1 : 0), lmode, lmode[0], false, false, x0, y0);
   }
@@ -713,12 +531,12 @@ struct Writer {
 __device__ void e2_row(const Args& a, uint8_t* ctx, int p, int ry, int lane) {
   const size_t row = (size_t)p * a.hctb + ry;
   if (lane == 0) {
-    Cabac cb{a.ss + row * a.ss_cap, a.ss_cap, 0, 0, 0, 0, 510, 0, true, false, ctx};
+    Cabac cb{RowSink{a.ss + row * a.ss_cap, a.ss_cap, 0, 0, 0, false}, ctx};
     Writer wr{a, p, cb};
     if (ry > 0 && a.wctb >= 2) {
       const uint8_t* src = a.wpp_ctx + (row - 1) * syn::CTX_COUNT;
       for (int i = 0; i < syn::CTX_COUNT; i++) ctx[i] = GE_LD(src + i);
-    } else init_ctx(ctx, a.slice_qp);
+    } else enc::init_contexts(ctx, a.slice_qp);
     for (int rx = 0; rx < a.wctb; rx++) {
       if (a.log2ctb == 6) wr.quadtree<6>(rx << a.log2ctb, ry << a.log2ctb, 0); else wr.quadtree<5>(rx << a.log2ctb, ry << a.log2ctb, 0);
       if (rx == 1) {
@@ -730,8 +548,8 @@ __device__ void e2_row(const Args& a, uint8_t* ctx, int p, int ry, int lane) {
       cb.terminate(last ? 1 : 0);                              // end_of_slice_segment_flag
       if (!last && rx == a.wctb - 1) cb.terminate(1);          // end_of_subset_one_bit + byte_alignment()
     }
-    a.ss_len[row] = (unsigned)cb.pos;
-    if (cb.overflow) atomicOr(a.error, 1u);
+    a.ss_len[row] = (unsigned)cb.bits.pos;
+    if (cb.bits.overflow) atomicOr(a.error, 1u);
   }
 }
 
@@ -826,12 +644,6 @@ int validate(const b200_hevc_enc_params* p, int n, const b200_planes* pics) {
 // SATD-domain Lagrangian: lambda = sqrt(0.57 * 2^((QP - 12) / 3)), in 1/16 units
 inline int lambda16(int qp) { return (int)(16.0 * std::sqrt(0.57 * std::pow(2.0, (qp - 12) / 3.0)) + 0.5); }
 
-inline int chroma_qp(int qpy, int off) {                      // 8.6.1, ChromaArrayType 1, 8 bit
-  static const uint8_t tab[14] = {29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37};
-  const int qpi = clip3(0, 57, qpy + off);
-  return qpi < 30 ? qpi : (qpi >= 43 ? qpi - 6 : tab[qpi - 30]);
-}
-
 int encode(b200_gpu_encoder* e, const b200_hevc_enc_params* p, int n, const Pic* host_pics, cudaStream_t s) {
   using clk = std::chrono::steady_clock;
   const auto t0 = clk::now();
@@ -856,8 +668,8 @@ int encode(b200_gpu_encoder* e, const b200_hevc_enc_params* p, int n, const Pic*
   a.pics = e->pics.d; a.n = n; a.W = W; a.H = H; a.Wc = Wc; a.Hc = Hc; a.sw = p->width; a.sh = p->height;
   a.cfmt = cfmt; a.log2ctb = log2ctb; a.wctb = wctb; a.hctb = hctb; a.max_th_depth = p->max_transform_hierarchy_depth_intra;
   a.strong = p->strong_intra_smoothing != 0; a.slice_qp = p->qp;
-  a.qp[0] = p->qp; a.qp[1] = chroma_qp(p->qp, p->cb_qp_offset + p->slice_cb_qp_offset * (p->slice_chroma_qp_offsets != 0));
-  a.qp[2] = chroma_qp(p->qp, p->cr_qp_offset + p->slice_cr_qp_offset * (p->slice_chroma_qp_offsets != 0));
+  a.qp[0] = p->qp; a.qp[1] = enc::chroma_qp(p->qp + p->cb_qp_offset + p->slice_cb_qp_offset * (p->slice_chroma_qp_offsets != 0), cfmt, 8);
+  a.qp[2] = enc::chroma_qp(p->qp + p->cr_qp_offset + p->slice_cr_qp_offset * (p->slice_chroma_qp_offsets != 0), cfmt, 8);
   a.lambda16 = lambda16(p->qp);
   a.rec = e->rec.d; a.coef = e->coef.d; a.pic_samples = pic_samples; a.ipm4 = e->ipm4.d; a.dec4 = e->dec4.d; a.map4 = map4;
   a.cu8 = e->cu8.d; a.map8 = map8;
