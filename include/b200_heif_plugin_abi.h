@@ -123,6 +123,9 @@ int b200_plugin_bind_libheif(void* dl_handle);
 /* Submission queue of the decoder plugin (concurrent decode_next_image2 calls are decoded as one batch, see b200_plugin.cc):
    out3 = {batches decoded, pictures decoded, largest batch}. */
 void b200_plugin_queue_stats(uint64_t out3[3]);
+/* The "b200-gpu" encoder instances of the process (still images, and the batched frames of sequences):
+   out3 = {GPU encode calls, pictures encoded, largest call}. */
+void b200_plugin_encoder_stats(uint64_t out3[3]);
 
 #ifdef __cplusplus
 }
