@@ -285,6 +285,44 @@ int b200_gpu_encoder_get_stats(b200_gpu_encoder* enc, b200_gpu_encode_stats* out
    more fails the call instead of writing past it. */
 size_t b200_gpu_encoder_substream_capacity(int width, int log2_ctb_size, int chroma_format_idc);
 
+/* One call from an 8-bit RGB picture to the access units of a HEIC grid: colour conversion, tiling and HEVC coding on the
+ * device -- what heif_context_encode_grid with the "b200-gpu" plugin does one tile per encode_image call
+ * (libheif/image-items/grid.cc:886-906), as two batches on the GPU.
+ * Tiles: cols = ceil(width / tile_w) x rows = ceil(height / tile_h), raster order; tile (c, r) is the tile_w x tile_h window at
+ * (c * tile_w, r * tile_h), edge-replicated (clamped coordinates) where it overhangs the picture.  Its access unit is byte for
+ * byte what b200_gpu_encode_intra_* writes for the 4:2:0 picture b200_rgb_to_ycbcr_ex_* makes from that padded window.
+ * Input: RGB24 / RGBA32 (B200_CHROMA_INTERLEAVED_RGB / _RGBA) or planar 8-bit R, G, B (B200_CHROMA_444) with an optional alpha
+ * plane.  Conversion target and SPS signalling: p's colour_primaries / matrix_coefficients / full_range; chroma_downsampling /
+ * only_use_preferred from opt (NULL = libheif's defaults).  p: as for b200_gpu_encode_intra_* with chroma_format_idc 1;
+ * width / height are set by the call (tile_w x tile_h).  An input with alpha gives a second batch of tiles, the padded alpha
+ * windows coded as 4:0:0 pictures with the same parameters (libheif codes alpha through the same plugin the same way).
+ * Output: b200_gpu_encoder_output(enc, i) -- i in [0, n) the colour tiles, [n, 2n) the alpha tiles (n = cols * rows);
+ * b200_gpu_encoder_get_stats sums both batches; b200_gpu_encoder_read_recon holds the last batch coded (alpha when present).
+ * Refusals, all before any CUDA call (b200_gpu_encode_rgb_grid_check): B200_E_UNSUPPORTED for a depth above 8 bits, for
+ * what b200_rgb_to_ycbcr_plan refuses for this target, and for what b200_gpu_encode_check refuses for a tile_w x tile_h
+ * picture; B200_E_INVALID for odd tile sizes or tiles outside 8..16384, NULL pointers, strides shorter than a row. */
+typedef struct b200_grid_encode_info {
+  int cols, rows, tile_w, tile_h;      /* tiles = ceil(W / tile_w) x ceil(H / tile_h), raster order */
+  int width, height;                   /* grid output size = the input picture's size */
+  int has_alpha;                       /* alpha tiles coded as 4:0:0 pictures in the same call */
+  int pipeline;                        /* B200_YCC_PIPE_* of the colour chain, as b200_rgb_to_ycbcr_plan reports */
+  double colour_ms, upload_ms;         /* CUDA events: colour kernels (summed over the bands of the host form), H2D of the host
+                                          form (0 for the device form); E1 / E2 / framing stay in b200_gpu_encoder_get_stats */
+} b200_grid_encode_info;
+
+int b200_gpu_encode_rgb_grid_check(const b200_rgb_image* in, int tile_w, int tile_h, const b200_hevc_enc_params* p,
+                                   const b200_rgb_to_ycbcr_options* opt);              /* host only, no CUDA */
+/* device RGB; `stream` = cudaStream_t (NULL = default stream); returns when the access units are in host memory.
+   info may be NULL. */
+int b200_gpu_encode_rgb_grid_device(b200_gpu_encoder* enc, const b200_rgb_image* in, int tile_w, int tile_h,
+                                    const b200_hevc_enc_params* p, const b200_rgb_to_ycbcr_options* opt,
+                                    void* stream, b200_grid_encode_info* info);
+/* host RGB: uploaded in row bands through the encoder's page-locked bounce buffer; band k is converted on the device while
+   band k + 1 is in flight.  The device buffers stay with the encoder for its next call. */
+int b200_gpu_encode_rgb_grid_host(b200_gpu_encoder* enc, const b200_rgb_image* in, int tile_w, int tile_h,
+                                  const b200_hevc_enc_params* p, const b200_rgb_to_ycbcr_options* opt,
+                                  b200_grid_encode_info* info);
+
 /* ------------------------------------------------------------------------------------------------
  * HEVC intra decoder: header parsing on the host; CABAC + slice-data syntax, reconstruction, deblocking and SAO as
  * sm_90a kernels (CABAC can be moved to host threads with b200_decoder_set_front_end).

@@ -589,7 +589,9 @@ struct b200_gpu_encoder {
   b200::Pool pool{std::max(1, std::min(16, (int)std::thread::hardware_concurrency()))};
   b200::Bounce bounce;
   b200::Stream stream;
+  b200::Stream work;                  // colour stage + encode of b200_gpu_encode_rgb_grid_host (`stream` carries its uploads)
   b200::Event ev[3];
+  b200::DevBuf<uint8_t> rgb;          // b200_gpu_encode_rgb_grid_host: the uploaded RGB
   b200::DevBuf<uint8_t> src, rec, ipm4, dec4, cu8, wpp_ctx, ss, packed;
   b200::DevBuf<int16_t> coef;
   b200::DevBuf<unsigned> sync, ss_len;
@@ -598,6 +600,7 @@ struct b200_gpu_encoder {
   std::vector<std::vector<uint8_t>> out;
   b200_hevc_enc_params params{};
   int n = 0, W = 0, H = 0, cfmt = 1;
+  int rec_first = 0;                  // output index of the first picture whose reconstruction `rec` holds
   b200_gpu_encode_stats stats{};
   bool ready = false;
 };
@@ -729,7 +732,154 @@ int encode(b200_gpu_encoder* e, const b200_hevc_enc_params* p, int n, const Pic*
   st.total_ms = std::chrono::duration<double, std::milli>(t2 - t0).count();
   st.bytes = 0; for (auto& o : e->out) st.bytes += o.size();
   st.ctus = (uint64_t)rows * wctb; st.pictures = (uint64_t)n;
-  e->params = *p; e->n = n; e->W = W; e->H = H; e->cfmt = cfmt; e->ready = true;
+  e->params = *p; e->n = n; e->W = W; e->H = H; e->cfmt = cfmt; e->rec_first = 0; e->ready = true;
+  return B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------- RGB grid in one call
+struct GridPlan {
+  int cols, rows, pw, ph, pipeline;
+  bool alpha, interleaved;
+  b200_hevc_enc_params q;             // the colour tiles' parameters (tile size, 4:2:0)
+};
+
+int grid_check(const b200_rgb_image* in, int tw, int th, const b200_hevc_enc_params* p, const b200_rgb_to_ycbcr_options* opt, GridPlan* g) {
+  if (!in || !p) return set_error(B200_E_INVALID, "null argument");
+  if (in->bit_depth > 8) return set_error(B200_E_UNSUPPORTED, "bit depth %d: the grid encoder takes 8-bit RGB (the GPU encoder codes 8-bit pictures)", in->bit_depth);
+  g->interleaved = in->chroma == B200_CHROMA_INTERLEAVED_RGB || in->chroma == B200_CHROMA_INTERLEAVED_RGBA;
+  if (!g->interleaved && in->chroma != B200_CHROMA_444)
+    return set_error(B200_E_UNSUPPORTED, "RGB input chroma %d: the grid encoder takes RGB24, RGBA32 or planar 8-bit RGB", in->chroma);
+  if (in->chroma == B200_CHROMA_444 && in->alpha && in->alpha_bit_depth > 8)
+    return set_error(B200_E_UNSUPPORTED, "alpha bit depth %d: the grid encoder takes 8-bit alpha", in->alpha_bit_depth);
+  if ((tw | th) & 1 || tw < 8 || th < 8 || tw > 16384 || th > 16384)
+    return set_error(B200_E_INVALID, "tile size %dx%d: even sizes from 8 to 16384", tw, th);
+  if (in->width <= 0 || in->height <= 0) return set_error(B200_E_INVALID, "picture size %dx%d", in->width, in->height);
+  b200_planes t{};                    // the conversion target: what the SPS signals
+  t.width = in->width; t.height = in->height; t.chroma = B200_CHROMA_420; t.bit_depth = 8;
+  t.colour_primaries = p->colour_primaries; t.transfer_characteristics = p->transfer_characteristics;
+  t.matrix_coefficients = p->matrix_coefficients; t.full_range = p->full_range;
+  if (int rc = plan_rgb_to_ycbcr(in, &t, opt, &g->pipeline)) return rc;
+  g->alpha = in->chroma == B200_CHROMA_INTERLEAVED_RGBA || (in->chroma == B200_CHROMA_444 && in->alpha);
+  if (g->interleaved) {
+    if (!in->rgb) return set_error(B200_E_INVALID, "RGB input plane missing");
+    if (in->rgb_stride < (size_t)in->width * (g->alpha ? 4 : 3)) return set_error(B200_E_INVALID, "RGB stride %zu < row of %d pixels", in->rgb_stride, in->width);
+  } else {
+    if (!in->r || !in->g || !in->b) return set_error(B200_E_INVALID, "RGB input planes missing");
+    const size_t st[4] = {in->r_stride, in->g_stride, in->b_stride, in->alpha_stride};
+    for (int c = 0; c < (g->alpha ? 4 : 3); c++)
+      if (st[c] < (size_t)in->width) return set_error(B200_E_INVALID, "plane %d stride %zu < row of %d samples", c, st[c], in->width);
+  }
+  g->q = *p;
+  g->q.width = tw; g->q.height = th;
+  b200_planes d{};                    // stands for every tile: only checked for NULL, size, chroma and depth
+  d.y = d.cb = d.cr = in; d.y_stride = (size_t)tw; d.c_stride = (size_t)tw / 2; d.width = tw; d.height = th; d.bit_depth = 8;
+  d.chroma = p->chroma_format_idc ? B200_CHROMA_420 : B200_CHROMA_MONO;
+  if (int rc = validate(&g->q, 1, &d)) return rc;
+  if (p->chroma_format_idc != 1) return set_error(B200_E_UNSUPPORTED, "chroma_format_idc %d: the colour tiles are coded 4:2:0", p->chroma_format_idc);
+  g->cols = (int)(((long long)in->width + tw - 1) / tw); g->rows = (int)(((long long)in->height + th - 1) / th);
+  if ((long long)g->cols * tw > (1 << 30) || (long long)g->rows * th > (1 << 30) || (long long)g->cols * g->rows > (1 << 24))
+    return set_error(B200_E_INVALID, "grid of %dx%d tiles of %dx%d", g->cols, g->rows, tw, th);
+  g->pw = g->cols * tw; g->ph = g->rows * th;
+  return B200_OK;
+}
+
+int grid_encode(b200_gpu_encoder* e, const b200_rgb_image* in, int tw, int th, const b200_hevc_enc_params* p, const b200_rgb_to_ycbcr_options* opt,
+                bool host, cudaStream_t s, b200_grid_encode_info* info) {
+  using clk = std::chrono::steady_clock;
+  const auto t0 = clk::now();
+  if (!e) return set_error(B200_E_INVALID, "null encoder");
+  GridPlan g;
+  if (int rc = grid_check(in, tw, th, p, opt, &g)) return rc;
+  e->ready = false;
+  // the padded picture: Y, Cb, Cr (and alpha) planes of pw x ph, the tiles are windows of it
+  const size_t ys = ((size_t)g.pw + 63) & ~(size_t)63, cs = ((size_t)g.pw / 2 + 63) & ~(size_t)63, ph = (size_t)g.ph;
+  if (int rc = e->src.reserve(ys * ph + cs * ph + (g.alpha ? ys * ph : 0), false)) return rc;
+  uint8_t* const Y = e->src.d; uint8_t* const Cb = Y + ys * ph; uint8_t* const Cr = Cb + cs * (ph / 2); uint8_t* const A = Cr + cs * (ph / 2);
+  b200_planes out{};
+  out.y = Y; out.cb = Cb; out.cr = Cr; out.alpha = g.alpha ? A : nullptr; out.y_stride = out.alpha_stride = ys; out.c_stride = cs;
+  out.width = g.pw; out.height = g.ph; out.chroma = B200_CHROMA_420; out.bit_depth = 8;
+  out.colour_primaries = p->colour_primaries; out.transfer_characteristics = p->transfer_characteristics;
+  out.matrix_coefficients = p->matrix_coefficients; out.full_range = p->full_range;
+  const int W = in->width, H = in->height;
+  int nb = 1;                         // row bands of the host form
+  size_t band = (size_t)H;
+  b200_rgb_image d = *in;             // the input as the colour stage reads it
+  const int nplanes = g.interleaved ? 1 : (g.alpha ? 4 : 3);
+  const size_t wb = g.interleaved ? (size_t)W * (g.alpha ? 4 : 3) : (size_t)W;
+  if (host) {
+    band = std::max<size_t>(2, (((size_t)32 << 20) / (wb * nplanes)) & ~(size_t)1);
+    nb = (int)((H + band - 1) / band);
+    if (!e->work.h) B200_CUDA_CHECK(cudaStreamCreateWithFlags(&e->work.h, cudaStreamNonBlocking));
+    if (int rc = e->rgb.reserve(wb * nplanes * (size_t)H, false)) return rc;
+    if (g.interleaved) { d.rgb = e->rgb.d; d.rgb_stride = wb; }
+    else {
+      d.r = e->rgb.d; d.g = e->rgb.d + wb * H; d.b = e->rgb.d + 2 * wb * H; d.alpha = g.alpha ? e->rgb.d + 3 * wb * H : nullptr;
+      d.r_stride = d.g_stride = d.b_stride = d.alpha_stride = wb;
+    }
+  }
+  cudaStream_t ws = host ? (cudaStream_t)e->work : s;
+  // events: [0] upload start, [1] band arrived, [2] upload end, then the start / end of each band's colour kernel
+  std::unique_ptr<Event[]> ev(new Event[3 + 2 * (size_t)nb]);
+  for (int k = 0; k < 3 + 2 * nb; k++) B200_CUDA_CHECK(cudaEventCreate(&ev[k].h));
+  if (host) B200_CUDA_CHECK(cudaEventRecord(ev[0], e->stream));
+  for (int k = 0, oy = 0; k < nb; k++) {
+    const size_t y0 = (size_t)k * band, y1 = std::min((size_t)H, y0 + band);
+    if (host) {
+      const void* srcs[4] = {in->rgb, nullptr, nullptr, nullptr};
+      size_t sst[4] = {in->rgb_stride, 0, 0, 0};
+      if (!g.interleaved) {
+        srcs[0] = in->r; srcs[1] = in->g; srcs[2] = in->b; srcs[3] = in->alpha;
+        sst[0] = in->r_stride; sst[1] = in->g_stride; sst[2] = in->b_stride; sst[3] = in->alpha_stride;
+      }
+      for (int c = 0; c < nplanes; c++)
+        if (int rc = e->bounce.upload(e->rgb.d + c * wb * H + y0 * wb, wb, (const uint8_t*)srcs[c] + y0 * sst[c], sst[c], wb, y1 - y0, e->stream, e->pool)) return rc;
+      B200_CUDA_CHECK(cudaEventRecord(ev[1], e->stream));
+      B200_CUDA_CHECK(cudaStreamWaitEvent(ws, ev[1], 0));
+    }
+    // output rows that need source rows < y1 only (all of them after the last band: the padding below the picture)
+    const int oy1 = k == nb - 1 ? g.ph : (int)y1;
+    B200_CUDA_CHECK(cudaEventRecord(ev[3 + 2 * k], ws));
+    if (int rc = launch_rgb_to_ycbcr_grid(&d, &out, g.pipeline, oy, oy1, ws)) return rc;
+    B200_CUDA_CHECK(cudaEventRecord(ev[4 + 2 * k], ws));
+    oy = oy1;
+  }
+  if (host) B200_CUDA_CHECK(cudaEventRecord(ev[2], e->stream));
+  // colour tiles, then alpha tiles, as windows of the padded picture
+  const int n = g.cols * g.rows;
+  std::vector<Pic> hp(n);
+  for (int i = 0; i < n; i++) {
+    const size_t r = (size_t)(i / g.cols), c = (size_t)(i % g.cols);
+    hp[i].src[0] = Y + r * th * ys + c * tw; hp[i].stride[0] = ys;
+    hp[i].src[1] = Cb + r * (th / 2) * cs + c * (tw / 2); hp[i].src[2] = Cr + r * (th / 2) * cs + c * (tw / 2); hp[i].stride[1] = hp[i].stride[2] = cs;
+  }
+  if (int rc = encode(e, &g.q, n, hp.data(), ws)) return rc;
+  if (g.alpha) {
+    std::vector<std::vector<uint8_t>> colour = std::move(e->out);
+    const b200_gpu_encode_stats st = e->stats;
+    for (int i = 0; i < n; i++) {
+      const size_t r = (size_t)(i / g.cols), c = (size_t)(i % g.cols);
+      hp[i].src[0] = A + r * th * ys + c * tw; hp[i].src[1] = hp[i].src[2] = nullptr;
+    }
+    b200_hevc_enc_params qa = g.q;
+    qa.chroma_format_idc = 0;
+    if (int rc = encode(e, &qa, n, hp.data(), ws)) return rc;
+    for (auto& o : e->out) colour.push_back(std::move(o));
+    e->out = std::move(colour);
+    e->n = 2 * n; e->rec_first = n;
+    b200_gpu_encode_stats& t = e->stats;
+    t.analyse_ms += st.analyse_ms; t.entropy_ms += st.entropy_ms; t.framing_ms += st.framing_ms;
+    t.bytes += st.bytes; t.ctus += st.ctus; t.pictures += st.pictures;
+  }
+  e->stats.total_ms = std::chrono::duration<double, std::milli>(clk::now() - t0).count();
+  if (info) {
+    float ms = 0;
+    info->cols = g.cols; info->rows = g.rows; info->tile_w = tw; info->tile_h = th; info->width = W; info->height = H;
+    info->has_alpha = g.alpha ? 1 : 0; info->pipeline = g.pipeline;
+    info->colour_ms = 0;
+    for (int k = 0; k < nb; k++) { cudaEventElapsedTime(&ms, ev[3 + 2 * k], ev[4 + 2 * k]); info->colour_ms += ms; }
+    info->upload_ms = 0;
+    if (host && cudaEventSynchronize(ev[2]) == cudaSuccess) { cudaEventElapsedTime(&ms, ev[0], ev[2]); info->upload_ms = ms; }
+  }
   return B200_OK;
 }
 
@@ -790,6 +940,22 @@ int b200_gpu_encode_intra_host(b200_gpu_encoder* enc, const b200_hevc_enc_params
   return genc::encode(enc, p, n, hp.data(), enc->stream);
 }
 
+int b200_gpu_encode_rgb_grid_check(const b200_rgb_image* in, int tile_w, int tile_h, const b200_hevc_enc_params* p,
+                                   const b200_rgb_to_ycbcr_options* opt) {
+  b200::genc::GridPlan g;
+  return b200::genc::grid_check(in, tile_w, tile_h, p, opt, &g);
+}
+
+int b200_gpu_encode_rgb_grid_device(b200_gpu_encoder* enc, const b200_rgb_image* in, int tile_w, int tile_h, const b200_hevc_enc_params* p,
+                                    const b200_rgb_to_ycbcr_options* opt, void* stream, b200_grid_encode_info* info) {
+  return b200::genc::grid_encode(enc, in, tile_w, tile_h, p, opt, false, (cudaStream_t)stream, info);
+}
+
+int b200_gpu_encode_rgb_grid_host(b200_gpu_encoder* enc, const b200_rgb_image* in, int tile_w, int tile_h, const b200_hevc_enc_params* p,
+                                  const b200_rgb_to_ycbcr_options* opt, b200_grid_encode_info* info) {
+  return b200::genc::grid_encode(enc, in, tile_w, tile_h, p, opt, true, nullptr, info);
+}
+
 int b200_gpu_encoder_output(b200_gpu_encoder* enc, int i, const uint8_t** data, size_t* size) {
   using namespace b200;
   if (!enc || !data || !size) return set_error(B200_E_INVALID, "null argument");
@@ -801,10 +967,10 @@ int b200_gpu_encoder_output(b200_gpu_encoder* enc, int i, const uint8_t** data, 
 int b200_gpu_encoder_read_recon(b200_gpu_encoder* enc, int i, void* y, void* cb, void* cr, size_t y_stride, size_t c_stride) {
   using namespace b200;
   if (!enc || !y) return set_error(B200_E_INVALID, "null argument");
-  if (!enc->ready || i < 0 || i >= enc->n) return set_error(B200_E_INVALID, "no picture %d in the last call", i);
+  if (!enc->ready || i < enc->rec_first || i >= enc->n) return set_error(B200_E_INVALID, "no picture %d in the last call", i);
   const int w = enc->params.width, h = enc->params.height, W = enc->W, H = enc->H;
   const size_t ps = (size_t)W * H + (enc->cfmt ? 2 * (size_t)(W / 2) * (H / 2) : 0);
-  const uint8_t* base = enc->rec.d + i * ps;
+  const uint8_t* base = enc->rec.d + (size_t)(i - enc->rec_first) * ps;
   B200_CUDA_CHECK(cudaMemcpy2D(y, y_stride, base, W, w, h, cudaMemcpyDeviceToHost));
   if (enc->cfmt && cb && cr) {
     const int cw = (w + 1) >> 1, ch = (h + 1) >> 1;

@@ -81,6 +81,54 @@ def substream_capacity(width, log2_ctb_size, chroma=True) -> int:
     return int(l.b200_gpu_encoder_substream_capacity(width, log2_ctb_size, 1 if chroma else 0))
 
 
+class GridEncodeInfo(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("cols", "rows", "tile_w", "tile_h", "width", "height", "has_alpha", "pipeline")] + \
+        [("colour_ms", C.c_double), ("upload_ms", C.c_double)]
+
+
+def _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferred, bit_depth, endianness, alpha_bit_depth, params):
+    """(b200_rgb_image, params, options, device?) of the b200_gpu_encode_rgb_grid_* calls; rgb: numpy array or CUDA tensor
+    [H, W, 3|4], or a tuple (R, G, B) of [H, W] planes with the optional alpha plane in `alpha`."""
+    from .color import _np_is16, _np_packed, _rgb_image
+    planar = isinstance(rgb, (tuple, list))
+    if alpha is not None and not planar:
+        raise ValueError("alpha= is the alpha plane of planar input; interleaved input carries alpha as RGBA")
+    if planar:
+        if len(rgb) != 3:
+            raise ValueError("planar input: (R, G, B) planes, alpha in alpha=")
+        rgb = tuple(rgb) + ((alpha,) if alpha is not None else ())
+    first = rgb[0] if planar else rgb
+    device = hasattr(first, "is_cuda") and first.is_cuda
+    if device:
+        d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda t: t.data_ptr(), lambda t: t.stride(0) * t.element_size(),
+                          lambda t: t.element_size() == 2, lambda t: t.stride(-1) == 1 and (t.dim() == 2 or t.stride(1) == t.shape[2]))
+    else:
+        d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda a: a.ctypes.data, lambda a: a.strides[0], _np_is16, _np_packed)
+    p = gpu_params(tile_w, tile_h, True, **params)
+    opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
+    return d, p, opt, device
+
+
+def _bind_grid(l):
+    l.b200_gpu_encode_rgb_grid_check.argtypes = [C.POINTER(_lib.RgbImage), C.c_int, C.c_int, C.POINTER(EncParams), C.POINTER(_lib.RgbToYCbCrOptions)]
+    l.b200_gpu_encode_rgb_grid_device.argtypes = [C.c_void_p, C.POINTER(_lib.RgbImage), C.c_int, C.c_int, C.POINTER(EncParams),
+                                                  C.POINTER(_lib.RgbToYCbCrOptions), C.c_void_p, C.POINTER(GridEncodeInfo)]
+    l.b200_gpu_encode_rgb_grid_host.argtypes = [C.c_void_p, C.POINTER(_lib.RgbImage), C.c_int, C.c_int, C.POINTER(EncParams),
+                                                C.POINTER(_lib.RgbToYCbCrOptions), C.POINTER(GridEncodeInfo)]
+
+
+def grid_encode_check(rgb, tile_w, tile_h, alpha=None, chroma_downsampling=2, only_use_preferred=False, input_bit_depth=None, endianness=None,
+                      alpha_bit_depth=None, **params):
+    """Host only, no CUDA (b200_gpu_encode_rgb_grid_check): raises B200Error with the code and message
+    GpuEncoder.encode_rgb_grid would fail with for these arguments (numpy input; no pixel is read).  input_bit_depth /
+    endianness / alpha_bit_depth describe uint16 inputs as rgb_to_ycbcr_ex's bit_depth / endianness / alpha_bit_depth do."""
+    l = _lib.lib()
+    _bind_grid(l)
+    d, p, opt, _ = _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferred, input_bit_depth, endianness, alpha_bit_depth,
+                              params)
+    _lib.check(l.b200_gpu_encode_rgb_grid_check(C.byref(d), tile_w, tile_h, C.byref(p), C.byref(opt)))
+
+
 class GpuEncoder:
     """HEVC intra encoder on the GPU (b200_gpu_encoder_*): N same-sized 8-bit 4:2:0 or 4:0:0 pictures per call.
 
@@ -148,6 +196,36 @@ class GpuEncoder:
             _lib.check(self._l.b200_gpu_encoder_output(self._h, i, C.byref(d), C.byref(n)))
             out.append(C.string_at(d, n.value))
         return out
+
+    def encode_rgb_grid(self, rgb, tile_w, tile_h, alpha=None, chroma_downsampling=2, only_use_preferred=False, **params):
+        """An 8-bit RGB picture -> the access units of a HEIC grid of tile_w x tile_h tiles in one call
+        (b200_gpu_encode_rgb_grid_host for numpy input, _device for CUDA tensors, on the tensor's current stream).
+
+        rgb: [H, W, 3|4] uint8 (RGB / RGBA), or a tuple (R, G, B) of [H, W] uint8 planes with the optional alpha plane in
+        `alpha`.  params: b200_hevc_enc_params fields as for encode(); colour_primaries / matrix_coefficients / full_range are
+        the conversion target as well.  Returns dict(tiles=[bytes] in raster order, alpha=[bytes] or None, cols, rows, width,
+        height, pipeline (B200_YCC_PIPE_* mask), colour_ms, upload_ms)."""
+        d, p, opt, device = _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferred, None, None, None, params)
+        _bind_grid(self._l)
+        info = GridEncodeInfo()
+        if device:
+            import torch
+            first = rgb[0] if isinstance(rgb, (tuple, list)) else rgb
+            with torch.cuda.device(first.device):
+                stream = torch.cuda.current_stream(first.device).cuda_stream
+                _lib.check(self._l.b200_gpu_encode_rgb_grid_device(self._h, C.byref(d), tile_w, tile_h, C.byref(p), C.byref(opt), stream,
+                                                                   C.byref(info)))
+        else:
+            _lib.check(self._l.b200_gpu_encode_rgb_grid_host(self._h, C.byref(d), tile_w, tile_h, C.byref(p), C.byref(opt), C.byref(info)))
+        self._shape = (tile_w, tile_h, not info.has_alpha)       # recon(): the last batch coded (the alpha tiles when present)
+        n = info.cols * info.rows
+        out = []
+        for i in range(n * (2 if info.has_alpha else 1)):
+            dp, sz = C.POINTER(C.c_uint8)(), C.c_size_t()
+            _lib.check(self._l.b200_gpu_encoder_output(self._h, i, C.byref(dp), C.byref(sz)))
+            out.append(C.string_at(dp, sz.value))
+        return dict(tiles=out[:n], alpha=out[n:] if info.has_alpha else None, cols=info.cols, rows=info.rows, width=info.width,
+                    height=info.height, pipeline=info.pipeline, colour_ms=info.colour_ms, upload_ms=info.upload_ms)
 
     def recon(self, i):
         """Picture i of the last call as reconstructed before in-loop filtering: [y, cb, cr] (uint8; [y] for 4:0:0)."""
