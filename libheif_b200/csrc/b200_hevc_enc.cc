@@ -9,11 +9,14 @@
 // DST 4x4, transform skip, sign-data hiding, cu_qp_delta, chroma QP offsets, SAO band/edge with merges,
 // deblocking overrides, WPP entry points, multiple slices and dependent slice segments, 8..12 bit,
 // 4:2:0 and 4:0:0.  Syntax follows ITU-T H.265 7.3 / 9.3; the reconstruction loop follows 8.4 / 8.6.
-// The arithmetic coder, residual_coding(), intra mode signalling and the constant tables are the ones the GPU encoder
-// uses too (b200_hevc_enc_cabac.h); the parameter sets and slice header come from b200_hevc_enc_headers.h.
+// The arithmetic coder, residual_coding() and intra mode signalling (b200_hevc_enc_cabac.h) and the prediction, transform
+// and (de)quantisation arithmetic (b200_hevc_enc_recon.h) are the ones the GPU encoder uses too; transform skip,
+// cu_transquant_bypass, sign-data hiding, scaling lists and PCM are this encoder's alone.  The parameter sets and slice
+// header come from b200_hevc_enc_headers.h.
 #define B200_SYNTAX_HOST_ONLY 1   // this translation unit uses the shared encoder / syntax code on the host only
 #include "b200_hevc_enc_cabac.h"
 #include "b200_hevc_enc_headers.h"
+#include "b200_hevc_enc_recon.h"
 #include <algorithm>
 #include <vector>
 
@@ -21,17 +24,6 @@ namespace b200 {
 namespace enc {
 
 using namespace syn;
-
-// ------------------------------------------------------------------------------------------ tables
-static int16_t g_mat[4][32][32];       // [log2n-2][k][n] DCT matrices
-static bool g_tables_ready = false;
-
-static void init_tables() {
-  if (g_tables_ready) return;
-  for (int l = 2; l <= 5; l++)
-    for (int k = 0; k < (1 << l); k++) for (int x = 0; x < (1 << l); x++) g_mat[l - 2][k][x] = (int16_t)dct_coef(l, k, x);
-  g_tables_ready = true;
-}
 
 // ------------------------------------------------------------------------------------------ NAL framing
 void append_nal(std::vector<uint8_t>& out, int type, const std::vector<uint8_t>& rbsp) {
@@ -239,7 +231,6 @@ struct SaoParams { int type[3], band_pos[3], eo_class[3], abs[3][4], sign[3][4];
 class Encoder {
  public:
   Encoder(const b200_hevc_enc_params& p, const uint16_t* const src[3], const int stride[3]) : P(p) {
-    init_tables();
     W = (p.width + 7) & ~7; H = (p.height + 7) & ~7;       // multiples of MinCbSizeY (8); conformance window crops
     cfmt = p.chroma_format_idc; chroma = cfmt ? 1 : 0;
     sx = (cfmt == 1 || cfmt == 2) ? 1 : 0; sy = cfmt == 1 ? 1 : 0;       // SubWidthC = 1 << sx, SubHeightC = 1 << sy (Table 6-1)
@@ -474,108 +465,33 @@ class Encoder {
   void predict(int c, int x0, int y0, int log2n, int mode, uint16_t* dst /* n*n */) const {
     const int n = 1 << log2n, shx = c ? sx : 0, shy = c ? sy : 0, st = stride_of(c);
     const uint16_t* pl = rec[c].data();
-    int refbuf[129], fbuf[129]; uint8_t av[129];
-    bool any = false;
+    int16_t r[129], f[129];
     for (int i = 0; i <= 4 * n; i++) {
       int px, py;
       if (i < 2 * n) { px = x0 - 1; py = y0 + 2 * n - 1 - i; } else if (i == 2 * n) { px = x0 - 1; py = y0 - 1; } else { px = x0 + (i - 2 * n - 1); py = y0 - 1; }
-      av[i] = avail(px << shx, py << shy);
-      if (av[i]) { refbuf[i] = pl[(size_t)py * st + px]; any = true; }
+      r[i] = avail(px << shx, py << shy) ? (int16_t)pl[(size_t)py * st + px] : (int16_t)-1;
     }
-    if (!any) for (int i = 0; i <= 4 * n; i++) refbuf[i] = 1 << (bd - 1);
-    else {
-      int first = 0; while (!av[first]) first++;
-      for (int i = 0; i < first; i++) refbuf[i] = refbuf[first];
-      for (int i = first + 1; i <= 4 * n; i++) if (!av[i]) refbuf[i] = refbuf[i - 1];
-    }
-    int* ref = refbuf;
-    if ((c == 0 || cfmt == 3) && mode != 1 && n != 4) {            // 8.4.4.2.3: filtering of the neighbours for luma, and for chroma in 4:4:4
-      int dist = std::min(std::abs(mode - 26), std::abs(mode - 10));
-      int thr = n == 8 ? 7 : (n == 16 ? 1 : 0);
-      if (dist > thr) {
-        int corner = ref[2 * n], bl = ref[0], tr = ref[4 * n];
-        if (P.strong_intra_smoothing && c == 0 && n == 32 && std::abs(corner + tr - 2 * ref[3 * n]) < (1 << (bd - 5)) && std::abs(corner + bl - 2 * ref[n]) < (1 << (bd - 5))) {
-          fbuf[2 * n] = corner; fbuf[0] = bl; fbuf[4 * n] = tr;
-          for (int y = 0; y < 63; y++) fbuf[2 * n - 1 - y] = ((63 - y) * corner + (y + 1) * bl + 32) >> 6;
-          for (int x = 0; x < 63; x++) fbuf[2 * n + 1 + x] = ((63 - x) * corner + (x + 1) * tr + 32) >> 6;
-        } else {
-          fbuf[0] = ref[0]; fbuf[4 * n] = ref[4 * n];
-          for (int i = 1; i < 4 * n; i++) fbuf[i] = (ref[i - 1] + 2 * ref[i] + ref[i + 1] + 2) >> 2;
-        }
-        ref = fbuf;
-      }
-    }
-    auto LEFT = [&](int y) { return ref[2 * n - 1 - y]; };
-    auto TOP = [&](int x) { return ref[2 * n + 1 + x]; };
-    const int maxv = (1 << bd) - 1;
-    if (mode == 0) {
-      for (int y = 0; y < n; y++) for (int x = 0; x < n; x++)
-        dst[y * n + x] = (uint16_t)(((n - 1 - x) * LEFT(y) + (x + 1) * TOP(n) + (n - 1 - y) * TOP(x) + (y + 1) * LEFT(n) + n) >> (log2n + 1));
-    } else if (mode == 1) {
-      int sum = n; for (int i = 0; i < n; i++) sum += LEFT(i) + TOP(i);
-      int dc = sum >> (log2n + 1);
-      for (int i = 0; i < n * n; i++) dst[i] = (uint16_t)dc;
-      if (c == 0 && n < 32) {
-        dst[0] = (uint16_t)((LEFT(0) + 2 * dc + TOP(0) + 2) >> 2);
-        for (int x = 1; x < n; x++) dst[x] = (uint16_t)((TOP(x) + 3 * dc + 2) >> 2);
-        for (int y = 1; y < n; y++) dst[y * n] = (uint16_t)((LEFT(y) + 3 * dc + 2) >> 2);
-      }
-    } else {
-      int ang = B200_T(kAngle)[mode], ia = B200_T(kInvAngle)[mode];
-      int rbuf[98]; int* r = rbuf + 32;
-      if (mode >= 18) {
-        for (int x = 0; x <= n; x++) r[x] = TOP(x - 1);
-        if (ang < 0) { int last = (n * ang) >> 5; if (last < -1) for (int x = last; x <= -1; x++) r[x] = LEFT(-1 + ((x * ia + 128) >> 8)); }
-        else for (int x = n + 1; x <= 2 * n; x++) r[x] = TOP(x - 1);
-        for (int y = 0; y < n; y++) {
-          int idx = ((y + 1) * ang) >> 5, f = ((y + 1) * ang) & 31;
-          for (int x = 0; x < n; x++) dst[y * n + x] = (uint16_t)(f ? ((32 - f) * r[x + idx + 1] + f * r[x + idx + 2] + 16) >> 5 : r[x + idx + 1]);
-        }
-        if (mode == 26 && c == 0 && n < 32) for (int y = 0; y < n; y++) dst[y * n] = (uint16_t)clip3(0, maxv, TOP(0) + ((LEFT(y) - LEFT(-1)) >> 1));
-      } else {
-        for (int x = 0; x <= n; x++) r[x] = LEFT(x - 1);
-        if (ang < 0) { int last = (n * ang) >> 5; if (last < -1) for (int x = last; x <= -1; x++) r[x] = TOP(-1 + ((x * ia + 128) >> 8)); }
-        else for (int x = n + 1; x <= 2 * n; x++) r[x] = LEFT(x - 1);
-        for (int x = 0; x < n; x++) {
-          int idx = ((x + 1) * ang) >> 5, f = ((x + 1) * ang) & 31;
-          for (int y = 0; y < n; y++) dst[y * n + x] = (uint16_t)(f ? ((32 - f) * r[y + idx + 1] + f * r[y + idx + 2] + 16) >> 5 : r[y + idx + 1]);
-        }
-        if (mode == 10 && c == 0 && n < 32) for (int x = 0; x < n; x++) dst[x] = (uint16_t)clip3(0, maxv, LEFT(0) + ((TOP(x) - TOP(-1)) >> 1));
-      }
-    }
+    substitute_refs(r, n, bd);
+    const bool filt = refs_filtered(c == 0 || cfmt == 3, mode, log2n);
+    if (filt) filter_refs(r, f, log2n, P.strong_intra_smoothing && c == 0, bd);
+    const int dc = dc_value(r, log2n), maxv = (1 << bd) - 1;
+    for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) dst[y * n + x] = (uint16_t)pred_sample(filt ? f : r, dc, log2n, mode, x, y, c == 0, maxv);
   }
 
   // ---------------------------------------------------------------------------- transforms
   void forward(const int* res, int* coef, int log2n, bool dst4, bool tskip) const {
-    int n = 1 << log2n;
+    const int n = 1 << log2n;
     if (tskip) { int s = 15 - bd - log2n; for (int i = 0; i < n * n; i++) coef[i] = res[i] << s; return; }
     int tmp[1024];
-    int s1 = log2n + bd - 9, s2 = log2n + 6;
-    for (int k = 0; k < n; k++) for (int x = 0; x < n; x++) {        // columns: tmp[k][x] = sum_y M[k][y] res[y][x]
-      long e = 0;
-      for (int y = 0; y < n; y++) e += (dst4 ? B200_T(kDst4)[k][y] : g_mat[log2n - 2][k][y]) * res[y * n + x];
-      tmp[k * n + x] = (int)((e + (s1 > 0 ? (1 << (s1 - 1)) : 0)) >> s1);
-    }
-    for (int k = 0; k < n; k++) for (int y = 0; y < n; y++) {        // rows
-      long e = 0;
-      for (int x = 0; x < n; x++) e += (dst4 ? B200_T(kDst4)[k][x] : g_mat[log2n - 2][k][x]) * tmp[y * n + x];
-      coef[y * n + k] = (int)((e + (1 << (s2 - 1))) >> s2);
-    }
+    for (int k = 0; k < n; k++) for (int x = 0; x < n; x++) tmp[k * n + x] = fwd_col(res, dst4, log2n, k, x, bd);
+    for (int y = 0; y < n; y++) for (int k = 0; k < n; k++) coef[y * n + k] = fwd_row(tmp, dst4, log2n, y, k);
   }
-  void inverse(const int16_t* d, int* res, int log2n, bool dst4, bool tskip) const {     // 8.6.4.2
-    int n = 1 << log2n, bs = 20 - bd;
-    if (tskip) { for (int i = 0; i < n * n; i++) res[i] = (((int)d[i] << 7) + (1 << (bs - 1))) >> bs; return; }
+  void inverse(const int* d, int* res, int log2n, bool dst4, bool tskip) const {     // 8.6.4.2
+    const int n = 1 << log2n;
+    if (tskip) { const int bs = 20 - bd; for (int i = 0; i < n * n; i++) res[i] = ((d[i] << 7) + (1 << (bs - 1))) >> bs; return; }
     int tmp[1024];
-    for (int x = 0; x < n; x++) for (int y = 0; y < n; y++) {
-      int e = 0;
-      for (int k = 0; k < n; k++) e += d[k * n + x] * (dst4 ? B200_T(kDst4)[k][y] : g_mat[log2n - 2][k][y]);
-      tmp[y * n + x] = clip3(-32768, 32767, (e + 64) >> 7);
-    }
-    for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) {
-      int e = 0;
-      for (int k = 0; k < n; k++) e += tmp[y * n + k] * (dst4 ? B200_T(kDst4)[k][x] : g_mat[log2n - 2][k][x]);
-      res[y * n + x] = (e + (1 << (bs - 1))) >> bs;
-    }
+    for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) tmp[y * n + x] = inv_col(d, dst4, log2n, y, x);
+    for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) res[y * n + x] = inv_row(tmp, dst4, log2n, y, x, bd);
   }
 
   // ---------------------------------------------------------------------------- QP (8.6.1)
@@ -590,16 +506,9 @@ class Encoder {
   // ---------------------------------------------------------------------------- residual (7.3.8.11)
   // quantise + (optionally) sign-hide; returns cbf. levels are in raster order [y][x].
   bool quantise(const int* coef, int16_t* lev, int log2n, int qp, int scan) const {
-    int n = 1 << log2n, ts = 15 - bd - log2n, qbits = 14 + qp / 6 + ts;
-    long add = 171L << (qbits - 9);
+    const int n = 1 << log2n;
     bool any = false;
-    for (int i = 0; i < n * n; i++) {
-      long a = std::labs((long)coef[i]);
-      int l = (int)((a * B200_T(kQuantScale)[qp % 6] + add) >> qbits);
-      l = std::min(l, 32767);
-      lev[i] = (int16_t)(coef[i] < 0 ? -l : l);
-      any |= l != 0;
-    }
+    for (int i = 0; i < n * n; i++) { lev[i] = (int16_t)quant_level(coef[i], qp, log2n, bd); any |= lev[i] != 0; }
     if (any && P.sign_data_hiding && !cu_bypass) {
       const int l2sb = log2n - 2;
       const uint8_t *sbx = B200_T(kScanX)[l2sb][scan], *sby = B200_T(kScanY)[l2sb][scan], *px = B200_T(kScanX)[2][scan], *py = B200_T(kScanY)[2][scan];
@@ -650,8 +559,8 @@ class Encoder {
     // was); the caller re-runs with the predicted QP when neither holds.
     uint16_t* rp = rec[c].data();
     if (r.cbf) {
-      int16_t d[1024]; int bs = bd + log2n - 5, scale = B200_T(kLevelScale)[qp % 6] << (qp / 6);
-      for (int i = 0; i < n * n; i++) { long t = ((long)r.lev[i] * scaling_factor(c, log2n, i) * scale + (1L << (bs - 1))) >> bs; d[i] = (int16_t)(t < -32768 ? -32768 : (t > 32767 ? 32767 : t)); }
+      int d[1024];
+      for (int i = 0; i < n * n; i++) d[i] = dequant(r.lev[i], scaling_factor(c, log2n, i), qp, log2n, bd);
       inverse(d, res, log2n, dst4, r.tskip);
       int maxv = (1 << bd) - 1;
       for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) rp[(size_t)(y0 + y) * st + x0 + x] = (uint16_t)clip3(0, maxv, pred[y * n + x] + res[y * n + x]);

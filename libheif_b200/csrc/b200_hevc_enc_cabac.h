@@ -1,36 +1,18 @@
 // b200_hevc_enc_cabac.h -- the entropy-coding half both HEVC intra encoders share, as one piece of host + device source:
 // the arithmetic encoder of 9.3.4.5 over a caller's bit sink, context initialisation (9.3.2.2), the residual_coding()
-// writer (7.3.8.11), intra luma mode signalling (8.4.2 / 7.3.8.5) and the encoders' constant tables (transform matrices,
-// intra angles, quantisation scales, Table 8-10).  The host encoder (b200_hevc_enc.cc) compiles it for the host only
+// writer (7.3.8.11), intra luma mode signalling (8.4.2 / 7.3.8.5), the tables of the last-position prefix and the
+// chroma QP mapping (Table 8-10).  The host encoder (b200_hevc_enc.cc) compiles it for the host only
 // (B200_SYNTAX_HOST_ONLY), the GPU encoder (b200_hevc_gpu_enc.cu) for both sides.  The context, state-transition, scan
-// and sig-map tables are the decoder's (b200_hevc_syntax.h).
+// and sig-map tables are the decoder's (b200_hevc_syntax.h); the reconstruction half is b200_hevc_enc_recon.h.
 #pragma once
 #include "b200_hevc_syntax.h"
 
 namespace b200 {
 namespace enc {
 
-B200_TABLE(int8_t, kDctT, [32], {64, 90, 90, 90, 89, 88, 87, 85, 83, 82, 80, 78, 75, 73, 70, 67,
-                                 64, 61, 57, 54, 50, 46, 43, 38, 36, 31, 25, 22, 18, 13, 9, 4})
-B200_TABLE(int8_t, kDst4, [4][4], {{29, 55, 74, 84}, {74, 74, 0, -74}, {84, -29, -74, 55}, {55, -84, 74, -29}})
-B200_TABLE(int8_t, kAngle, [35], {0, 0, 32, 26, 21, 17, 13, 9, 5, 2, 0, -2, -5, -9, -13, -17, -21, -26, -32,
-                                  -26, -21, -17, -13, -9, -5, -2, 0, 2, 5, 9, 13, 17, 21, 26, 32})
-B200_TABLE(int16_t, kInvAngle, [35], {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, -4096, -1638, -910, -630, -482, -390, -315, -256,
-                                      -315, -390, -482, -630, -910, -1638, -4096, 0, 0, 0, 0, 0, 0, 0, 0, 0})
-B200_TABLE(int32_t, kQuantScale, [6], {26214, 23302, 20560, 18396, 16384, 14564})
-B200_TABLE(uint8_t, kLevelScale, [6], {40, 45, 51, 57, 64, 72})
 B200_TABLE(uint8_t, kQpcTab, [14], {29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37})        // Table 8-10, qPi 30..43
 B200_TABLE(uint8_t, kLastGroup, [32], {0, 1, 2, 3, 4, 4, 5, 5, 6, 6, 6, 6, 7, 7, 7, 7, 8, 8, 8, 8, 8, 8, 8, 8, 9, 9, 9, 9, 9, 9, 9, 9})
 B200_TABLE(uint8_t, kLastGroupMin, [10], {0, 1, 2, 3, 4, 6, 8, 12, 16, 24})
-
-// DCT matrix entry [k][x] of an n x n transform (8.6.4.2)
-B200_HD inline int dct_coef(int log2n, int k, int x) {
-  if (k == 0) return 64;
-  int j = ((k << (5 - log2n)) * (2 * x + 1)) & 127, sgn = 1;
-  if (j > 64) j = 128 - j;
-  if (j > 32) { j = 64 - j; sgn = -1; }
-  return sgn * B200_T(kDctT)[j];
-}
 
 // Qp'Cb / Qp'Cr (8.6.1): qPi = Clip3(-QpBdOffsetC, 57, QpY + the chroma offsets), mapped by Table 8-10 when
 // ChromaArrayType is 1 and capped at 51 otherwise, plus QpBdOffsetC

@@ -6,16 +6,17 @@
 //      forward DST 4x4 / DCT 4..32, uniform quantisation with the intra rounding offset 171/512, reconstruction with the
 //      inverse path of 8.6.  Writes the reconstruction (HBM plane: the neighbours of the next row), the luma modes per 4x4,
 //      the CU size / partition per 8x8 and the quantised levels (a coefficient plane: every TB's levels at its position).
-//      Rows trail the row above by two CTBs through per-row progress counters.
+//      Rows trail the row above by two CTBs through per-row progress counters.  The prediction, transform and
+//      (de)quantisation arithmetic is the host encoder's (b200_hevc_enc_recon.h), at bit depth 8.
 //   E2 (CABAC), one warp per WPP sub-stream (= CTB row): the syntax of 7.3.8 from E1's records, context hand-over after
 //      the 2nd CTB of the row above (9.3.2.2), end_of_slice_segment_flag per CTB and end_of_subset_one_bit + byte
-//      alignment per row, into a per-row buffer sized for the worst case.  The arithmetic coder, residual_coding(), the
-//      intra mode signalling and the constant tables are the host encoder's (b200_hevc_enc_cabac.h).
+//      alignment per row, into a per-row buffer sized for the worst case.  The arithmetic coder, residual_coding() and the
+//      intra mode signalling are the host encoder's (b200_hevc_enc_cabac.h).
 //   Framing (host): parameter sets and slice header (b200_hevc_enc_headers.h, shared with the host encoder), entry points
 //      over the escaped sub-stream sizes, emulation prevention, length prefixes.
 //
-// Prediction, transforms and dequantisation are written here rather than taken from the reconstruction kernel
-// (b200_hevc_recon.cu): its predict_tb reconstructs one TB of a known mode inside K1's per-lane padded tile, from a packed
+// Prediction, transforms and dequantisation are shared with the host encoder rather than taken from the reconstruction
+// kernel (b200_hevc_recon.cu): its predict_tb reconstructs one TB of a known mode inside K1's per-lane padded tile, from a packed
 // descriptor whose neighbour availability is precomputed as index intervals, and residual4_lane / residual_big consume sparse
 // CoefEntry lists.  The mode search needs the predicted sample of any of the 35 modes at any position as a pure function,
 // many modes per block without reconstructing, and dense residual blocks; both files are separate translation units built
@@ -24,6 +25,7 @@
 #include "b200_staging.h"
 #include "b200_hevc_enc_headers.h"
 #include "b200_hevc_enc_cabac.h"
+#include "b200_hevc_enc_recon.h"
 #include <algorithm>
 #include <chrono>
 #include <memory>
@@ -93,8 +95,6 @@ struct Ctx2 { const Args& a; int p; int lane; Work& w;
   }
 };
 
-__device__ inline int tmat(bool dst4, int log2n, int k, int x) { return dst4 ? enc::B200_T(kDst4)[k][x] : enc::dct_coef(log2n, k, x); }
-
 // 8.4.2: the three most probable modes of the PU at luma (x, y)
 __device__ inline void mpm_cand(const uint8_t* ipm, int w4, int log2ctb, int x, int y, int cand[3]) {
   int ca = 1, cb = 1;
@@ -116,69 +116,16 @@ __device__ void gather_refs(Ctx2& e, int c, int x0, int y0, int log2n) {
   }
   GE_SYNC();
   if (e.lane == 0) {
-    int16_t* r = w.ref[0];
-    int first = 0; while (first <= 4 * n && r[first] < 0) first++;
-    if (first > 4 * n) for (int i = 0; i <= 4 * n; i++) r[i] = 128;
-    else {
-      for (int i = 0; i < first; i++) r[i] = r[first];
-      for (int i = first + 1; i <= 4 * n; i++) if (r[i] < 0) r[i] = r[i - 1];
-    }
-    int16_t* f = w.ref[1];
-    if (c == 0 && n != 4) {
-      const int corner = r[2 * n], bl = r[0], tr = r[4 * n];
-      if (e.a.strong && n == 32 && abs(corner + tr - 2 * r[3 * n]) < 8 && abs(corner + bl - 2 * r[n]) < 8) {
-        f[2 * n] = (int16_t)corner; f[0] = (int16_t)bl; f[4 * n] = (int16_t)tr;
-        for (int y = 0; y < 63; y++) f[2 * n - 1 - y] = (int16_t)(((63 - y) * corner + (y + 1) * bl + 32) >> 6);
-        for (int x = 0; x < 63; x++) f[2 * n + 1 + x] = (int16_t)(((63 - x) * corner + (x + 1) * tr + 32) >> 6);
-      } else {
-        f[0] = r[0]; f[4 * n] = r[4 * n];
-        for (int i = 1; i < 4 * n; i++) f[i] = (int16_t)((r[i - 1] + 2 * r[i] + r[i + 1] + 2) >> 2);
-      }
-    }
-    int sum = n; for (int i = 0; i < n; i++) sum += r[2 * n - 1 - i] + r[2 * n + 1 + i];
-    w.dc = sum >> (log2n + 1);
+    enc::substitute_refs(w.ref[0], n, 8);
+    if (c == 0 && n != 4) enc::filter_refs(w.ref[0], w.ref[1], log2n, e.a.strong, 8);
+    w.dc = enc::dc_value(w.ref[0], log2n);
   }
   GE_SYNC();
 }
 
-// predicted sample (x, y) of mode `mode` (8.4.4.2.4 .. .6) from the neighbours gathered above
-__device__ inline int pred_px(const Work& w, int c, int log2n, int mode, int x, int y) {
-  const int n = 1 << log2n;
-  bool filt = false;
-  if (c == 0 && mode != 1 && n != 4) {
-    const int dist = min(abs(mode - 26), abs(mode - 10)), thr = n == 8 ? 7 : (n == 16 ? 1 : 0);
-    filt = dist > thr;
-  }
-  const int16_t* ref = w.ref[filt ? 1 : 0];
-#define LEFT(i) ((int)ref[2 * n - 1 - (i)])
-#define TOP(i) ((int)ref[2 * n + 1 + (i)])
-  if (mode == 0) return ((n - 1 - x) * LEFT(y) + (x + 1) * TOP(n) + (n - 1 - y) * TOP(x) + (y + 1) * LEFT(n) + n) >> (log2n + 1);
-  if (mode == 1) {
-    const int dc = w.dc;
-    if (c == 0 && n < 32) {
-      if (x == 0 && y == 0) return (LEFT(0) + 2 * dc + TOP(0) + 2) >> 2;
-      if (y == 0) return (TOP(x) + 3 * dc + 2) >> 2;
-      if (x == 0) return (LEFT(y) + 3 * dc + 2) >> 2;
-    }
-    return dc;
-  }
-  const int ang = enc::B200_T(kAngle)[mode], ia = enc::B200_T(kInvAngle)[mode];
-  if (mode >= 18) {
-    if (mode == 26 && c == 0 && n < 32 && x == 0) return clip3(0, 255, TOP(0) + ((LEFT(y) - LEFT(-1)) >> 1));
-    const int idx = ((y + 1) * ang) >> 5, f = ((y + 1) * ang) & 31, k1 = x + idx + 1, k2 = k1 + 1;
-    const int r1 = k1 >= 0 ? TOP(k1 - 1) : LEFT(-1 + ((k1 * ia + 128) >> 8));
-    if (!f) return r1;
-    const int r2 = k2 >= 0 ? TOP(k2 - 1) : LEFT(-1 + ((k2 * ia + 128) >> 8));
-    return ((32 - f) * r1 + f * r2 + 16) >> 5;
-  }
-  if (mode == 10 && c == 0 && n < 32 && y == 0) return clip3(0, 255, LEFT(0) + ((TOP(x) - TOP(-1)) >> 1));
-  const int idx = ((x + 1) * ang) >> 5, f = ((x + 1) * ang) & 31, k1 = y + idx + 1, k2 = k1 + 1;
-  const int r1 = k1 >= 0 ? LEFT(k1 - 1) : TOP(-1 + ((k1 * ia + 128) >> 8));
-  if (!f) return r1;
-  const int r2 = k2 >= 0 ? LEFT(k2 - 1) : TOP(-1 + ((k2 * ia + 128) >> 8));
-  return ((32 - f) * r1 + f * r2 + 16) >> 5;
-#undef LEFT
-#undef TOP
+// predicted sample (x, y) of mode `mode` from the neighbours gathered above
+__device__ inline int predicted(const Work& w, int c, int log2n, int mode, int x, int y) {
+  return enc::pred_sample(w.ref[enc::refs_filtered(c == 0, mode, log2n) ? 1 : 0], w.dc, log2n, mode, x, y, c == 0, 255);
 }
 
 __device__ inline int satd4(const int d[16]) {                   // 4x4 Hadamard
@@ -204,7 +151,7 @@ __device__ int search_mode(Ctx2& e, int x0, int y0, int log2n, long long* cost) 
   for (int it = e.lane; it < 35 * nsb; it += GE_LANES) {
     const int mode = it % 35, sb = it / 35, bx = (sb % (n >> 2)) << 2, by = (sb / (n >> 2)) << 2;
     int d[16];
-    for (int k = 0; k < 16; k++) d[k] = e.org(0, x0 + bx + (k & 3), y0 + by + (k >> 2)) - pred_px(w, 0, log2n, mode, bx + (k & 3), by + (k >> 2));
+    for (int k = 0; k < 16; k++) d[k] = e.org(0, x0 + bx + (k & 3), y0 + by + (k >> 2)) - predicted(w, 0, log2n, mode, bx + (k & 3), by + (k >> 2));
     GE_ATOMIC_ADD(&w.satd[mode], satd4(d));
   }
   GE_SYNC();
@@ -231,7 +178,7 @@ __device__ int code_tb(Ctx2& e, int c, int x0, int y0, int log2n, int mode, bool
   gather_refs(e, c, x0, y0, log2n);
   if (e.lane == 0) { w.any = 0; w.acc = 0; }
   for (int i = e.lane; i < nn; i += GE_LANES) {
-    const int x = i & (n - 1), y = i >> log2n, pv = pred_px(w, c, log2n, mode, x, y);
+    const int x = i & (n - 1), y = i >> log2n, pv = predicted(w, c, log2n, mode, x, y);
     w.pred[i] = (uint8_t)pv; w.res[i] = e.org(c, x0 + x, y0 + y) - pv;
   }
   GE_SYNC();
@@ -242,45 +189,25 @@ __device__ int code_tb(Ctx2& e, int c, int x0, int y0, int log2n, int mode, bool
       GE_ATOMIC_ADD(&w.acc, satd4(d));
     }
   }
-  // forward transform: columns then rows (shifts log2n - 1 and log2n + 6 at 8 bit)
-  const int s1 = log2n - 1, s2 = log2n + 6;
-  for (int i = e.lane; i < nn; i += GE_LANES) {
-    const int k = i >> log2n, x = i & (n - 1);
-    int s = 0; for (int y = 0; y < n; y++) s += tmat(dst4, log2n, k, y) * w.res[y * n + x];
-    w.tmp[i] = (s + (1 << (s1 - 1))) >> s1;
-  }
+  // forward transform: columns, then rows and quantisation
+  for (int i = e.lane; i < nn; i += GE_LANES) w.tmp[i] = enc::fwd_col(w.res, dst4, log2n, i >> log2n, i & (n - 1), 8);
   GE_SYNC();
-  const int qbits = 14 + qp / 6 + (7 - log2n), qs = enc::B200_T(kQuantScale)[qp % 6];
-  const long long add = 171LL << (qbits - 9);
   for (int i = e.lane; i < nn; i += GE_LANES) {
-    const int y = i >> log2n, k = i & (n - 1);
-    int s = 0; for (int x = 0; x < n; x++) s += tmat(dst4, log2n, k, x) * w.tmp[y * n + x];
-    const int cf = (s + (1 << (s2 - 1))) >> s2;
-    int l = (int)(((long long)abs(cf) * qs + add) >> qbits);
-    l = min(l, 32767);
-    w.lev[i] = (int16_t)(cf < 0 ? -l : l);
+    const int l = enc::quant_level(enc::fwd_row(w.tmp, dst4, log2n, i >> log2n, i & (n - 1)), qp, log2n, 8);
+    w.lev[i] = (int16_t)l;
     if (l) w.any = 1;
   }
   GE_SYNC();
   if (final) { int16_t* cp = e.cplane(c); for (int i = e.lane; i < nn; i += GE_LANES) cp[(size_t)(y0 + (i >> log2n)) * st + x0 + (i & (n - 1))] = w.lev[i]; }
   uint8_t* rp = e.plane(c);
   if (w.any) {
-    const int bs = log2n + 3, scale = enc::B200_T(kLevelScale)[qp % 6] << (qp / 6);
-    for (int i = e.lane; i < nn; i += GE_LANES) {
-      const long long t = ((long long)w.lev[i] * 16 * scale + (1LL << (bs - 1))) >> bs;
-      w.coef[i] = (int)(t < -32768 ? -32768 : (t > 32767 ? 32767 : t));
-    }
+    for (int i = e.lane; i < nn; i += GE_LANES) w.coef[i] = enc::dequant(w.lev[i], 16, qp, log2n, 8);
     GE_SYNC();
-    for (int i = e.lane; i < nn; i += GE_LANES) {       // tmp[y][x] = sum_k d[k][x] M[k][y]
-      const int y = i >> log2n, x = i & (n - 1);
-      int s = 0; for (int k = 0; k < n; k++) s += w.coef[k * n + x] * tmat(dst4, log2n, k, y);
-      w.tmp[i] = clip3(-32768, 32767, (s + 64) >> 7);
-    }
+    for (int i = e.lane; i < nn; i += GE_LANES) w.tmp[i] = enc::inv_col(w.coef, dst4, log2n, i >> log2n, i & (n - 1));
     GE_SYNC();
     for (int i = e.lane; i < nn; i += GE_LANES) {
       const int y = i >> log2n, x = i & (n - 1);
-      int s = 0; for (int k = 0; k < n; k++) s += w.tmp[y * n + k] * tmat(dst4, log2n, k, x);
-      rp[(size_t)(y0 + y) * st + x0 + x] = (uint8_t)clip3(0, 255, w.pred[i] + ((s + (1 << 11)) >> 12));
+      rp[(size_t)(y0 + y) * st + x0 + x] = (uint8_t)clip3(0, 255, w.pred[i] + enc::inv_row(w.tmp, dst4, log2n, y, x, 8));
     }
   } else {
     for (int i = e.lane; i < nn; i += GE_LANES) rp[(size_t)(y0 + (i >> log2n)) * st + x0 + (i & (n - 1))] = w.pred[i];
