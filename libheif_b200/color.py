@@ -63,15 +63,72 @@ class YCbCrImage:
     _keep: list = field(default_factory=list, repr=False)
 
 
-def _fill_planes(img: YCbCrImage, ptr, stride):
+class _Host:
+    """numpy arrays, converted by the _host entry points (which stage them through the GPU inside the call)."""
+    u8, u16, rgb16 = np.uint8, np.uint16, np.uint16     # rgb16: convert_colorspace_host's 16-bit planar RGB
+
+    ptr = staticmethod(lambda a: a.ctypes.data)
+    stride = staticmethod(lambda a: a.strides[0])
+
+    @staticmethod
+    def is16(a):
+        if a.dtype not in (np.uint8, np.uint16):
+            raise ValueError("uint8 / uint16 arrays only")
+        return a.dtype == np.uint16
+
+    @staticmethod
+    def packed(a):
+        return a.strides[-1] == a.itemsize and (a.ndim == 2 or a.strides[1] == a.shape[2] * a.itemsize)
+
+    @staticmethod
+    def empty(shape, dtype):
+        return np.empty(shape, dtype)
+
+    @staticmethod
+    def call(name, *args, pipeline=True):
+        """name + "_host"(*args[, &pipeline]); returns the pipeline mask"""
+        pipe = C.c_int(0)
+        _lib.check(getattr(_lib.lib(), name + "_host")(*args, *((C.byref(pipe),) if pipeline else ())))
+        return pipe.value
+
+
+class _Cuda:
+    """CUDA tensors on `device`, converted by the _device entry points on `stream` (default: the device's current stream)."""
+
+    def __init__(self, device, stream=None):
+        import torch
+        self.torch, self.device, self.stream = torch, device, stream
+        self.u8, self.u16, self.rgb16 = torch.uint8, torch.uint16, torch.int16   # rgb16: convert_colorspace's 16-bit planar RGB
+
+    ptr = staticmethod(lambda t: t.data_ptr())
+    stride = staticmethod(lambda t: t.stride(0) * t.element_size())
+    is16 = staticmethod(lambda t: t.element_size() == 2)
+    packed = staticmethod(lambda t: t.stride(-1) == 1 and (t.dim() == 2 or t.stride(1) == t.shape[2]))
+
+    def empty(self, shape, dtype):
+        return self.torch.empty(shape, dtype=dtype, device=self.device)
+
+    def call(self, name, *args, pipeline=True):
+        """name + "_device"(*args, stream[, &pipeline]); returns the pipeline mask"""
+        s = self.stream if self.stream is not None else self.torch.cuda.current_stream(self.device)
+        pipe = C.c_int(0)
+        with self.torch.cuda.device(self.device):
+            _lib.check(getattr(_lib.lib(), name + "_device")(*args, C.c_void_p(s.cuda_stream), *((C.byref(pipe),) if pipeline else ())))
+        return pipe.value
+
+
+_HOST = _Host()
+
+
+def _fill_planes(img: YCbCrImage, mem):
     p = _lib.Planes()
     h, w = img.y.shape
-    p.y = ptr(img.y); p.y_stride = stride(img.y)
+    p.y = mem.ptr(img.y); p.y_stride = mem.stride(img.y)
     if img.chroma != CHROMA_MONO:
-        p.cb = ptr(img.cb); p.cr = ptr(img.cr); p.c_stride = stride(img.cb)
-        assert stride(img.cb) == stride(img.cr)
+        p.cb = mem.ptr(img.cb); p.cr = mem.ptr(img.cr); p.c_stride = mem.stride(img.cb)
+        assert mem.stride(img.cb) == mem.stride(img.cr)
     if img.alpha is not None:
-        p.alpha = ptr(img.alpha); p.alpha_stride = stride(img.alpha)
+        p.alpha = mem.ptr(img.alpha); p.alpha_stride = mem.stride(img.alpha)
     p.width, p.height, p.chroma, p.bit_depth = w, h, img.chroma, img.bit_depth
     p.colour_primaries, p.transfer_characteristics = img.colour_primaries, img.transfer_characteristics
     p.matrix_coefficients, p.full_range = img.matrix_coefficients, int(bool(img.full_range))
@@ -79,57 +136,38 @@ def _fill_planes(img: YCbCrImage, ptr, stride):
 
 
 def _out_shape(out_chroma, w, h, bit_depth):
+    """(shape, whether the samples are 16 bit) of the conversion's output"""
     if out_chroma == CHROMA_444:
-        return (3, h, w), (np.uint16 if bit_depth > 8 else np.uint8)
-    return (h, w * _BYTES_PER_PIXEL[out_chroma]), np.uint8
+        return (3, h, w), bit_depth > 8
+    return (h, w * _BYTES_PER_PIXEL[out_chroma]), False
+
+
+def _convert(mem, img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry], out=None, bilinear: bool = False):
+    h, w = img.y.shape
+    geom = geometry or Geometry(w, h)
+    if out is None:
+        shape, wide = _out_shape(out_chroma, *geom.size, img.bit_depth)
+        out = mem.empty(shape, mem.rgb16 if wide else mem.u8)
+    if out_chroma == CHROMA_444:
+        o, og, ob = mem.ptr(out[0]), mem.ptr(out[1]), mem.ptr(out[2])
+    else:
+        o, og, ob = mem.ptr(out), None, None
+    opt = _lib.ColorOptions(out_chroma, 0, 1 if bilinear else 0)
+    pipe = mem.call("b200_color_convert", C.byref(_fill_planes(img, mem)), C.byref(geom.g), C.byref(opt), o, og, ob,
+                    mem.stride(out[0] if out_chroma == CHROMA_444 else out))
+    return out, pipe
 
 
 def convert_colorspace(img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry] = None, out=None, stream=None, bilinear: bool = False):
     """Device -> device. `img` planes are CUDA torch tensors (uint8, or int16/uint16 for >8 bit).
 
     Returns a CUDA uint8 tensor [H, W*bytes_per_pixel] (interleaved) or [3, H, W] (planar RGB 4:4:4)."""
-    import torch
-    l = _lib.lib()
-    h, w = img.y.shape
-    geom = geometry or Geometry(w, h)
-    ow, oh = geom.size
-    shape, dt = _out_shape(out_chroma, ow, oh, img.bit_depth)
-    tdt = torch.uint8 if dt == np.uint8 else torch.int16
-    if out is None:
-        out = torch.empty(shape, dtype=tdt, device=img.y.device)
-    planes = _fill_planes(img, lambda t: t.data_ptr(), lambda t: t.stride(0) * t.element_size())
-    opt = _lib.ColorOptions(out_chroma, 0, 1 if bilinear else 0)
-    s = stream if stream is not None else torch.cuda.current_stream(img.y.device)
-    pipe = C.c_int(0)
-    if out_chroma == CHROMA_444:
-        o, og, ob = out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr()
-        ostride = out.stride(1) * out.element_size()
-    else:
-        o, og, ob = out.data_ptr(), None, None
-        ostride = out.stride(0) * out.element_size()
-    with torch.cuda.device(img.y.device):
-        _lib.check(l.b200_color_convert_device(C.byref(planes), C.byref(geom.g), C.byref(opt), o, og, ob, ostride,
-                                               C.c_void_p(s.cuda_stream), C.byref(pipe)))
-    return out
+    return _convert(_Cuda(img.y.device, stream), img, out_chroma, geometry, out, bilinear)[0]
 
 
 def convert_colorspace_host(img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry] = None):
     """Host -> host through the C ABI (H2D + kernel + D2H inside the call). Planes are numpy arrays."""
-    l = _lib.lib()
-    h, w = img.y.shape
-    geom = geometry or Geometry(w, h)
-    ow, oh = geom.size
-    shape, dt = _out_shape(out_chroma, ow, oh, img.bit_depth)
-    out = np.empty(shape, dtype=dt)
-    planes = _fill_planes(img, lambda a: a.ctypes.data, lambda a: a.strides[0])
-    opt = _lib.ColorOptions(out_chroma, 0, 0)
-    pipe = C.c_int(0)
-    if out_chroma == CHROMA_444:
-        o, og, ob, ostride = out[0].ctypes.data, out[1].ctypes.data, out[2].ctypes.data, out.strides[1]
-    else:
-        o, og, ob, ostride = out.ctypes.data, None, None, out.strides[0]
-    _lib.check(l.b200_color_convert_host(C.byref(planes), C.byref(geom.g), C.byref(opt), o, og, ob, ostride, C.byref(pipe)))
-    return out, pipe.value
+    return _convert(_HOST, img, out_chroma, geometry)
 
 
 def _ycc_out_planes(w, h, out_chroma, want_alpha, alloc):
@@ -142,40 +180,31 @@ def _ycc_out_planes(w, h, out_chroma, want_alpha, alloc):
     return y, cb, cr, a
 
 
+def _rgb_to_ycbcr(mem, rgb, out_chroma, matrix_coefficients, colour_primaries, full_range, want_alpha) -> YCbCrImage:
+    assert rgb.dtype == mem.u8 and rgb.ndim == 3 and rgb.shape[2] in (3, 4) and mem.packed(rgb)
+    h, w, bpp = rgb.shape
+    if want_alpha is None:
+        want_alpha = bpp == 4
+    y, cb, cr, a = _ycc_out_planes(w, h, out_chroma, want_alpha, lambda s: mem.empty(s, mem.u8))
+    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=8, colour_primaries=colour_primaries,
+                     matrix_coefficients=matrix_coefficients, full_range=full_range)
+    mem.call("b200_rgb_to_ycbcr", C.c_void_p(mem.ptr(rgb)), C.c_size_t(mem.stride(rgb)), int(bpp == 4), C.byref(_fill_planes(img, mem)),
+             pipeline=False)
+    return img
+
+
 def rgb_to_ycbcr(rgb, out_chroma: int = CHROMA_420, matrix_coefficients: int = 6, colour_primaries: int = 1, full_range: bool = True,
                  want_alpha: Optional[bool] = None, stream=None) -> YCbCrImage:
     """Encoder-side direction, device -> device: interleaved RGB / RGBA (CUDA uint8 tensor [H, W, 3 or 4]) -> YCbCrImage of
     CUDA uint8 planes, as Op_RGB24_32_to_YCbCr does (libheif/color-conversion/rgb2yuv.cc:575-808).
     want_alpha: None = an alpha plane iff the source has one (what the reference's planner targets for has_alpha)."""
-    import torch
-    assert rgb.dtype == torch.uint8 and rgb.dim() == 3 and rgb.shape[2] in (3, 4) and rgb.stride(2) == 1 and rgb.stride(1) == rgb.shape[2]
-    h, w, bpp = rgb.shape
-    if want_alpha is None:
-        want_alpha = bpp == 4
-    y, cb, cr, a = _ycc_out_planes(w, h, out_chroma, want_alpha, lambda s: torch.empty(s, dtype=torch.uint8, device=rgb.device))
-    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=8, colour_primaries=colour_primaries,
-                     matrix_coefficients=matrix_coefficients, full_range=full_range)
-    planes = _fill_planes(img, lambda t: t.data_ptr(), lambda t: t.stride(0) * t.element_size())
-    s = stream if stream is not None else torch.cuda.current_stream(rgb.device)
-    with torch.cuda.device(rgb.device):
-        _lib.check(_lib.lib().b200_rgb_to_ycbcr_device(C.c_void_p(rgb.data_ptr()), C.c_size_t(rgb.stride(0)), int(bpp == 4), C.byref(planes),
-                                                       C.c_void_p(s.cuda_stream)))
-    return img
+    return _rgb_to_ycbcr(_Cuda(rgb.device, stream), rgb, out_chroma, matrix_coefficients, colour_primaries, full_range, want_alpha)
 
 
 def rgb_to_ycbcr_host(rgb: np.ndarray, out_chroma: int = CHROMA_420, matrix_coefficients: int = 6, colour_primaries: int = 1,
                       full_range: bool = True, want_alpha: Optional[bool] = None) -> YCbCrImage:
     """Host -> host through the C ABI (H2D + kernel + D2H inside the call). rgb: uint8 [H, W, 3 or 4], rows may be strided."""
-    assert rgb.dtype == np.uint8 and rgb.ndim == 3 and rgb.shape[2] in (3, 4) and rgb.strides[2] == 1 and rgb.strides[1] == rgb.shape[2]
-    h, w, bpp = rgb.shape
-    if want_alpha is None:
-        want_alpha = bpp == 4
-    y, cb, cr, a = _ycc_out_planes(w, h, out_chroma, want_alpha, lambda s: np.empty(s, np.uint8))
-    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=8, colour_primaries=colour_primaries,
-                     matrix_coefficients=matrix_coefficients, full_range=full_range)
-    planes = _fill_planes(img, lambda x: x.ctypes.data, lambda x: x.strides[0])
-    _lib.check(_lib.lib().b200_rgb_to_ycbcr_host(C.c_void_p(rgb.ctypes.data), C.c_size_t(rgb.strides[0]), int(bpp == 4), C.byref(planes)))
-    return img
+    return _rgb_to_ycbcr(_HOST, rgb, out_chroma, matrix_coefficients, colour_primaries, full_range, want_alpha)
 
 
 # ---- every RGB layout heif_context_encode_image accepts (b200_rgb_to_ycbcr_ex_*) ----------------------------------------
@@ -238,27 +267,30 @@ def _ycc_target(img_planes, w, h, out_chroma, bit_depth, mc, cp, full):
     return p
 
 
-def _np_is16(a):
-    if a.dtype not in (np.uint8, np.uint16):
-        raise ValueError("uint8 / uint16 arrays only")
-    return a.dtype == np.uint16
-
-
-def _np_packed(a):
-    return a.strides[-1] == a.itemsize and (a.ndim == 2 or a.strides[1] == a.shape[2] * a.itemsize)
-
-
 def rgb_to_ycbcr_plan(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[int] = None, endianness: Optional[str] = None,
                       matrix_coefficients: int = 6, colour_primaries: int = 1, full_range: bool = True, chroma_downsampling: int = 2,
                       only_use_preferred: bool = False, alpha_bit_depth: Optional[int] = None) -> int:
     """Host only: the B200_YCC_PIPE_* mask of the reference chain for this input (numpy arrays, arguments as for
     rgb_to_ycbcr_ex; no pixel is read); raises B200Error (code -2) where the conversion is refused."""
-    d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda a: a.ctypes.data, lambda a: a.strides[0], _np_is16, _np_packed)
+    d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, _HOST.ptr, _HOST.stride, _HOST.is16, _HOST.packed)
     t = _ycc_target(None, d.width, d.height, out_chroma, d.bit_depth, matrix_coefficients, colour_primaries, full_range)
     opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
     pipe = C.c_int(0)
     _lib.check(_lib.lib().b200_rgb_to_ycbcr_plan(C.byref(d), C.byref(t), C.byref(opt), C.byref(pipe)))
     return pipe.value
+
+
+def _rgb_to_ycbcr_ex(mem, rgb, out_chroma, bit_depth, endianness, matrix_coefficients, colour_primaries, full_range, chroma_downsampling,
+                     only_use_preferred, alpha_bit_depth):
+    d, has_alpha = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, mem.ptr, mem.stride, mem.is16, mem.packed)
+    dt = mem.u16 if d.bit_depth > 8 else mem.u8
+    y, cb, cr, a = _ycc_out_planes(d.width, d.height, out_chroma, has_alpha, lambda s: mem.empty(s, dt))
+    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=d.bit_depth, colour_primaries=colour_primaries,
+                     matrix_coefficients=matrix_coefficients, full_range=full_range)
+    t = _ycc_target((y, cb, cr, a, mem.ptr, mem.stride), d.width, d.height, out_chroma, d.bit_depth, matrix_coefficients,
+                    colour_primaries, full_range)
+    opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
+    return img, mem.call("b200_rgb_to_ycbcr_ex", C.byref(d), C.byref(t), C.byref(opt))
 
 
 def rgb_to_ycbcr_ex(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[int] = None, endianness: Optional[str] = None,
@@ -276,22 +308,8 @@ def rgb_to_ycbcr_ex(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[int] 
     for t in (rgb if isinstance(rgb, (tuple, list)) else (rgb,)):
         if t.device != first.device or t.device.type != "cuda" or t.dtype not in (torch.uint8, torch.uint16):
             raise ValueError("rgb_to_ycbcr_ex: uint8 / uint16 CUDA tensors on one device")
-    is16 = lambda t: t.element_size() == 2   # noqa: E731
-    packed = lambda t: t.stride(-1) == 1 and (t.dim() == 2 or t.stride(1) == t.shape[2])   # noqa: E731
-    d, has_alpha = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda t: t.data_ptr(),
-                              lambda t: t.stride(0) * t.element_size(), is16, packed)
-    tdt = torch.uint16 if d.bit_depth > 8 else torch.uint8
-    y, cb, cr, a = _ycc_out_planes(d.width, d.height, out_chroma, has_alpha, lambda s: torch.empty(s, dtype=tdt, device=first.device))
-    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=d.bit_depth, colour_primaries=colour_primaries,
-                     matrix_coefficients=matrix_coefficients, full_range=full_range)
-    t = _ycc_target((y, cb, cr, a, lambda x: x.data_ptr(), lambda x: x.stride(0) * x.element_size()), d.width, d.height, out_chroma,
-                    d.bit_depth, matrix_coefficients, colour_primaries, full_range)
-    opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
-    pipe = C.c_int(0)
-    s = stream if stream is not None else torch.cuda.current_stream(first.device)
-    with torch.cuda.device(first.device):
-        _lib.check(_lib.lib().b200_rgb_to_ycbcr_ex_device(C.byref(d), C.byref(t), C.byref(opt), C.c_void_p(s.cuda_stream), C.byref(pipe)))
-    return img, pipe.value
+    return _rgb_to_ycbcr_ex(_Cuda(first.device, stream), rgb, out_chroma, bit_depth, endianness, matrix_coefficients, colour_primaries,
+                            full_range, chroma_downsampling, only_use_preferred, alpha_bit_depth)
 
 
 def rgb_to_ycbcr_ex_host(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[int] = None, endianness: Optional[str] = None,
@@ -299,14 +317,5 @@ def rgb_to_ycbcr_ex_host(rgb, out_chroma: int = CHROMA_420, bit_depth: Optional[
                          only_use_preferred: bool = False, alpha_bit_depth: Optional[int] = None):
     """Host -> host form of rgb_to_ycbcr_ex (b200_rgb_to_ycbcr_ex_host: H2D + kernel + D2H inside the call); numpy input,
     rows may be strided."""
-    d, has_alpha = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda a: a.ctypes.data, lambda a: a.strides[0], _np_is16, _np_packed)
-    dt = np.uint16 if d.bit_depth > 8 else np.uint8
-    y, cb, cr, a = _ycc_out_planes(d.width, d.height, out_chroma, has_alpha, lambda s: np.empty(s, dt))
-    img = YCbCrImage(y, cb, cr, a, chroma=out_chroma, bit_depth=d.bit_depth, colour_primaries=colour_primaries,
-                     matrix_coefficients=matrix_coefficients, full_range=full_range)
-    t = _ycc_target((y, cb, cr, a, lambda x: x.ctypes.data, lambda x: x.strides[0]), d.width, d.height, out_chroma, d.bit_depth,
-                    matrix_coefficients, colour_primaries, full_range)
-    opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
-    pipe = C.c_int(0)
-    _lib.check(_lib.lib().b200_rgb_to_ycbcr_ex_host(C.byref(d), C.byref(t), C.byref(opt), C.byref(pipe)))
-    return img, pipe.value
+    return _rgb_to_ycbcr_ex(_HOST, rgb, out_chroma, bit_depth, endianness, matrix_coefficients, colour_primaries, full_range,
+                            chroma_downsampling, only_use_preferred, alpha_bit_depth)

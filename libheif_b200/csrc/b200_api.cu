@@ -2,6 +2,7 @@
 #include "b200_internal.h"
 #include "b200_staging.h"
 #include <algorithm>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <unistd.h>
@@ -34,10 +35,7 @@ void b200_geometry_identity(int w, int h, b200_geometry* g) { b200_geometry_init
 
 // new(u,v) -> old(u',v') = T(u,v), then old mapping applied: m' = m o T
 static void compose(b200_geometry* g, const int t[6], int nw, int nh) {
-  int n[6];
-  n[0] = g->m[0] * t[0] + g->m[1] * t[3]; n[1] = g->m[0] * t[1] + g->m[1] * t[4]; n[2] = g->m[0] * t[2] + g->m[1] * t[5] + g->m[2];
-  n[3] = g->m[3] * t[0] + g->m[4] * t[3]; n[4] = g->m[3] * t[1] + g->m[4] * t[4]; n[5] = g->m[3] * t[2] + g->m[4] * t[5] + g->m[5];
-  for (int i = 0; i < 6; i++) g->m[i] = n[i];
+  affine_compose(g->m, t, g->m);
   g->out_w = nw; g->out_h = nh;
 }
 
@@ -137,40 +135,69 @@ int finish(HostXfer& X, int rc) {
   if (rc == B200_OK && e != cudaSuccess) return set_error(B200_E_CUDA, "sync: %s", cudaGetErrorString(e));
   return rc;
 }
+
+// A host plane of `rows` rows of `row_bytes` bytes, `stride` bytes apart.  A plane with a null pointer is absent.
+struct HostPlane { const void* p; size_t stride, row_bytes, rows; };
+// A plane's device copy: a null pointer for an absent plane.
+struct DevPlane { char* p; size_t pitch; };
+
+// The staging of a host entry point: copies of the planes `in` and `out` (in that order) at 256-byte pitches in one block
+// of the calling thread's GPU's device buffer.  Uploads `in` in order, calls `run` with the copies (dev[i]: the i-th plane
+// of `in`, then of `out`) and the staging stream, downloads `out` in order and waits for the stream.
+int stage(const std::vector<HostPlane>& in, const std::vector<HostPlane>& out, const std::function<int(const DevPlane*, cudaStream_t)>& run) {
+  std::vector<HostPlane> all(in);
+  all.insert(all.end(), out.begin(), out.end());
+  std::vector<DevPlane> dev(all.size());
+  size_t bytes = 0;
+  for (size_t i = 0; i < all.size(); i++) {
+    dev[i].pitch = (all[i].row_bytes + 255) & ~(size_t)255;
+    if (all[i].p) bytes += dev[i].pitch * all[i].rows;
+  }
+  std::lock_guard<std::mutex> lock(g_xfer_mu);
+  HostXfer* X = nullptr;
+  int rc;
+  if ((rc = host_xfer(&X)) || (rc = X->dev.reserve(bytes, false))) return rc;
+  char* next = X->dev.d;
+  for (size_t i = 0; i < all.size(); i++)
+    if (all[i].p) { dev[i].p = next; next += dev[i].pitch * all[i].rows; }
+  Pool& pool = copy_pool();
+  for (size_t i = 0; i < in.size() && rc == B200_OK; i++)
+    if (in[i].p) rc = X->bounce.upload(dev[i].p, dev[i].pitch, in[i].p, in[i].stride, in[i].row_bytes, in[i].rows, X->s, pool);
+  if (rc == B200_OK) rc = run(dev.data(), X->s);
+  for (size_t i = in.size(); i < all.size() && rc == B200_OK; i++)
+    if (all[i].p) rc = X->bounce.download((void*)all[i].p, all[i].stride, dev[i].p, dev[i].pitch, all[i].row_bytes, all[i].rows, X->s, pool);
+  return finish(*X, rc);
+}
+
+// Y, Cb, Cr and alpha of `p` at `bps` bytes per sample (no chroma planes for monochrome)
+std::vector<HostPlane> ycc_planes(const b200_planes& p, size_t bps) {
+  int cw, ch;
+  chroma_size(p.chroma, p.width, p.height, cw, ch);
+  const size_t w = (size_t)p.width, h = (size_t)p.height;
+  return {{p.y, p.y_stride, w * bps, h}, {cw ? p.cb : nullptr, p.c_stride, cw * bps, (size_t)ch},
+          {cw ? p.cr : nullptr, p.c_stride, cw * bps, (size_t)ch}, {p.alpha, p.alpha_stride, w * bps, h}};
+}
+// `p` on the device copies dev[0..3] of its ycc_planes()
+b200_planes on_device(b200_planes p, const DevPlane* dev) {
+  p.y = dev[0].p; p.cb = dev[1].p; p.cr = dev[2].p; p.alpha = dev[3].p;
+  p.y_stride = dev[0].pitch; p.c_stride = dev[1].pitch; p.alpha_stride = dev[3].pitch;
+  return p;
+}
 }  // namespace
 }  // extern "C++"
 
 int b200_color_convert_host(const b200_planes* in, const b200_geometry* geom, const b200_color_options* opt, void* out,
                             void* out_g, void* out_b, size_t out_stride, int* pipeline) {
   if (!in || !geom || !opt || !out) return set_error(B200_E_INVALID, "null argument");
-  const int bps = in->bit_depth > 8 ? 2 : 1;
-  const int sh = (in->chroma == B200_CHROMA_420 || in->chroma == B200_CHROMA_422) ? 1 : 0;
-  const int sv = in->chroma == B200_CHROMA_420 ? 1 : 0;
-  const int cw = in->chroma == B200_CHROMA_MONO ? 0 : (in->width + sh) >> sh, ch = in->chroma == B200_CHROMA_MONO ? 0 : (in->height + sv) >> sv;
-  const size_t ypitch = (((size_t)in->width * bps) + 255) & ~(size_t)255, cpitch = (((size_t)cw * bps) + 255) & ~(size_t)255;
-  const size_t rowb = out_row_bytes(opt->out_chroma, geom->out_w, in->bit_depth);
-  const size_t opitch = (rowb + 255) & ~(size_t)255;
-  const int nout = opt->out_chroma == B200_CHROMA_444 ? 3 : 1;
-  if (nout == 3 && (!out_g || !out_b)) return set_error(B200_E_INVALID, "planar output needs three planes");
-  const size_t ybytes = ypitch * (size_t)in->height, cbytes = cpitch * (size_t)ch, abytes = in->alpha ? ybytes : 0, obytes = opitch * (size_t)geom->out_h;
-  std::lock_guard<std::mutex> lock(g_xfer_mu);
-  HostXfer* X = nullptr;
-  int rc;
-  if ((rc = host_xfer(&X)) || (rc = X->dev.reserve(ybytes + 2 * cbytes + abytes + obytes * (size_t)nout, false))) return rc;
-  char* dy = X->dev.d; char* dcb = dy + ybytes; char* dcr = dcb + cbytes; char* da = dcr + cbytes; char* dout = da + abytes;
-  Pool& pool = copy_pool();
-  rc = X->bounce.upload(dy, ypitch, in->y, in->y_stride, (size_t)in->width * bps, (size_t)in->height, X->s, pool);
-  if (cw && rc == B200_OK) rc = X->bounce.upload(dcb, cpitch, in->cb, in->c_stride, (size_t)cw * bps, (size_t)ch, X->s, pool);
-  if (cw && rc == B200_OK) rc = X->bounce.upload(dcr, cpitch, in->cr, in->c_stride, (size_t)cw * bps, (size_t)ch, X->s, pool);
-  if (in->alpha && rc == B200_OK) rc = X->bounce.upload(da, ypitch, in->alpha, in->alpha_stride, (size_t)in->width * bps, (size_t)in->height, X->s, pool);
-  if (rc == B200_OK) {
-    b200_planes d = *in;
-    d.y = dy; d.cb = cw ? dcb : nullptr; d.cr = cw ? dcr : nullptr; d.alpha = in->alpha ? da : nullptr; d.y_stride = ypitch; d.c_stride = cpitch; d.alpha_stride = ypitch;
-    rc = launch_color(&d, geom, opt, dout, dout + obytes, dout + 2 * obytes, opitch, X->s, pipeline);
-  }
-  void* outs[3] = {out, out_g, out_b};
-  for (int c = 0; c < nout && rc == B200_OK; c++) rc = X->bounce.download(outs[c], out_stride, dout + (size_t)c * obytes, opitch, rowb, (size_t)geom->out_h, X->s, pool);
-  return finish(*X, rc);
+  const size_t rowb = out_row_bytes(opt->out_chroma, geom->out_w, in->bit_depth), oh = (size_t)geom->out_h;
+  const bool planar = opt->out_chroma == B200_CHROMA_444;
+  if (planar && (!out_g || !out_b)) return set_error(B200_E_INVALID, "planar output needs three planes");
+  return stage(ycc_planes(*in, in->bit_depth > 8 ? 2 : 1),
+               {{out, out_stride, rowb, oh}, {planar ? out_g : nullptr, out_stride, rowb, oh}, {planar ? out_b : nullptr, out_stride, rowb, oh}},
+               [&](const DevPlane* dev, cudaStream_t s) {
+                 const b200_planes d = on_device(*in, dev);
+                 return launch_color(&d, geom, opt, dev[4].p, dev[5].p, dev[6].p, dev[4].pitch, s, pipeline);
+               });
 }
 
 int b200_rgb_to_ycbcr_device(const void* rgb, size_t rgb_stride, int has_alpha, const b200_planes* out, void* stream) {
@@ -183,28 +210,11 @@ int b200_rgb_to_ycbcr_host(const void* rgb, size_t rgb_stride, int has_alpha, co
   if (out->chroma != B200_CHROMA_420 && out->chroma != B200_CHROMA_422 && out->chroma != B200_CHROMA_444)
     return set_error(B200_E_UNSUPPORTED, "RGB -> YCbCr: target chroma %d", out->chroma);
   if (!out->cb || !out->cr) return set_error(B200_E_INVALID, "RGB -> YCbCr: chroma planes missing");
-  const int w = out->width, h = out->height, bpp = has_alpha ? 4 : 3;
-  const int sh = out->chroma == B200_CHROMA_444 ? 0 : 1, sv = out->chroma == B200_CHROMA_420 ? 1 : 0;
-  const int cw = (w + sh) >> sh, ch = (h + sv) >> sv;
-  const size_t ipitch = (((size_t)w * bpp) + 255) & ~(size_t)255, ypitch = ((size_t)w + 255) & ~(size_t)255, cpitch = ((size_t)cw + 255) & ~(size_t)255;
-  const size_t ibytes = ipitch * (size_t)h, ybytes = ypitch * (size_t)h, cbytes = cpitch * (size_t)ch, abytes = out->alpha ? ybytes : 0;
-  std::lock_guard<std::mutex> lock(g_xfer_mu);
-  HostXfer* X = nullptr;
-  int rc;
-  if ((rc = host_xfer(&X)) || (rc = X->dev.reserve(ibytes + ybytes + 2 * cbytes + abytes, false))) return rc;
-  char* din = X->dev.d; char* dy = din + ibytes; char* dcb = dy + ybytes; char* dcr = dcb + cbytes; char* da = out->alpha ? dcr + cbytes : nullptr;
-  Pool& pool = copy_pool();
-  rc = X->bounce.upload(din, ipitch, rgb, rgb_stride, (size_t)w * bpp, (size_t)h, X->s, pool);
-  if (rc == B200_OK) {
-    b200_planes d = *out;
-    d.y = dy; d.cb = dcb; d.cr = dcr; d.alpha = da; d.y_stride = ypitch; d.c_stride = cpitch; d.alpha_stride = ypitch;
-    rc = launch_rgb_to_ycbcr(din, ipitch, has_alpha, &d, X->s);
-  }
-  if (rc == B200_OK) rc = X->bounce.download((void*)out->y, out->y_stride, dy, ypitch, (size_t)w, (size_t)h, X->s, pool);
-  if (rc == B200_OK) rc = X->bounce.download((void*)out->cb, out->c_stride, dcb, cpitch, (size_t)cw, (size_t)ch, X->s, pool);
-  if (rc == B200_OK) rc = X->bounce.download((void*)out->cr, out->c_stride, dcr, cpitch, (size_t)cw, (size_t)ch, X->s, pool);
-  if (out->alpha && rc == B200_OK) rc = X->bounce.download((void*)out->alpha, out->alpha_stride, da, ypitch, (size_t)w, (size_t)h, X->s, pool);
-  return finish(*X, rc);
+  return stage({{rgb, rgb_stride, (size_t)out->width * (has_alpha ? 4 : 3), (size_t)out->height}}, ycc_planes(*out, 1),
+               [&](const DevPlane* dev, cudaStream_t s) {
+                 const b200_planes d = on_device(*out, dev + 1);
+                 return launch_rgb_to_ycbcr(dev[0].p, dev[0].pitch, has_alpha, &d, s);
+               });
 }
 
 int b200_rgb_to_ycbcr_plan(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, int* pipeline) {
@@ -232,39 +242,27 @@ int b200_rgb_to_ycbcr_ex_host(const b200_rgb_image* in, const b200_planes* out, 
   const int nin = planar ? (in->alpha ? 4 : 3) : 1;
   const void* src[4] = {planar ? in->r : in->rgb, in->g, in->b, in->alpha};
   const size_t sstride[4] = {planar ? in->r_stride : in->rgb_stride, in->g_stride, in->b_stride, in->alpha_stride};
-  const int sh = out->chroma == B200_CHROMA_444 ? 0 : 1, sv = out->chroma == B200_CHROMA_420 ? 1 : 0;
-  const int cw = (w + sh) >> sh, ch = (h + sv) >> sv;
-  const size_t irow = (size_t)w * nch * bps, ipitch = (irow + 255) & ~(size_t)255;
+  int cw, ch;
+  chroma_size(out->chroma, w, h, cw, ch);
+  const size_t irow = (size_t)w * nch * bps;
   // the caller's rows are read on the host: every stride is checked before anything is staged
+  std::vector<HostPlane> rgb(4);
   for (int c = 0; c < nin; c++) {
     if (!src[c]) return set_error(B200_E_INVALID, "RGB input planes missing");
     if (sstride[c] < irow) return set_error(B200_E_INVALID, "RGB input plane %d: stride %zu < row of %zu bytes", c, sstride[c], irow);
+    rgb[c] = {src[c], sstride[c], irow, (size_t)h};
   }
   if (out->y_stride < (size_t)w * bps || out->c_stride < (size_t)cw * bps || (out->alpha && out->alpha_stride < (size_t)w * bps))
     return set_error(B200_E_INVALID, "YCbCr output stride smaller than a row");
-  const size_t ypitch = (((size_t)w * bps) + 255) & ~(size_t)255, cpitch = (((size_t)cw * bps) + 255) & ~(size_t)255;
-  const size_t ibytes = ipitch * (size_t)h, ybytes = ypitch * (size_t)h, cbytes = cpitch * (size_t)ch, abytes = out->alpha ? ybytes : 0;
-  std::lock_guard<std::mutex> lock(g_xfer_mu);
-  HostXfer* X = nullptr;
-  if ((rc = host_xfer(&X)) || (rc = X->dev.reserve(ibytes * nin + ybytes + 2 * cbytes + abytes, false))) return rc;
-  char* din = X->dev.d; char* dy = din + ibytes * nin; char* dcb = dy + ybytes; char* dcr = dcb + cbytes; char* da = out->alpha ? dcr + cbytes : nullptr;
-  Pool& pool = copy_pool();
-  for (int c = 0; c < nin && rc == B200_OK; c++) rc = X->bounce.upload(din + (size_t)c * ibytes, ipitch, src[c], sstride[c], irow, (size_t)h, X->s, pool);
-  if (rc == B200_OK) {
+  return stage(rgb, ycc_planes(*out, bps), [&](const DevPlane* dev, cudaStream_t s) {
     b200_rgb_image d = *in;
     if (planar) {
-      d.r = din; d.g = din + ibytes; d.b = din + 2 * ibytes; d.alpha = in->alpha ? din + 3 * ibytes : nullptr;
-      d.r_stride = d.g_stride = d.b_stride = d.alpha_stride = ipitch;
-    } else { d.rgb = din; d.rgb_stride = ipitch; }
-    b200_planes o = *out;
-    o.y = dy; o.cb = dcb; o.cr = dcr; o.alpha = da; o.y_stride = ypitch; o.c_stride = cpitch; o.alpha_stride = ypitch;
-    rc = launch_rgb_to_ycbcr_ex(&d, &o, opt, X->s, pipeline);
-  }
-  if (rc == B200_OK) rc = X->bounce.download((void*)out->y, out->y_stride, dy, ypitch, (size_t)w * bps, (size_t)h, X->s, pool);
-  if (rc == B200_OK) rc = X->bounce.download((void*)out->cb, out->c_stride, dcb, cpitch, (size_t)cw * bps, (size_t)ch, X->s, pool);
-  if (rc == B200_OK) rc = X->bounce.download((void*)out->cr, out->c_stride, dcr, cpitch, (size_t)cw * bps, (size_t)ch, X->s, pool);
-  if (out->alpha && rc == B200_OK) rc = X->bounce.download((void*)out->alpha, out->alpha_stride, da, ypitch, (size_t)w * bps, (size_t)h, X->s, pool);
-  return finish(*X, rc);
+      d.r = dev[0].p; d.g = dev[1].p; d.b = dev[2].p; d.alpha = dev[3].p;
+      d.r_stride = d.g_stride = d.b_stride = d.alpha_stride = dev[0].pitch;
+    } else { d.rgb = dev[0].p; d.rgb_stride = dev[0].pitch; }
+    const b200_planes o = on_device(*out, dev + 4);
+    return launch_rgb_to_ycbcr_ex(&d, &o, opt, s, pipeline);
+  });
 }
 
 }  // extern "C"

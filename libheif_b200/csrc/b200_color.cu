@@ -470,47 +470,51 @@ static int convert_via_444(const b200_planes* in, const b200_geometry* g, const 
   const int bps = in->bit_depth > 8 ? 2 : 1;
   const bool c422 = in->chroma == B200_CHROMA_422;
   const int shy = c422 ? 0 : 1;
-  const int pw = g->pre_w, ph = g->pre_h, pcw = (pw + 1) / 2, pch = c422 ? ph : (ph + 1) / 2;
-  const bool pre_identity = g->pre[0] == 1 && g->pre[1] == 0 && g->pre[2] == 0 && g->pre[3] == 0 && g->pre[4] == 1 && g->pre[5] == 0 && pw == in->width && ph == in->height;
+  const int pw = g->pre_w, ph = g->pre_h;
+  int pcw, pch;
+  chroma_size(in->chroma, pw, ph, pcw, pch);
+  const bool pre_identity = is_identity(g->pre, pw, ph, in->width, in->height);
   const size_t pitch = (((size_t)pw * bps) + 255) & ~(size_t)255, cpitch = (((size_t)pcw * bps) + 255) & ~(size_t)255;
-  const size_t n_full = pitch * ph, n_c = cpitch * pch;
+  // scratch planes, each only where the call writes it: Y' (geometry or range conversion), A' (geometry of alpha),
+  // Cb444, Cr444, Cb' and Cr' (geometry)
+  const size_t n_full = pitch * ph, n_y = !pre_identity || range_convert ? n_full : 0, n_a = !pre_identity && in->alpha ? n_full : 0;
+  const size_t n_c = pre_identity ? 0 : cpitch * pch;
   char* tmp = nullptr;
-  B200_CUDA_CHECK(cudaMallocAsync(&tmp, 4 * n_full + 2 * n_c, stream));    // Y', A', Cb444, Cr444, Cb', Cr'
-  char *ty = tmp, *ta = tmp + n_full, *u_cb = tmp + 2 * n_full, *u_cr = tmp + 3 * n_full, *tcb = tmp + 4 * n_full, *tcr = tmp + 4 * n_full + n_c;
+  B200_CUDA_CHECK(cudaMallocAsync(&tmp, n_y + n_a + 2 * n_full + 2 * n_c, stream));
+  char *ty = tmp, *ta = ty + n_y, *u_cb = ta + n_a, *u_cr = u_cb + n_full, *tcb = u_cr + n_full, *tcr = tcb + n_c;
   b200_planes p = *in;
-  if (!pre_identity) {
-    const int* q = g->pre;
-    auto run = [&](const void* src, size_t sstride, void* dst, size_t dstride, int w, int h, int sx, int sy) {
-      dim3 grid((w + 255) / 256, h);
-      if (bps == 1) plane_geometry_kernel<uint8_t><<<grid, 256, 0, stream>>>((const uint8_t*)src, (long long)sstride, (uint8_t*)dst, (long long)dstride, w, h, q[0], q[1], q[2], q[3], q[4], q[5], sx, sy);
-      else plane_geometry_kernel<uint16_t><<<grid, 256, 0, stream>>>((const uint16_t*)src, (long long)sstride / 2, (uint16_t*)dst, (long long)dstride / 2, w, h, q[0], q[1], q[2], q[3], q[4], q[5], sx, sy);
-    };
-    run(in->y, in->y_stride, ty, pitch, pw, ph, 0, 0);
-    run(in->cb, in->c_stride, tcb, cpitch, pcw, pch, 1, shy);
-    run(in->cr, in->c_stride, tcr, cpitch, pcw, pch, 1, shy);
-    if (in->alpha) run(in->alpha, in->alpha_stride, ta, pitch, pw, ph, 0, 0);
-    p.y = ty; p.y_stride = pitch; p.cb = tcb; p.cr = tcr; p.c_stride = cpitch;
-    if (in->alpha) { p.alpha = ta; p.alpha_stride = pitch; }
-    p.width = pw; p.height = ph;
-  }
-  dim3 grid((pw + 255) / 256, ph);
-  if (c422) {
-    if (bps == 1) bilinear_422_to_444_kernel<uint8_t><<<grid, 256, 0, stream>>>((const uint8_t*)p.cb, (const uint8_t*)p.cr, (long long)p.c_stride, (uint8_t*)u_cb, (uint8_t*)u_cr, (long long)pitch, pw, ph);
-    else bilinear_422_to_444_kernel<uint16_t><<<grid, 256, 0, stream>>>((const uint16_t*)p.cb, (const uint16_t*)p.cr, (long long)p.c_stride / 2, (uint16_t*)u_cb, (uint16_t*)u_cr, (long long)pitch / 2, pw, ph);
-  } else {
-    if (bps == 1) bilinear_420_to_444_kernel<uint8_t><<<grid, 256, 0, stream>>>((const uint8_t*)p.cb, (const uint8_t*)p.cr, (long long)p.c_stride, (uint8_t*)u_cb, (uint8_t*)u_cr, (long long)pitch, pw, ph);
-    else bilinear_420_to_444_kernel<uint16_t><<<grid, 256, 0, stream>>>((const uint16_t*)p.cb, (const uint16_t*)p.cr, (long long)p.c_stride / 2, (uint16_t*)u_cb, (uint16_t*)u_cr, (long long)pitch / 2, pw, ph);
-  }
-  p.cb = u_cb; p.cr = u_cr; p.c_stride = pitch; p.chroma = B200_CHROMA_444;
-  if (range_convert) {
-    // limited -> full range through RGB; Y goes to the scratch plane (the caller's luma plane is never written)
-    RangeArgs ra; ra.bpp = in->bit_depth;
-    ycbcr_to_rgb_coefficients(in->matrix_coefficients, in->colour_primaries, ra.cf);
-    rgb_to_ycbcr_coefficients(in->matrix_coefficients, in->colour_primaries, ra.c);
-    if (bps == 1) range_limited_to_full_444_kernel<uint8_t><<<grid, 256, 0, stream>>>((const uint8_t*)p.y, (long long)p.y_stride, (const uint8_t*)u_cb, (const uint8_t*)u_cr, (long long)pitch, (uint8_t*)ty, (long long)pitch, (uint8_t*)u_cb, (uint8_t*)u_cr, (long long)pitch, pw, ph, ra);
-    else range_limited_to_full_444_kernel<uint16_t><<<grid, 256, 0, stream>>>((const uint16_t*)p.y, (long long)p.y_stride / 2, (const uint16_t*)u_cb, (const uint16_t*)u_cr, (long long)pitch / 2, (uint16_t*)ty, (long long)pitch / 2, (uint16_t*)u_cb, (uint16_t*)u_cr, (long long)pitch / 2, pw, ph, ra);
-    p.y = ty; p.y_stride = pitch; p.width = pw; p.height = ph; p.full_range = 1;
-  }
+  auto run = [&](auto sample) {
+    using T = decltype(sample);
+    auto el = [](size_t stride) { return (long long)(stride / sizeof(T)); };      // byte stride -> elements
+    if (!pre_identity) {
+      const int* q = g->pre;
+      auto geom = [&](const void* src, size_t sstride, void* dst, size_t dstride, int w, int h, int sx, int sy) {
+        plane_geometry_kernel<T><<<dim3((w + 255) / 256, h), 256, 0, stream>>>((const T*)src, el(sstride), (T*)dst, el(dstride), w, h,
+                                                                               q[0], q[1], q[2], q[3], q[4], q[5], sx, sy);
+      };
+      geom(in->y, in->y_stride, ty, pitch, pw, ph, 0, 0);
+      geom(in->cb, in->c_stride, tcb, cpitch, pcw, pch, 1, shy);
+      geom(in->cr, in->c_stride, tcr, cpitch, pcw, pch, 1, shy);
+      if (in->alpha) geom(in->alpha, in->alpha_stride, ta, pitch, pw, ph, 0, 0);
+      p.y = ty; p.y_stride = pitch; p.cb = tcb; p.cr = tcr; p.c_stride = cpitch;
+      if (in->alpha) { p.alpha = ta; p.alpha_stride = pitch; }
+      p.width = pw; p.height = ph;
+    }
+    const dim3 grid((pw + 255) / 256, ph);
+    if (c422) bilinear_422_to_444_kernel<T><<<grid, 256, 0, stream>>>((const T*)p.cb, (const T*)p.cr, el(p.c_stride), (T*)u_cb, (T*)u_cr, el(pitch), pw, ph);
+    else bilinear_420_to_444_kernel<T><<<grid, 256, 0, stream>>>((const T*)p.cb, (const T*)p.cr, el(p.c_stride), (T*)u_cb, (T*)u_cr, el(pitch), pw, ph);
+    p.cb = u_cb; p.cr = u_cr; p.c_stride = pitch; p.chroma = B200_CHROMA_444;
+    if (range_convert) {
+      // limited -> full range through RGB; Y goes to the scratch plane (the caller's luma plane is never written)
+      RangeArgs ra; ra.bpp = in->bit_depth;
+      ycbcr_to_rgb_coefficients(in->matrix_coefficients, in->colour_primaries, ra.cf);
+      rgb_to_ycbcr_coefficients(in->matrix_coefficients, in->colour_primaries, ra.c);
+      range_limited_to_full_444_kernel<T><<<grid, 256, 0, stream>>>((const T*)p.y, el(p.y_stride), (const T*)u_cb, (const T*)u_cr, el(pitch), (T*)ty,
+                                                                     el(pitch), (T*)u_cb, (T*)u_cr, el(pitch), pw, ph, ra);
+      p.y = ty; p.y_stride = pitch; p.width = pw; p.height = ph; p.full_range = 1;
+    }
+  };
+  if (bps == 1) run(uint8_t()); else run(uint16_t());
   b200_geometry rest = *g; rest.detour = 0; rest.chroma = B200_CHROMA_444;
   b200_color_options o2 = *opt; o2.chroma_upsampling = 0;
   int rc = launch_color(&p, &rest, &o2, out, out_g, out_b, out_stride, stream, pipeline);
@@ -537,11 +541,10 @@ int launch_color(const b200_planes* in, const b200_geometry* g, const b200_color
   if (g->detour && !subsampled) {
     // the chain was composed with the rules of a subsampled format but the picture is not subsampled: one affine map
     b200_geometry t = *g; t.detour = 0;
-    t.m[0] = g->pre[0] * g->m[0] + g->pre[1] * g->m[3]; t.m[1] = g->pre[0] * g->m[1] + g->pre[1] * g->m[4]; t.m[2] = g->pre[0] * g->m[2] + g->pre[1] * g->m[5] + g->pre[2];
-    t.m[3] = g->pre[3] * g->m[0] + g->pre[4] * g->m[3]; t.m[4] = g->pre[3] * g->m[1] + g->pre[4] * g->m[4]; t.m[5] = g->pre[3] * g->m[2] + g->pre[4] * g->m[5] + g->pre[5];
+    affine_compose(g->pre, g->m, t.m);
     return launch_color(in, &t, opt, out, out_g, out_b, out_stride, stream, pipeline);
   }
-  const bool geom_identity = g->m[0] == 1 && g->m[1] == 0 && g->m[2] == 0 && g->m[3] == 0 && g->m[4] == 1 && g->m[5] == 0 && g->out_w == in->width && g->out_h == in->height && !g->detour;
+  const bool geom_identity = is_identity(g->m, g->out_w, g->out_h, in->width, in->height) && !g->detour;
   if (subsampled && !geom_identity && g->chroma != in->chroma)
     return set_error(B200_E_INVALID, "geometry was composed for chroma format %d, the picture has %d (b200_geometry_init)", g->chroma, in->chroma);
   if (g->detour) {
@@ -553,30 +556,14 @@ int launch_color(const b200_planes* in, const b200_geometry* g, const b200_color
   }
   if (opt->chroma_upsampling == 1 && in->chroma == B200_CHROMA_420) {
     // heif_color_conversion_options.only_use_preferred_chroma_algorithm with bilinear upsampling: the reference runs
-    // Op_YCbCr420_bilinear_to_YCbCr444 first and converts from 4:4:4 with the generic float op.
-    const bool identity = g->m[0] == 1 && g->m[1] == 0 && g->m[2] == 0 && g->m[3] == 0 && g->m[4] == 1 && g->m[5] == 0 && g->out_w == in->width && g->out_h == in->height;
-    if (!identity) {
-      // geometry happens on the planes BEFORE the colour conversion in the reference, so the bilinear op sees the
-      // transformed 4:2:0 picture: all of the chain is `pre`, nothing is left after the upsampling
-      b200_geometry t = *g; t.detour = 1;
-      for (int i = 0; i < 6; i++) t.pre[i] = g->m[i];
-      t.pre_w = g->out_w; t.pre_h = g->out_h;
-      t.m[0] = 1; t.m[1] = 0; t.m[2] = 0; t.m[3] = 0; t.m[4] = 1; t.m[5] = 0;
-      return convert_via_444(in, &t, opt, out, out_g, out_b, out_stride, stream, pipeline, false);
-    }
-    const int bps = in->bit_depth > 8 ? 2 : 1;
-    const size_t pitch = (((size_t)in->width * bps) + 255) & ~(size_t)255;
-    char* tmp = nullptr;
-    B200_CUDA_CHECK(cudaMallocAsync(&tmp, 2 * pitch * in->height, stream));
-    dim3 grid((in->width + 255) / 256, in->height);
-    if (bps == 1) bilinear_420_to_444_kernel<uint8_t><<<grid, 256, 0, stream>>>((const uint8_t*)in->cb, (const uint8_t*)in->cr, (long long)in->c_stride, (uint8_t*)tmp, (uint8_t*)(tmp + pitch * in->height), (long long)pitch, in->width, in->height);
-    else bilinear_420_to_444_kernel<uint16_t><<<grid, 256, 0, stream>>>((const uint16_t*)in->cb, (const uint16_t*)in->cr, (long long)in->c_stride / 2, (uint16_t*)tmp, (uint16_t*)(tmp + pitch * in->height), (long long)pitch / 2, in->width, in->height);
-    b200_planes up = *in; up.cb = tmp; up.cr = tmp + pitch * in->height; up.c_stride = pitch; up.chroma = B200_CHROMA_444;
-    b200_color_options o2 = *opt; o2.chroma_upsampling = 0;
-    int rc = launch_color(&up, g, &o2, out, out_g, out_b, out_stride, stream, pipeline);
-    if (pipeline) *pipeline |= B200_PIPE_BILINEAR;
-    cudaFreeAsync(tmp, stream);
-    return rc;
+    // Op_YCbCr420_bilinear_to_YCbCr444 first and converts from 4:4:4 with the generic float op.  Geometry happens on the
+    // planes BEFORE the colour conversion in the reference, so the bilinear op sees the transformed 4:2:0 picture: all of
+    // the chain is `pre`, nothing is left after the upsampling
+    b200_geometry t = *g; t.detour = 1;
+    for (int i = 0; i < 6; i++) t.pre[i] = g->m[i];
+    t.pre_w = g->out_w; t.pre_h = g->out_h;
+    t.m[0] = 1; t.m[1] = 0; t.m[2] = 0; t.m[3] = 0; t.m[4] = 1; t.m[5] = 0;
+    return convert_via_444(in, &t, opt, out, out_g, out_b, out_stride, stream, pipeline, false);
   }
   K6Args a{};
   a.y = in->y; a.cb = in->cb; a.cr = in->cr; a.a = in->alpha;
@@ -622,7 +609,7 @@ int launch_color(const b200_planes* in, const b200_geometry* g, const b200_color
   if (pipeline) *pipeline = pipe;
   if (g->out_w <= 0 || g->out_h <= 0) return B200_OK;
   // fast path: identity geometry, 4:2:0, no alpha, everything 16-byte aligned (the grid / single-image decode case)
-  const bool identity = g->m[0] == 1 && g->m[1] == 0 && g->m[2] == 0 && g->m[3] == 0 && g->m[4] == 1 && g->m[5] == 0 && g->out_w == in->width && g->out_h == in->height;
+  const bool identity = is_identity(g->m, g->out_w, g->out_h, in->width, in->height);
   const uintptr_t al = (uintptr_t)in->y | (uintptr_t)in->cb | (uintptr_t)in->cr | (uintptr_t)out | (uintptr_t)in->y_stride | (uintptr_t)in->c_stride | (uintptr_t)out_stride;
   if (identity && in->chroma == B200_CHROMA_420 && !has_alpha && !a.special && (al & 15) == 0 && in->width % 16 == 0 && in->height % 2 == 0 && fmt != B200_CHROMA_444 && !(a.sdr_shift && a.out_bytes == 2)) {
     bool done;

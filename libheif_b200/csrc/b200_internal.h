@@ -18,6 +18,25 @@ int set_error(int code, const char* fmt, ...);     // records a thread-local mes
     if (e__ != cudaSuccess) return ::b200::set_error(B200_E_CUDA, "%s: %s", #expr, cudaGetErrorString(e__)); \
   } while (0)
 
+// size of the chroma planes of a w x h picture; 0 x 0 for monochrome
+inline void chroma_size(int chroma, int w, int h, int& cw, int& ch) {
+  const int sh = chroma == B200_CHROMA_420 || chroma == B200_CHROMA_422, sv = chroma == B200_CHROMA_420;
+  cw = chroma == B200_CHROMA_MONO ? 0 : (w + sh) >> sh;
+  ch = chroma == B200_CHROMA_MONO ? 0 : (h + sv) >> sv;
+}
+
+// Affine maps of b200_geometry, {m0, ..., m5}: output (u, v) -> source (m0 u + m1 v + m2, m3 u + m4 v + m5).
+// out = a o b, i.e. b applied first; out may be a or b.
+inline void affine_compose(const int a[6], const int b[6], int out[6]) {
+  const int n[6] = {a[0] * b[0] + a[1] * b[3], a[0] * b[1] + a[1] * b[4], a[0] * b[2] + a[1] * b[5] + a[2],
+                    a[3] * b[0] + a[4] * b[3], a[3] * b[1] + a[4] * b[4], a[3] * b[2] + a[4] * b[5] + a[5]};
+  for (int i = 0; i < 6; i++) out[i] = n[i];
+}
+// whether m with a w x h output leaves a w_in x h_in picture as it is
+inline bool is_identity(const int m[6], int w, int h, int w_in, int h_in) {
+  return m[0] == 1 && m[1] == 0 && m[2] == 0 && m[3] == 0 && m[4] == 1 && m[5] == 0 && w == w_in && h == h_in;
+}
+
 void ycbcr_to_rgb_coefficients(int matrix, int primaries, float out[4]);
 int launch_color(const b200_planes* in, const b200_geometry* g, const b200_color_options* opt, void* out, void* out_g,
                  void* out_b, size_t out_stride, cudaStream_t stream, int* pipeline);

@@ -89,7 +89,7 @@ class GridEncodeInfo(C.Structure):
 def _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferred, bit_depth, endianness, alpha_bit_depth, params):
     """(b200_rgb_image, params, options, device?) of the b200_gpu_encode_rgb_grid_* calls; rgb: numpy array or CUDA tensor
     [H, W, 3|4], or a tuple (R, G, B) of [H, W] planes with the optional alpha plane in `alpha`."""
-    from .color import _np_is16, _np_packed, _rgb_image
+    from .color import _HOST, _Cuda, _rgb_image
     planar = isinstance(rgb, (tuple, list))
     if alpha is not None and not planar:
         raise ValueError("alpha= is the alpha plane of planar input; interleaved input carries alpha as RGBA")
@@ -99,11 +99,8 @@ def _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferr
         rgb = tuple(rgb) + ((alpha,) if alpha is not None else ())
     first = rgb[0] if planar else rgb
     device = hasattr(first, "is_cuda") and first.is_cuda
-    if device:
-        d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda t: t.data_ptr(), lambda t: t.stride(0) * t.element_size(),
-                          lambda t: t.element_size() == 2, lambda t: t.stride(-1) == 1 and (t.dim() == 2 or t.stride(1) == t.shape[2]))
-    else:
-        d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, lambda a: a.ctypes.data, lambda a: a.strides[0], _np_is16, _np_packed)
+    mem = _Cuda(first.device) if device else _HOST
+    d, _ = _rgb_image(rgb, bit_depth, endianness, alpha_bit_depth, mem.ptr, mem.stride, mem.is16, mem.packed)
     p = gpu_params(tile_w, tile_h, True, **params)
     opt = _lib.RgbToYCbCrOptions(chroma_downsampling, int(bool(only_use_preferred)))
     return d, p, opt, device
