@@ -237,6 +237,7 @@ typedef struct b200_hevc_enc_params {
   int tiles_uniform;                 /* 1 = uniform_spacing_flag, 0 = column widths / row heights drawn by the LCG and coded explicitly */
   int loop_filter_across_tiles;      /* loop_filter_across_tiles_enabled_flag */
   int slice_per_tile;                /* 1 = every tile is a slice of its own, 0 = one slice holds all tiles (one entry point per tile) */
+  int speed;                         /* GPU encoder only (the host encoder ignores it): mode-decision speed 0..2, see below */
 } b200_hevc_enc_params;
 
 void b200_hevc_enc_params_default(b200_hevc_enc_params* p);
@@ -252,10 +253,17 @@ void b200_free(void* p);
  * Coding decisions are deterministic (no LCG): the same input gives the same bytes, alone or in any batch.
  * Accepted b200_hevc_enc_params: width / height 8..16384 (coded size rounded up to 8, conformance window), log2_ctb_size 5
  * or 6, qp / init_qp 0..51, wpp = 1 (required), max_transform_hierarchy_depth_intra, strong_intra_smoothing, PPS and slice
- * Cb / Cr QP offsets, every deblocking field, still_picture, VUI / colour fields.  mode_decision, split_threshold and seed
- * are ignored.  B200_E_UNSUPPORTED (message names the field): sao, sign_data_hiding, transform_skip, cu_qp_delta,
+ * Cb / Cr QP offsets, every deblocking field, still_picture, VUI / colour fields, speed.  mode_decision, split_threshold and
+ * seed are ignored.  B200_E_UNSUPPORTED (message names the field): sao, sign_data_hiding, transform_skip, cu_qp_delta,
  * scaling_lists, pcm, transquant_bypass, tile_cols / tile_rows > 1, slice_ctb_rows, dependent_slice_segments, bit_depth != 8,
- * chroma_format_idc 2 / 3, wpp = 0.  All validation happens before any CUDA call.
+ * chroma_format_idc 2 / 3, wpp = 0.  B200_E_INVALID (message names `speed`): speed outside 0..2.  All validation happens
+ * before any CUDA call.
+ * speed trades compression for encoding time in the mode decision; the quadtree walk (CTB down to 8x8, NxN at 8x8) and the
+ * final pass, which codes the chosen CUs closed loop in decoding order, are the same at every speed:
+ *   0 (default): all 35 luma modes of every PU, decisions in closed loop (neighbours from the reconstruction);
+ *   1: coarse-to-fine search of at most 18 modes per PU (planar, DC, angular 2, 6, .., 34 and the three MPMs, then the
+ *      angular modes within 2 of the best angular one), closed loop;
+ *   2: as 1, with open-loop decisions: neighbours from the source, no transform round trip before the final pass.
  * Pictures: b200_planes with width / height = the params', chroma B200_CHROMA_420 (chroma_format_idc 1) or B200_CHROMA_MONO
  * (0, cb / cr ignored), bit_depth 8.
  * ------------------------------------------------------------------------------------------------ */
@@ -264,6 +272,8 @@ typedef struct b200_gpu_encode_stats {
   double analyse_ms, entropy_ms;     /* CUDA events: E1 (analysis + reconstruction), E2 (CABAC) of the last call */
   double framing_ms, total_ms;       /* host clock: sub-stream D2H + framing; the whole call */
   uint64_t bytes, ctus, pictures;    /* access-unit bytes, CTBs and pictures of the last call */
+  uint64_t mode_evaluations;         /* decision pass: candidate luma modes whose SATD was computed, over all PU searches */
+  uint64_t cu_evaluations;           /* decision pass: coding units evaluated (the no-split CU and, at 8x8, the NxN one) */
 } b200_gpu_encode_stats;
 
 /* Host only, no CUDA: B200_OK if b200_gpu_encode_intra_* would accept these arguments, else the code and message it would
@@ -284,6 +294,9 @@ int b200_gpu_encoder_get_stats(b200_gpu_encoder* enc, b200_gpu_encode_stats* out
 /* Host only: bytes reserved per CABAC sub-stream (one CTB row) -- the worst case of the syntax; a sub-stream that would need
    more fails the call instead of writing past it. */
 size_t b200_gpu_encoder_substream_capacity(int width, int log2_ctb_size, int chroma_format_idc);
+/* Resident E1 (analysis) warps per SM of the current device for the given speed (cudaOccupancyMaxActiveBlocksPerMultiprocessor):
+   what sizes a batch that fills the device in one wave. */
+int b200_gpu_encoder_e1_warps_per_sm(int speed, int* warps);
 
 /* One call from an 8-bit RGB picture to the access units of a HEIC grid: colour conversion, tiling and HEVC coding on the
  * device -- what heif_context_encode_grid with the "b200-gpu" plugin does one tile per encode_image call

@@ -1,8 +1,11 @@
 // b200_hevc_gpu_enc.cu -- HEVC intra encoder on the GPU: N same-sized 8-bit 4:2:0 / 4:0:0 pictures per call.
 //
 //   E1 (analyse + reconstruct), one warp per (picture, CTB row): CU quadtree from the CTB down to 8x8 (NxN at 8x8), decided
-//      bottom-up on J = SATD(prediction residual) + lambda(QP) * estimated mode bits; all 35 luma modes at every PU size, in
-//      closed loop (neighbours from the encoder's own reconstruction); chroma = DM; TU = CU (implicit splits: NxN, > 32);
+//      bottom-up on J = SATD(prediction residual) + lambda(QP) * estimated mode bits; chroma = DM; TU = CU (implicit splits:
+//      NxN, > 32).  The decision pass has three speeds, each an instantiation of its own (b200_hevc_enc_params::speed):
+//        0: all 35 luma modes at every PU, closed loop (neighbours from the encoder's own reconstruction);
+//        1: a coarse-to-fine search of at most 18 modes (search_mode), closed loop;
+//        2: as 1, open loop: neighbours from the source, no transform round trip before the final pass.
 //      forward DST 4x4 / DCT 4..32, uniform quantisation with the intra rounding offset 171/512, reconstruction with the
 //      inverse path of 8.6.  Writes the reconstruction (HBM plane: the neighbours of the next row), the luma modes per 4x4,
 //      the CU size / partition per 8x8 and the quantised levels (a coefficient plane: every TB's levels at its position).
@@ -27,6 +30,7 @@
 #include "b200_hevc_enc_cabac.h"
 #include "b200_hevc_enc_recon.h"
 #include <algorithm>
+#include <climits>
 #include <chrono>
 #include <memory>
 #include <vector>
@@ -66,6 +70,10 @@ struct Args {
   unsigned* progress; unsigned* progress2; unsigned* ticket; unsigned* error;   // rows, rows, 2, 1
   uint8_t* wpp_ctx;                                          // per row: CTX_COUNT context bytes after its 2nd CTB
   uint8_t* ss; size_t ss_cap; unsigned* ss_len;              // per row sub-stream
+  unsigned long long* work;                                  // E1's work counters: [0] mode evaluations, [1] eval_cu calls
+                                                             // (lane 0 adds to them per PU search / eval_cu: a reduction
+                                                             // without a result, and no counter register kept across the
+                                                             // quadtree calls)
 };
 
 // ---------------------------------------------------------------------------------------------------- E1 workspace
@@ -76,8 +84,15 @@ struct Work {
   int16_t ref[2][132];               // neighbours (8.4.4.2.2): [0] substituted, [1] filtered
   int satd[36];
   int dc, any, acc, mode;
-  uint8_t save[4][4096 + 256];       // per quadtree depth: luma recon + modes of the no-split alternative
 };
+// E1's shared memory at speed S: Work, then per quadtree depth the state of the no-split alternative that the split
+// alternative overwrites -- luma reconstruction and modes (closed loop), or the modes alone (speed 2, which reconstructs in
+// the final pass only); speeds 1 and 2 add the candidate list of the coarse-to-fine search.
+template <int S> struct E1Work : Work {
+  uint8_t save[4][(S == 2 ? 0 : 4096) + 256];
+  uint8_t list[20];                  // candidate modes of the coarse-to-fine search
+};
+template <> struct E1Work<0> : Work { uint8_t save[4][4096 + 256]; };
 
 struct Ctx2 { const Args& a; int p; int lane; Work& w;
   __device__ uint8_t* plane(int c) const { return a.rec + (size_t)p * a.pic_samples + (c == 0 ? 0 : (size_t)a.W * a.H + (size_t)(c - 1) * a.Wc * a.Hc); }
@@ -104,7 +119,10 @@ __device__ inline void mpm_cand(const uint8_t* ipm, int w4, int log2ctb, int x, 
 }
 __device__ inline int mode_bits(int mode, const int cand[3]) { return mode == cand[0] ? 2 : (mode == cand[1] || mode == cand[2]) ? 3 : 6; }
 
-// neighbours of the n x n block of component c at (x0, y0): availability, substitution, filtering (8.4.4.2.2 / .3)
+// neighbours of the n x n block of component c at (x0, y0): availability, substitution, filtering (8.4.4.2.2 / .3).
+// Src: the sample values from the edge-padded source instead of the reconstruction (open-loop decisions), with the same
+// availability.
+template <bool Src = false>
 __device__ void gather_refs(Ctx2& e, int c, int x0, int y0, int log2n) {
   Work& w = e.w;
   const int n = 1 << log2n, sh = c ? 1 : 0, st = c ? e.a.Wc : e.a.W;
@@ -112,7 +130,8 @@ __device__ void gather_refs(Ctx2& e, int c, int x0, int y0, int log2n) {
   for (int i = e.lane; i <= 4 * n; i += GE_LANES) {
     int px, py;
     if (i < 2 * n) { px = x0 - 1; py = y0 + 2 * n - 1 - i; } else if (i == 2 * n) { px = x0 - 1; py = y0 - 1; } else { px = x0 + (i - 2 * n - 1); py = y0 - 1; }
-    w.ref[0][i] = e.avail(px << sh, py << sh) ? (int16_t)GE_LD(pl + (size_t)py * st + px) : (int16_t)-1;
+    if constexpr (Src) w.ref[0][i] = e.avail(px << sh, py << sh) ? (int16_t)e.org(c, px, py) : (int16_t)-1;
+    else w.ref[0][i] = e.avail(px << sh, py << sh) ? (int16_t)GE_LD(pl + (size_t)py * st + px) : (int16_t)-1;
   }
   GE_SYNC();
   if (e.lane == 0) {
@@ -141,24 +160,102 @@ __device__ inline int satd4(const int d[16]) {                   // 4x4 Hadamard
   return (s + 1) >> 1;
 }
 
-// best luma mode of the n x n PU at (x0, y0) on SATD + lambda * mode bits; returns the mode, *cost = its J (x16)
-__device__ int search_mode(Ctx2& e, int x0, int y0, int log2n, long long* cost) {
+// SATD of the n x n block at (x0, y0) for the `cnt` modes mode_at(0 .. cnt - 1), added to w.satd[mode]: one (mode, 4x4
+// sub-block) pair per lane and step (the full search's loop)
+template <typename ModeAt>
+__device__ inline void add_satd(Ctx2& e, int x0, int y0, int log2n, int cnt, ModeAt mode_at) {
   Work& w = e.w;
   const int n = 1 << log2n, nsb = (n * n) >> 4;
-  gather_refs(e, 0, x0, y0, log2n);
-  for (int i = e.lane; i < 35; i += GE_LANES) w.satd[i] = 0;
-  GE_SYNC();
-  for (int it = e.lane; it < 35 * nsb; it += GE_LANES) {
-    const int mode = it % 35, sb = it / 35, bx = (sb % (n >> 2)) << 2, by = (sb / (n >> 2)) << 2;
+  for (int it = e.lane; it < cnt * nsb; it += GE_LANES) {
+    const int mode = mode_at(it % cnt), sb = it / cnt, bx = (sb % (n >> 2)) << 2, by = (sb / (n >> 2)) << 2;
     int d[16];
     for (int k = 0; k < 16; k++) d[k] = e.org(0, x0 + bx + (k & 3), y0 + by + (k >> 2)) - predicted(w, 0, log2n, mode, bx + (k & 3), by + (k >> 2));
     GE_ATOMIC_ADD(&w.satd[mode], satd4(d));
   }
+}
+
+// The same sums for the modes list[0 .. cnt) in mode-major order: the lanes of a step share a mode on consecutive 4x4
+// sub-blocks (a whole warp from 16x16 up), so the prediction does not diverge, and the indices are a shift and a mask.
+__device__ inline void add_satd_list(Ctx2& e, int x0, int y0, int log2n, int cnt, const uint8_t* list) {
+  Work& w = e.w;
+  const int lsb = 2 * log2n - 4, lw = log2n - 2;               // log2 of the sub-blocks per block / per row
+  for (int it = e.lane; it < (cnt << lsb); it += GE_LANES) {
+    const int mode = list[it >> lsb], sb = it & ((1 << lsb) - 1), bx = (sb & ((1 << lw) - 1)) << 2, by = (sb >> lw) << 2;
+    int d[16];
+    for (int k = 0; k < 16; k++) d[k] = e.org(0, x0 + bx + (k & 3), y0 + by + (k >> 2)) - predicted(w, 0, log2n, mode, bx + (k & 3), by + (k >> 2));
+    GE_ATOMIC_ADD(&w.satd[mode], satd4(d));
+  }
+}
+
+// the lowest J x 16 over the modes of `set`, shifted left by 6 with the mode in the low bits (ties: the lower mode); every
+// lane gets it
+__device__ inline long long best_mode(const Ctx2& e, unsigned long long set, const int cand[3]) {
+  long long k = LLONG_MAX;
+  for (int m = e.lane; m < 35; m += GE_LANES)
+    if ((set >> m) & 1) k = min(k, ((((long long)e.w.satd[m] << 4) + (long long)e.a.lambda16 * mode_bits(m, cand)) << 6) | m);
+  for (int o = 16; o; o >>= 1) k = min(k, (long long)__shfl_xor_sync(0xffffffffu, k, o));
+  return k;
+}
+
+// best luma mode of the n x n PU at (x0, y0) on SATD + lambda * mode bits; returns the mode, *cost = its J (x16).
+// S = 0: all 35 modes.  S >= 1, coarse to fine: round 1 planar, DC, the angular modes 2, 6, .., 34 and the three MPM
+// candidates; round 2 the angular modes within 2 of round 1's best angular mode a* (clamped to 2..34), those not evaluated
+// yet.  Ties go to the lower mode number in both rounds.  S = 2 predicts from the source (open loop).
+template <int S>
+__device__ int search_mode(Ctx2& e, int x0, int y0, int log2n, long long* cost) {
+  Work& w = e.w;
+  gather_refs<S == 2>(e, 0, x0, y0, log2n);
+  unsigned long long done = (1ull << 35) - 1;                 // the modes evaluated
+  if constexpr (S == 0) {
+    for (int i = e.lane; i < 35; i += GE_LANES) w.satd[i] = 0;
+    GE_SYNC();
+    add_satd(e, x0, y0, log2n, 35, [](int m) { return m; });
+  } else {
+    // The candidate sets are bit masks held alike by every lane (no per-candidate serial work, nothing in local memory); each
+    // round's modes are listed in shared memory in mode order, one lane per mode, behind those of the rounds before.
+    uint8_t* list = static_cast<E1Work<S>&>(w).list;
+    int org[16];                                               // a 4x4 PU: its source samples, loaded once for both rounds
+    if (log2n == 2)
+      for (int k = 0; k < 16; k++) org[k] = e.org(0, x0 + (k & 3), y0 + (k >> 2));
+    int cand[3]; mpm_cand(e.ipm(), e.a.W >> 2, e.a.log2ctb, x0, y0, cand);
+    constexpr unsigned long long kCoarse = 0x444444447ull;     // planar, DC, angular 2, 6, .., 34
+    unsigned long long round = kCoarse | (1ull << cand[0]) | (1ull << cand[1]) | (1ull << cand[2]);
+    done = 0;
+    for (int i = e.lane; i < 35; i += GE_LANES) w.satd[i] = 0;
+    for (int r = 0; r < 2; r++) {
+      const int first = __popcll(done), cnt = __popcll(round);
+      for (int m = e.lane; m < 35; m += GE_LANES)
+        if ((round >> m) & 1) list[first + __popcll(round & ((1ull << m) - 1))] = (uint8_t)m;
+      done |= round;
+      GE_SYNC();
+      if (log2n == 2) {                                        // at most 14 modes a round: one lane each
+        if (e.lane < cnt) {
+          const int mode = list[first + e.lane];
+          int d[16];
+          for (int k = 0; k < 16; k++) d[k] = org[k] - predicted(w, 0, 2, mode, k & 3, k >> 2);
+          w.satd[mode] = satd4(d);
+        }
+      } else add_satd_list(e, x0, y0, log2n, cnt, list + first);
+      GE_SYNC();
+      if (r == 0) {                                            // round 2: the angular modes within 2 of round 1's best one
+        const int a = (int)(best_mode(e, done & ~3ull, cand) & 63);
+        round = 0;
+        for (int d = -2; d <= 2; d++) round |= 1ull << clip3(2, 34, a + d);
+        round &= ~done;
+      }
+    }
+    if (e.lane == 0) atomicAdd(e.a.work, (unsigned long long)__popcll(done));
+    const long long best = best_mode(e, done, cand);
+    *cost = best >> 6;
+    return (int)(best & 63);
+  }
+  if (e.lane == 0) atomicAdd(e.a.work, (unsigned long long)__popcll(done));
   GE_SYNC();
   if (e.lane == 0) {
     int cand[3]; mpm_cand(e.ipm(), e.a.W >> 2, e.a.log2ctb, x0, y0, cand);
     long long best = -1; int bm = 0;
     for (int m = 0; m < 35; m++) {
+      if (!((done >> m) & 1)) continue;
       const long long j = ((long long)w.satd[m] << 4) + (long long)e.a.lambda16 * mode_bits(m, cand);
       if (best < 0 || j < best) { best = j; bm = m; }
     }
@@ -230,64 +327,97 @@ __device__ void set_cu(Ctx2& e, int x0, int y0, int n, int v) {
   for (int i = e.lane; i < n8 * n8; i += GE_LANES) m[(size_t)((y0 >> 3) + i / n8) * (e.a.W >> 3) + (x0 >> 3) + i % n8] = (uint8_t)v;
   GE_SYNC();
 }
-// save / restore / invalidate the luma reconstruction and modes of an n x n region (decision pass)
+// save / restore / invalidate the luma reconstruction (Samples) and modes of an n x n region (decision pass)
+template <bool Samples>
 __device__ void region(Ctx2& e, int x0, int y0, int n, uint8_t* buf, int op /* 0 save, 1 restore, 2 mark not reconstructed */) {
   const int W = e.a.W, n4 = n >> 2; uint8_t* pl = e.plane(0); uint8_t* m = e.ipm(); uint8_t* d = e.dec();
-  for (int i = e.lane; i < n * n; i += GE_LANES) {
-    uint8_t* p = pl + (size_t)(y0 + i / n) * W + x0 + i % n;
-    if (op == 0) buf[i] = *p; else if (op == 1) *p = buf[i];
-  }
+  const int nm = Samples ? n * n : 0;                         // where the modes start in buf
+  if constexpr (Samples)
+    for (int i = e.lane; i < n * n; i += GE_LANES) {
+      uint8_t* p = pl + (size_t)(y0 + i / n) * W + x0 + i % n;
+      if (op == 0) buf[i] = *p; else if (op == 1) *p = buf[i];
+    }
   for (int i = e.lane; i < n4 * n4; i += GE_LANES) {
     const size_t k = (size_t)((y0 >> 2) + i / n4) * (W >> 2) + (x0 >> 2) + i % n4;
-    if (op == 0) buf[n * n + i] = m[k]; else if (op == 1) m[k] = buf[n * n + i]; else d[k] = 0;
+    if (op == 0) buf[nm + i] = m[k]; else if (op == 1) m[k] = buf[nm + i]; else d[k] = 0;
   }
   GE_SYNC();
 }
 
-// luma of one CU, closed loop; returns J x 16
+// open-loop decisions: the n x n luma block at (x0, y0) counts as reconstructed from here on (z-scan availability of the
+// PUs that follow), as code_tb marks it in closed loop
+__device__ void mark_coded(Ctx2& e, int x0, int y0, int n) {
+  const int n4 = n >> 2; uint8_t* d = e.dec();
+  for (int i = e.lane; i < n4 * n4; i += GE_LANES) d[(size_t)((y0 >> 2) + i / n4) * (e.a.W >> 2) + (x0 >> 2) + i % n4] = 1;
+  GE_SYNC();
+}
+
+// open-loop SATD of the 32x32 luma block at (x0, y0) predicted with `mode` from the source; marks it coded
+__device__ int satd_open(Ctx2& e, int x0, int y0, int mode) {
+  Work& w = e.w;
+  gather_refs<true>(e, 0, x0, y0, 5);
+  if (e.lane == 0) w.satd[mode] = 0;
+  GE_SYNC();
+  add_satd(e, x0, y0, 5, 1, [mode](int) { return mode; });
+  mark_coded(e, x0, y0, 32);
+  return w.satd[mode];
+}
+
+// luma of one CU: closed loop (S < 2: the CU's TBs reconstructed), or open loop (S = 2: the J of the mode search alone);
+// returns J x 16
+template <int S>
 __device__ long long eval_cu(Ctx2& e, int x0, int y0, int log2cb, bool nxn) {
   long long j = 0, jm;
+  if (e.lane == 0) atomicAdd(e.a.work + 1, 1ull);
   if (nxn) {
     for (int k = 0; k < 4; k++) {
       const int px = x0 + (k & 1) * 4, py = y0 + (k >> 1) * 4;
-      const int m = search_mode(e, px, py, 2, &jm);
+      const int m = search_mode<S>(e, px, py, 2, &jm);
       set_modes(e, px, py, 4, m);
-      code_tb(e, 0, px, py, 2, m, false);
+      if constexpr (S == 2) mark_coded(e, px, py, 4);
+      else code_tb(e, 0, px, py, 2, m, false);
       j += jm;
     }
     return j + e.a.lambda16;                                  // part_mode bin
   }
   const int lg = log2cb < 5 ? log2cb : 5;
-  const int m = search_mode(e, x0, y0, lg, &jm);              // a 64x64 CU: chosen on its first 32x32 block
+  const int m = search_mode<S>(e, x0, y0, lg, &jm);           // a 64x64 CU: chosen on its first 32x32 block
   set_modes(e, x0, y0, 1 << log2cb, m);
-  if (log2cb < 6) { code_tb(e, 0, x0, y0, log2cb, m, false); return jm; }
-  j = jm - ((long long)e.w.satd[m] << 4);
-  for (int k = 0; k < 4; k++) j += (long long)code_tb(e, 0, x0 + (k & 1) * 32, y0 + (k >> 1) * 32, 5, m, false) << 4;
-  return j;
+  if constexpr (S == 2) {
+    mark_coded(e, x0, y0, 1 << lg);
+    if (log2cb == 6)                                           // + the open-loop SATDs of the other three 32x32 blocks
+      for (int k = 1; k < 4; k++) j += (long long)satd_open(e, x0 + (k & 1) * 32, y0 + (k >> 1) * 32, m) << 4;
+    return jm + j;
+  } else {
+    if (log2cb < 6) { code_tb(e, 0, x0, y0, log2cb, m, false); return jm; }
+    j = jm - ((long long)e.w.satd[m] << 4);
+    for (int k = 0; k < 4; k++) j += (long long)code_tb(e, 0, x0 + (k & 1) * 32, y0 + (k >> 1) * 32, 5, m, false) << 4;
+    return j;
+  }
 }
 
-// decision pass: bottom-up quadtree, leaves the chosen luma reconstruction / modes / CU sizes; returns J x 16
+// decision pass: bottom-up quadtree, leaves the chosen luma reconstruction (closed loop) / modes / CU sizes; returns J x 16
 // (The quadtree walks are templates on the block size: no run-time recursion, so the stack size is known at compile time.)
-template <int L>
+template <int S, int L>
 __device__ long long decide(Ctx2& e, int x0, int y0, int depth) {
   const int n = 1 << L, log2cb = L;
   if (x0 + n > e.a.W || y0 + n > e.a.H) {                     // crosses the picture border: split implied
     long long j = 0;
     if constexpr (L > 3)
-      for (int k = 0; k < 4; k++) { const int x1 = x0 + (k & 1) * (n >> 1), y1 = y0 + (k >> 1) * (n >> 1); if (x1 < e.a.W && y1 < e.a.H) j += decide<L - 1>(e, x1, y1, depth + 1); }
+      for (int k = 0; k < 4; k++) { const int x1 = x0 + (k & 1) * (n >> 1), y1 = y0 + (k >> 1) * (n >> 1); if (x1 < e.a.W && y1 < e.a.H) j += decide<S, L - 1>(e, x1, y1, depth + 1); }
     return j;
   }
-  const long long j0 = eval_cu(e, x0, y0, log2cb, false);
-  uint8_t* buf = e.w.save[depth];
-  region(e, x0, y0, n, buf, 0);
-  region(e, x0, y0, n, buf, 2);
+  const long long j0 = eval_cu<S>(e, x0, y0, log2cb, false);
+  uint8_t* buf = static_cast<E1Work<S>&>(e.w).save[depth];
+  region<S != 2>(e, x0, y0, n, buf, 0);
+  region<S != 2>(e, x0, y0, n, buf, 2);
   long long j1;
-  if constexpr (L == 3) j1 = eval_cu(e, x0, y0, 3, true);
+  if constexpr (L == 3) j1 = eval_cu<S>(e, x0, y0, 3, true);
   else {
     j1 = e.a.lambda16;                                         // split_cu_flag
-    for (int k = 0; k < 4; k++) j1 += decide<L - 1>(e, x0 + (k & 1) * (n >> 1), y0 + (k >> 1) * (n >> 1), depth + 1);
+    for (int k = 0; k < 4; k++) j1 += decide<S, L - 1>(e, x0 + (k & 1) * (n >> 1), y0 + (k >> 1) * (n >> 1), depth + 1);
   }
-  if (j0 <= j1) { region(e, x0, y0, n, buf, 1); set_cu(e, x0, y0, n, log2cb); return j0; }
+  if (j0 <= j1) { region<S != 2>(e, x0, y0, n, buf, 1); set_cu(e, x0, y0, n, log2cb); return j0; }
   if (log2cb == 3) set_cu(e, x0, y0, 8, 3 | CU_NXN);
   return j1;
 }
@@ -335,13 +465,14 @@ __device__ inline void publish(unsigned* p, unsigned v, int lane) {
   if (lane == 0) { __threadfence(); atomicExch(p, v); }
 }
 
+template <int S>
 __device__ void e1_row(const Args& a, Work& w, int p, int ry, int lane) {
   Ctx2 e{a, p, lane, w};
   const size_t row = (size_t)p * a.hctb + ry;
   for (int rx = 0; rx < a.wctb; rx++) {
     if (ry > 0) wait_for(a.progress + row - 1, (unsigned)min(rx + 2, a.wctb), lane);
     const int x0 = rx << a.log2ctb, y0 = ry << a.log2ctb;
-    if (a.log2ctb == 6) decide<6>(e, x0, y0, 0); else decide<5>(e, x0, y0, 0);
+    if (a.log2ctb == 6) decide<S, 6>(e, x0, y0, 0); else decide<S, 5>(e, x0, y0, 0);
     {                                                          // the final pass sees the CTB's blocks appear in decoding order again
       const int w4 = min(1 << a.log2ctb, a.W - x0) >> 2, h4 = min(1 << a.log2ctb, a.H - y0) >> 2;
       for (int i = lane; i < w4 * h4; i += GE_LANES) e.dec()[(size_t)((y0 >> 2) + i / w4) * (a.W >> 2) + (x0 >> 2) + i % w4] = 0;
@@ -480,14 +611,15 @@ __device__ void e2_row(const Args& a, uint8_t* ctx, int p, int ry, int lane) {
   }
 }
 
+template <int S>
 __global__ void __launch_bounds__(32) e1_kernel(Args a) {
-  __shared__ Work w;
+  __shared__ E1Work<S> w;
   __shared__ unsigned t;
   if (threadIdx.x == 0) t = atomicAdd(a.ticket, 1u);
   __syncwarp();
   const unsigned row = t;
   __syncwarp();
-  e1_row(a, w, (int)(row / a.hctb), (int)(row % a.hctb), threadIdx.x);
+  e1_row<S>(a, w, (int)(row / a.hctb), (int)(row % a.hctb), threadIdx.x);
 }
 
 __global__ void __launch_bounds__(32) e2_kernel(Args a) {
@@ -522,7 +654,7 @@ struct b200_gpu_encoder {
   b200::DevBuf<uint8_t> src, rec, ipm4, dec4, cu8, wpp_ctx, ss, packed;
   b200::DevBuf<int16_t> coef;
   b200::DevBuf<unsigned> sync, ss_len;
-  b200::DevBuf<unsigned long long> off;
+  b200::DevBuf<unsigned long long> off, counters;
   b200::DevBuf<b200::genc::Pic> pics;
   std::vector<std::vector<uint8_t>> out;
   b200_hevc_enc_params params{};
@@ -539,6 +671,7 @@ int validate(const b200_hevc_enc_params* p, int n, const b200_planes* pics) {
   if (!p || !pics) return set_error(B200_E_INVALID, "null argument");
   if (n <= 0) return set_error(B200_E_INVALID, "picture count %d", n);
   if (p->width < 8 || p->height < 8 || p->width > 16384 || p->height > 16384) return set_error(B200_E_INVALID, "size %dx%d", p->width, p->height);
+  if (p->speed < 0 || p->speed > 2) return set_error(B200_E_INVALID, "speed %d: 0, 1 or 2", p->speed);
   if (p->bit_depth != 8) return set_error(B200_E_UNSUPPORTED, "bit_depth %d: the GPU encoder codes 8-bit pictures", p->bit_depth);
   if (p->chroma_format_idc != 0 && p->chroma_format_idc != 1) return set_error(B200_E_UNSUPPORTED, "chroma_format_idc %d: 4:2:0 and 4:0:0 only", p->chroma_format_idc);
   if (p->log2_ctb_size != 5 && p->log2_ctb_size != 6) return set_error(B200_E_UNSUPPORTED, "log2_ctb_size %d: 5 or 6", p->log2_ctb_size);
@@ -588,12 +721,13 @@ int encode(b200_gpu_encoder* e, const b200_hevc_enc_params* p, int n, const Pic*
   if ((rc = e->rec.reserve(n * pic_samples, false)) || (rc = e->coef.reserve(n * pic_samples, false)) || (rc = e->ipm4.reserve(n * map4, false)) ||
       (rc = e->dec4.reserve(n * map4, false)) || (rc = e->cu8.reserve(n * map8, false)) || (rc = e->wpp_ctx.reserve(rows * syn::CTX_COUNT, false)) ||
       (rc = e->ss.reserve(rows * cap, false)) || (rc = e->sync.reserve(2 * rows + 3, false)) || (rc = e->ss_len.reserve(rows)) ||
-      (rc = e->off.reserve(rows)) || (rc = e->pics.reserve(n)))
+      (rc = e->off.reserve(rows)) || (rc = e->pics.reserve(n)) || (rc = e->counters.reserve(2)))
     return rc;
   for (int i = 0; i < n; i++) e->pics.h[i] = host_pics[i];
   B200_CUDA_CHECK(cudaMemcpyAsync(e->pics.d, e->pics.h, n * sizeof(Pic), cudaMemcpyHostToDevice, s));
   B200_CUDA_CHECK(cudaMemsetAsync(e->dec4.d, 0, n * map4, s));
   B200_CUDA_CHECK(cudaMemsetAsync(e->sync.d, 0, (2 * rows + 3) * sizeof(unsigned), s));
+  B200_CUDA_CHECK(cudaMemsetAsync(e->counters.d, 0, 2 * sizeof(unsigned long long), s));
   Args a{};
   a.pics = e->pics.d; a.n = n; a.W = W; a.H = H; a.Wc = Wc; a.Hc = Hc; a.sw = p->width; a.sh = p->height;
   a.cfmt = cfmt; a.log2ctb = log2ctb; a.wctb = wctb; a.hctb = hctb; a.max_th_depth = p->max_transform_hierarchy_depth_intra;
@@ -604,15 +738,20 @@ int encode(b200_gpu_encoder* e, const b200_hevc_enc_params* p, int n, const Pic*
   a.rec = e->rec.d; a.coef = e->coef.d; a.pic_samples = pic_samples; a.ipm4 = e->ipm4.d; a.dec4 = e->dec4.d; a.map4 = map4;
   a.cu8 = e->cu8.d; a.map8 = map8;
   a.progress = e->sync.d; a.progress2 = e->sync.d + rows; a.ticket = e->sync.d + 2 * rows; a.error = e->sync.d + 2 * rows + 2;
-  a.wpp_ctx = e->wpp_ctx.d; a.ss = e->ss.d; a.ss_cap = cap; a.ss_len = e->ss_len.d;
+  a.wpp_ctx = e->wpp_ctx.d; a.ss = e->ss.d; a.ss_cap = cap; a.ss_len = e->ss_len.d; a.work = e->counters.d;
   B200_CUDA_CHECK(cudaEventRecord(e->ev[0], s));
-  e1_kernel<<<(unsigned)rows, 32, 0, s>>>(a);
+  switch (p->speed) {
+    case 0: e1_kernel<0><<<(unsigned)rows, 32, 0, s>>>(a); break;
+    case 1: e1_kernel<1><<<(unsigned)rows, 32, 0, s>>>(a); break;
+    default: e1_kernel<2><<<(unsigned)rows, 32, 0, s>>>(a); break;
+  }
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaEventRecord(e->ev[1], s));
   e2_kernel<<<(unsigned)rows, 32, 0, s>>>(a);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaEventRecord(e->ev[2], s));
   B200_CUDA_CHECK(cudaMemcpyAsync(e->ss_len.h, e->ss_len.d, rows * sizeof(unsigned), cudaMemcpyDeviceToHost, s));
+  B200_CUDA_CHECK(cudaMemcpyAsync(e->counters.h, e->counters.d, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
   unsigned err = 0;
   B200_CUDA_CHECK(cudaMemcpyAsync(&err, a.error, sizeof(unsigned), cudaMemcpyDeviceToHost, s));
   B200_CUDA_CHECK(cudaStreamSynchronize(s));
@@ -659,6 +798,7 @@ int encode(b200_gpu_encoder* e, const b200_hevc_enc_params* p, int n, const Pic*
   st.total_ms = std::chrono::duration<double, std::milli>(t2 - t0).count();
   st.bytes = 0; for (auto& o : e->out) st.bytes += o.size();
   st.ctus = (uint64_t)rows * wctb; st.pictures = (uint64_t)n;
+  st.mode_evaluations = e->counters.h[0]; st.cu_evaluations = e->counters.h[1];
   e->params = *p; e->n = n; e->W = W; e->H = H; e->cfmt = cfmt; e->rec_first = 0; e->ready = true;
   return B200_OK;
 }
@@ -796,6 +936,7 @@ int grid_encode(b200_gpu_encoder* e, const b200_rgb_image* in, int tw, int th, c
     b200_gpu_encode_stats& t = e->stats;
     t.analyse_ms += st.analyse_ms; t.entropy_ms += st.entropy_ms; t.framing_ms += st.framing_ms;
     t.bytes += st.bytes; t.ctus += st.ctus; t.pictures += st.pictures;
+    t.mode_evaluations += st.mode_evaluations; t.cu_evaluations += st.cu_evaluations;
   }
   e->stats.total_ms = std::chrono::duration<double, std::milli>(clk::now() - t0).count();
   if (info) {
@@ -831,6 +972,15 @@ int b200_gpu_encode_check(const b200_hevc_enc_params* p, int n, const b200_plane
 
 size_t b200_gpu_encoder_substream_capacity(int width, int log2_ctb_size, int chroma_format_idc) {
   return b200::genc::substream_capacity(width, log2_ctb_size, chroma_format_idc);
+}
+
+int b200_gpu_encoder_e1_warps_per_sm(int speed, int* warps) {
+  using namespace b200;
+  if (!warps) return set_error(B200_E_INVALID, "null argument");
+  if (speed < 0 || speed > 2) return set_error(B200_E_INVALID, "speed %d: 0, 1 or 2", speed);
+  const void* k = speed == 0 ? (const void*)genc::e1_kernel<0> : speed == 1 ? (const void*)genc::e1_kernel<1> : (const void*)genc::e1_kernel<2>;
+  B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(warps, k, 32, 0));
+  return B200_OK;
 }
 
 int b200_gpu_encode_intra_device(b200_gpu_encoder* enc, const b200_hevc_enc_params* p, int n, const b200_planes* pics, void* stream) {

@@ -687,6 +687,7 @@ const b200h_encoder_plugin g_encoder_plugin = {
 struct GpuEncInstance : EncInstance {
   b200_gpu_encoder* gpu = nullptr;
   int seq_batch = 0;                                              // "sequence-batch": 0 = automatic
+  int speed = 0;                                                  // "speed": b200_hevc_enc_params::speed
   int batch_cap = 0;                                              // frames per GPU call for the running sequence
   b200_hevc_enc_params batch_prm{};                               // parameters of the queued frames
   std::vector<uintptr_t> pend;                                    // frame numbers of the queued frames, in staging order
@@ -721,8 +722,12 @@ void init_gpu_params() {
   auto& b = g_gpu_params[4];
   b.version = 2; b.name = "sequence-batch"; b.type = 1; b.integer.default_value = 0; b.integer.have_minimum_maximum = 1;
   b.integer.minimum = 0; b.integer.maximum = kMaxSeqBatch; b.has_default = 1;
-  for (int i = 0; i < 5; i++) g_gpu_param_ptrs[i] = &g_gpu_params[i];
-  g_gpu_param_ptrs[5] = nullptr;
+  // mode-decision speed of the GPU encoder (b200_hevc_enc_params::speed): 0 = full search, 1 = coarse to fine, 2 = also open loop
+  auto& sp = g_gpu_params[5];
+  sp.version = 2; sp.name = "speed"; sp.type = 1; sp.integer.default_value = 0; sp.integer.have_minimum_maximum = 1;
+  sp.integer.minimum = 0; sp.integer.maximum = 2; sp.has_default = 1;
+  for (int i = 0; i < 6; i++) g_gpu_param_ptrs[i] = &g_gpu_params[i];
+  g_gpu_param_ptrs[6] = nullptr;
 }
 const b200h_encoder_parameter** genc_list(void*) { std::call_once(g_gpu_params_once, init_gpu_params); return g_gpu_param_ptrs; }
 b200h_error genc_set_int(void* p, const char* n, int v) {
@@ -733,10 +738,16 @@ b200h_error genc_set_int(void* p, const char* n, int v) {
     static_cast<GpuEncInstance*>((EncInstance*)p)->seq_batch = v;
     return ok_err();
   }
+  if (!strcmp(n, "speed")) {
+    if (v < 0 || v > 2) return make_err(B200H_ERR_USAGE, 0, "speed out of range (0..2)");
+    static_cast<GpuEncInstance*>((EncInstance*)p)->speed = v;
+    return ok_err();
+  }
   return enc_set_int(p, n, v);
 }
 b200h_error genc_get_int(void* p, const char* n, int* v) {
   if (!strcmp(n, "sequence-batch")) { *v = static_cast<GpuEncInstance*>((EncInstance*)p)->seq_batch; return ok_err(); }
+  if (!strcmp(n, "speed")) { *v = static_cast<GpuEncInstance*>((EncInstance*)p)->speed; return ok_err(); }
   return enc_get_int(p, n, v);
 }
 
@@ -746,6 +757,7 @@ b200h_error gpu_input(GpuEncInstance* e, const b200h_image* image, EncInput& in)
   if (err.code) return err;
   if (in.prm.bit_depth != 8) return make_err(B200H_ERR_ENCODER_PLUGIN, B200H_SUBERR_UNSUPPORTED_BIT_DEPTH, "the GPU encoder codes 8-bit pictures");
   in.prm.sao = 0; in.prm.sign_data_hiding = 0; in.prm.cu_qp_delta = 0; in.prm.wpp = 1;
+  in.prm.speed = e->speed;
   return ok_err();
 }
 b200h_error gpu_code(GpuEncInstance* e, const b200_hevc_enc_params& prm, int n, const b200_planes* pl) {
@@ -776,21 +788,25 @@ b200h_error genc_encode(void* p, const b200h_image* image, int /*image_class*/) 
 // ---- GPU sequences
 // Staging bytes of one queued frame: Y, then Cb and Cr, each packed at its width.
 size_t frame_bytes(int w, int h, bool mono) { return (size_t)w * h + (mono ? 0 : 2 * (size_t)((w + 1) >> 1) * ((h + 1) >> 1)); }
-// Automatic batch: enough frames for about one full wave of E1 (one warp per picture CTB row; 6 resident E1 warps per SM, set by
-// its 33460 bytes of static shared memory per warp), capped so that the staging stays within kSeqStagingBudget.
+// Automatic batch: enough frames for about one full wave of E1 (one warp per picture CTB row; at speeds 0 and 1, 6 resident E1
+// warps per SM, set by their 33460 bytes of static shared memory per warp; speed 2's E1 needs less, so the runtime is asked),
+// capped so that the staging stays within kSeqStagingBudget.
 constexpr int kE1WarpsPerSm = 6;
 constexpr size_t kSeqStagingBudget = size_t(256) << 20;
 int seq_batch_frames(const GpuEncInstance* e, const b200_hevc_enc_params& prm) {
   const size_t fb = frame_bytes(prm.width, prm.height, prm.chroma_format_idc == 0);
   const int budget = (int)std::max<size_t>(1, std::min<size_t>(kMaxSeqBatch, kSeqStagingBudget / fb));
   if (e->seq_batch > 0) return std::min(e->seq_batch, budget);
-  int dev = 0, sms = 0;
+  int dev = 0, sms = 0, warps = kE1WarpsPerSm;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) {
     cudaGetLastError();
     sms = 132;                                                    // H100 SXM; the encode call reports a missing device
+  } else if (prm.speed == 2 && (b200_gpu_encoder_e1_warps_per_sm(2, &warps) != B200_OK || warps <= 0)) {
+    cudaGetLastError();
+    warps = kE1WarpsPerSm;
   }
   const int ctb = 1 << prm.log2_ctb_size, rows = (((prm.height + 7) & ~7) + ctb - 1) / ctb;
-  return std::max(1, std::min(budget, sms * kE1WarpsPerSm / rows));
+  return std::max(1, std::min(budget, sms * warps / rows));
 }
 // code the queued frames in one GPU call; their access units join `coded` in frame order
 b200h_error gpu_flush(GpuEncInstance* e) {

@@ -18,7 +18,7 @@ class EncParams(C.Structure):
         "slice_tc_offset_div2", "mode_decision", "split_threshold", "still_picture", "vui_present",
         "colour_description_present", "colour_primaries", "transfer_characteristics", "matrix_coefficients", "full_range")] + \
         [("seed", C.c_uint32), ("scaling_lists", C.c_int), ("pcm", C.c_int), ("transquant_bypass", C.c_int), ("tile_cols", C.c_int), ("tile_rows", C.c_int), ("tiles_uniform", C.c_int),
-         ("loop_filter_across_tiles", C.c_int), ("slice_per_tile", C.c_int)]
+         ("loop_filter_across_tiles", C.c_int), ("slice_per_tile", C.c_int), ("speed", C.c_int)]
 
 
 def default_params(**kw) -> EncParams:
@@ -62,7 +62,8 @@ def encode_intra(y, cb=None, cr=None, **kw) -> bytes:
 
 class GpuEncodeStats(C.Structure):
     _fields_ = [("analyse_ms", C.c_double), ("entropy_ms", C.c_double), ("framing_ms", C.c_double), ("total_ms", C.c_double),
-                ("bytes", C.c_uint64), ("ctus", C.c_uint64), ("pictures", C.c_uint64)]
+                ("bytes", C.c_uint64), ("ctus", C.c_uint64), ("pictures", C.c_uint64),
+                ("mode_evaluations", C.c_uint64), ("cu_evaluations", C.c_uint64)]
 
 
 # What the GPU encoder codes (b200_heif.h): no SAO, sign hiding or cu_qp_delta, one WPP sub-stream per CTB row.
@@ -130,7 +131,8 @@ class GpuEncoder:
     """HEVC intra encoder on the GPU (b200_gpu_encoder_*): N same-sized 8-bit 4:2:0 or 4:0:0 pictures per call.
 
     encode(pictures, **params) takes a list of (y, cb, cr) tuples -- numpy uint8 host planes or uint8 CUDA tensors,
-    cb = cr = None for monochrome -- and returns one access unit (length-prefixed NALs) per picture."""
+    cb = cr = None for monochrome -- and returns one access unit (length-prefixed NALs) per picture.  speed=0 (default), 1 or
+    2 selects the mode decision (b200_heif.h): 1 searches at most 18 of the 35 luma modes per PU, 2 also decides open loop."""
 
     def __init__(self):
         l = self._l = _lib.lib()
@@ -142,6 +144,7 @@ class GpuEncoder:
         l.b200_gpu_encoder_output.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)]
         l.b200_gpu_encoder_read_recon.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]
         l.b200_gpu_encoder_get_stats.argtypes = [C.c_void_p, C.POINTER(GpuEncodeStats)]
+        l.b200_gpu_encoder_e1_warps_per_sm.argtypes = [C.c_int, C.POINTER(C.c_int)]
         self._h = C.c_void_p()
         _lib.check(l.b200_gpu_encoder_create(C.byref(self._h)))
         self._shape = None
@@ -238,6 +241,12 @@ class GpuEncoder:
         s = GpuEncodeStats()
         _lib.check(self._l.b200_gpu_encoder_get_stats(self._h, C.byref(s)))
         return s
+
+    def e1_warps_per_sm(self, speed=0) -> int:
+        """Resident analysis (E1) warps per SM of the current device at this speed."""
+        n = C.c_int()
+        _lib.check(self._l.b200_gpu_encoder_e1_warps_per_sm(speed, C.byref(n)))
+        return n.value
 
 
 def synthetic_image(seed: int, width: int, height: int, bit_depth: int = 8, chroma=True):
