@@ -318,6 +318,9 @@ class Encoder {
 
   const std::vector<uint16_t>& recon(int c) const { return rec[c]; }
   int coded_w() const { return W; } int coded_h() const { return H; }
+  // test-only: the levels of the first `count` transform-coded blocks of 8x8 and larger of every component become the
+  // top-left n x n of `pattern` (32 x 32, raster), whatever quantisation gave; the reconstruction follows those levels
+  void force_levels(const int16_t* pattern, int count) { forced = pattern; forced_left[0] = forced_left[1] = forced_left[2] = count; }
 
  private:
   b200_hevc_enc_params P;
@@ -337,6 +340,7 @@ class Encoder {
   int cu_x0 = 0, cu_y0 = 0;
   sl::Lists sl_lists; sl::Factors sl_f; uint8_t sl_kind[4][6] = {}; bool sl_on = false;
   int pcm_bd_y = 8, pcm_bd_c = 8; bool cu_bypass = false;
+  const int16_t* forced = nullptr; int forced_left[3] = {0, 0, 0};
 
   int scaling_factor(int c, int log2n, int pos) const {          // m[x][y] of 8.6.4.2 for raster position pos of an n x n block
     if (!sl_on) return 16;
@@ -555,6 +559,11 @@ class Encoder {
     forward(res, coef, log2n, dst4, r.tskip);
     int qp = c == 0 ? qg_target_qp + 6 * (bd - 8) : chroma_qp(qg_target_qp + (c == 1 ? P.cb_qp_offset : P.cr_qp_offset) + (P.slice_chroma_qp_offsets ? (c == 1 ? P.slice_cb_qp_offset : P.slice_cr_qp_offset) : 0), cfmt, bd);
     r.cbf = quantise(coef, r.lev, log2n, qp, r.scan);
+    if (forced && log2n >= 3 && forced_left[c] > 0) {        // test-only: the caller's levels instead of the quantised ones
+      forced_left[c]--;
+      r.cbf = false;
+      for (int y = 0; y < n; y++) for (int x = 0; x < n; x++) { r.lev[y * n + x] = forced[y * 32 + x]; r.cbf |= forced[y * 32 + x] != 0; }
+    }
     // NOTE: the QP used here (qg_target_qp) is only valid if a cu_qp_delta can still be sent (or already
     // was); the caller re-runs with the predicted QP when neither holds.
     uint16_t* rp = rec[c].data();
@@ -823,9 +832,14 @@ void b200_hevc_enc_params_default(b200_hevc_enc_params* p) {
   p->still_picture = 1; p->vui_present = 0; p->colour_primaries = 2; p->transfer_characteristics = 2; p->matrix_coefficients = 2;
 }
 
-int b200_hevc_encode_intra(const b200_hevc_enc_params* p, const void* y, const void* cb, const void* cr, size_t y_stride,
-                           size_t c_stride, uint8_t** out_data, size_t* out_size) {
-  using namespace b200;
+}  // extern "C"
+
+namespace b200 {
+namespace enc {
+// b200_hevc_encode_intra; forced / nforced: Encoder::force_levels (test-only), rec[3]: the encoder's reconstruction of the
+// coded size (rounded up to 8), or nullptr
+static int encode_intra(const b200_hevc_enc_params* p, const void* y, const void* cb, const void* cr, size_t y_stride, size_t c_stride,
+                        uint8_t** out_data, size_t* out_size, const int16_t* forced, int nforced, uint16_t* const rec[3]) {
   if (!p || !y || !out_data || !out_size) return set_error(B200_E_INVALID, "null argument");
   if (p->width < 8 || p->height < 8 || p->width > 16384 || p->height > 16384) return set_error(B200_E_INVALID, "size %dx%d", p->width, p->height);
   if (p->bit_depth < 8 || p->bit_depth > 12) return set_error(B200_E_UNSUPPORTED, "bit depth %d", p->bit_depth);
@@ -844,16 +858,90 @@ int b200_hevc_encode_intra(const b200_hevc_enc_params* p, const void* y, const v
       tmp[c][(size_t)yy * w + xx] = bps == 1 ? ((const uint8_t*)in[c])[yy * st + xx] : ((const uint16_t*)((const uint8_t*)in[c] + yy * st))[xx];
     src[c] = tmp[c].data(); stride[c] = w;
   }
-  enc::Encoder e(*p, src, stride);
+  Encoder e(*p, src, stride);
+  if (forced) e.force_levels(forced, nforced);
   std::vector<uint8_t> out;
   e.encode(out);
   *out_data = (uint8_t*)malloc(out.size() ? out.size() : 1);
   if (!*out_data) return set_error(B200_E_INVALID, "out of memory");
   memcpy(*out_data, out.data(), out.size());
   *out_size = out.size();
+  if (rec)
+    for (int c = 0; c < (p->chroma_format_idc ? 3 : 1); c++) if (rec[c]) memcpy(rec[c], e.recon(c).data(), e.recon(c).size() * 2);
   return B200_OK;
 }
 
+}  // namespace enc
+}  // namespace b200
+
+extern "C" {
+
+int b200_hevc_encode_intra(const b200_hevc_enc_params* p, const void* y, const void* cb, const void* cr, size_t y_stride,
+                           size_t c_stride, uint8_t** out_data, size_t* out_size) {
+  return b200::enc::encode_intra(p, y, cb, cr, y_stride, c_stride, out_data, out_size, nullptr, 0, nullptr);
+}
+
 void b200_free(void* p) { free(p); }
+
+// Test-only entry points (declared by the tests, not in include/b200_heif.h).
+//
+// b200_hevc_encode_intra, except that the levels of the first `count` transform-coded blocks of 8x8 and larger of every
+// component are the top-left n x n of `pattern` (32 x 32 raster int16) instead of the quantised ones.  Sign-data hiding must be
+// off: it would drop signs of the pattern.  rec_*: the encoder's reconstruction before the in-loop filters, coded size
+// (width and height rounded up to 8; chroma planes subsampled from that), uint16.
+int b200_debug_hevc_encode_forced_levels(const b200_hevc_enc_params* p, const void* y, const void* cb, const void* cr, size_t y_stride,
+                                         size_t c_stride, const int16_t* pattern, int count, uint8_t** out_data, size_t* out_size,
+                                         uint16_t* rec_y, uint16_t* rec_cb, uint16_t* rec_cr) {
+  using namespace b200;
+  if (!p || !pattern || !rec_y || (p->chroma_format_idc && (!rec_cb || !rec_cr))) return set_error(B200_E_INVALID, "null argument");
+  if (count < 0) return set_error(B200_E_INVALID, "count %d", count);
+  if (p->sign_data_hiding) return set_error(B200_E_INVALID, "forced levels need sign_data_hiding = 0");
+  uint16_t* const rec[3] = {rec_y, rec_cb, rec_cr};
+  return enc::encode_intra(p, y, cb, cr, y_stride, c_stride, out_data, out_size, pattern, count, rec);
+}
+
+// The transform chain of the host encoder, element by element on n given blocks: prm[i * DT_FIELDS ..] = (log2 size 2..5,
+// DST 0/1 (4x4 only), bit depth 8..12, qp 0 .. 51 + 6 * (bd - 8), scaling factor 1..255), in[i * 1024 ..] = the block's
+// input (n x n raster, int16 range).  out[(i * 6 + st) * 1024 ..] = stage st applied to that input: fwd_col (row k, column
+// x), fwd_row (row y, column k), quant_level, dequant (the inputs as levels), inv_col, inv_row.
+int b200_debug_enc_transform_host(int n, const int32_t* prm, const int32_t* in, int32_t* out) {
+  using namespace b200;
+  if (n < 1 || n > 65536 || !prm || !in || !out) return set_error(B200_E_INVALID, "enc_transform: %d blocks, null argument", n);
+  for (int i = 0; i < n; i++)
+    if (const char* why = enc::debug_transform_args(prm + (size_t)i * enc::DT_FIELDS, in + (size_t)i * 1024)) return set_error(B200_E_INVALID, "enc_transform: block %d: %s", i, why);
+  for (int i = 0; i < n; i++) {
+    const int32_t* p = prm + (size_t)i * enc::DT_FIELDS;
+    const int lg = p[enc::DT_LOG2N], nn = 1 << lg;
+    for (int st = 0; st < enc::DT_STAGES; st++)
+      for (int e = 0; e < nn * nn; e++) out[((size_t)i * enc::DT_STAGES + st) * 1024 + e] = enc::debug_transform_stage(st, p, in + (size_t)i * 1024, e >> lg, e & (nn - 1));
+  }
+  return B200_OK;
+}
+
+// Intra prediction of the host encoder on n given blocks: prm[i * DP_FIELDS ..] = (log2 size 2..5, bit depth 8..12, luma (DC
+// and mode 10 / 26 edge filters), plane filtered (luma, or chroma in 4:4:4), strong intra smoothing), refs[i * 129 ..] = the
+// neighbours r[0 .. 4n] of b200_hevc_enc_recon.h, -1 = unavailable.  Outputs: rf[i * 258 ..] = r after substitute_refs and
+// filter_refs of it (129 each), pred[(i * 35 + mode) * 1024 ..] = the n x n prediction of every mode, raster.
+int b200_debug_enc_predict_host(int n, const int32_t* prm, const int16_t* refs, int16_t* rf, int32_t* pred) {
+  using namespace b200;
+  if (n < 1 || n > 65536 || !prm || !refs || !rf || !pred) return set_error(B200_E_INVALID, "enc_predict: %d blocks, null argument", n);
+  for (int i = 0; i < n; i++)
+    if (const char* why = enc::debug_predict_args(prm + (size_t)i * enc::DP_FIELDS, refs + (size_t)i * 129)) return set_error(B200_E_INVALID, "enc_predict: block %d: %s", i, why);
+  for (int i = 0; i < n; i++) {
+    const int32_t* p = prm + (size_t)i * enc::DP_FIELDS;
+    const int lg = p[enc::DP_LOG2N], bd = p[enc::DP_BD], nn = 1 << lg;
+    int16_t* r = rf + (size_t)i * 258; int16_t* f = r + 129;
+    memcpy(r, refs + (size_t)i * 129, 129 * 2);
+    enc::substitute_refs(r, nn, bd);
+    enc::filter_refs(r, f, lg, p[enc::DP_STRONG] != 0, bd);
+    const int dc = enc::dc_value(r, lg);
+    for (int mode = 0; mode < 35; mode++) {
+      const bool filt = enc::refs_filtered(p[enc::DP_PLANE] != 0, mode, lg);
+      for (int e = 0; e < nn * nn; e++)
+        pred[((size_t)i * 35 + mode) * 1024 + e] = enc::pred_sample(filt ? f : r, dc, lg, mode, e & (nn - 1), e >> lg, p[enc::DP_LUMA] != 0, (1 << bd) - 1);
+    }
+  }
+  return B200_OK;
+}
 
 }  // extern "C"

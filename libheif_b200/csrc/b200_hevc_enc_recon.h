@@ -170,5 +170,45 @@ B200_HD inline int dequant(int level, int m, int qp, int log2n, int bd) {
   return (int)(t < -32768 ? -32768 : (t > 32767 ? 32767 : t));
 }
 
+// ------------------------------------------------------------------------------------------ test-only entry points
+// b200_debug_enc_transform_{host,device} and b200_debug_enc_predict_{host,device} run the functions above on given blocks
+// (b200_hevc_enc.cc on the host, b200_hevc_gpu_enc.cu on the device).  These check one block's arguments: nullptr when they
+// are in the functions' domain, else what is wrong.
+enum { DT_LOG2N, DT_DST4, DT_BD, DT_QP, DT_M, DT_FIELDS };       // transform block: [DT_FIELDS] parameters + 1024 inputs
+enum { DP_LOG2N, DP_BD, DP_LUMA, DP_PLANE, DP_STRONG, DP_FIELDS };   // prediction block: [DP_FIELDS] parameters + 129 neighbours
+enum { DT_STAGES = 6 };                                           // fwd_col, fwd_row, quant_level, dequant, inv_col, inv_row
+inline const char* debug_transform_args(const int32_t* p, const int32_t* in) {
+  const int lg = p[DT_LOG2N], bd = p[DT_BD];
+  if (lg < 2 || lg > 5) return "log2 size";
+  if (bd < 8 || bd > 12) return "bit depth";
+  if (p[DT_DST4] != 0 && !(p[DT_DST4] == 1 && lg == 2)) return "DST (4x4 only)";
+  if (p[DT_QP] < 0 || p[DT_QP] > 51 + 6 * (bd - 8)) return "qp";
+  if (p[DT_M] < 1 || p[DT_M] > 255) return "scaling factor";
+  for (int i = 0; i < (1 << (2 * lg)); i++) if (in[i] < -32768 || in[i] > 32767) return "input outside int16";
+  return nullptr;
+}
+inline const char* debug_predict_args(const int32_t* p, const int16_t* refs) {
+  const int lg = p[DP_LOG2N], bd = p[DP_BD];
+  if (lg < 2 || lg > 5) return "log2 size";
+  if (bd < 8 || bd > 12) return "bit depth";
+  for (int f = DP_LUMA; f <= DP_STRONG; f++) if (p[f] != 0 && p[f] != 1) return "flag";
+  if (p[DP_LUMA] && !p[DP_PLANE]) return "luma without neighbour filtering";
+  for (int i = 0; i <= 4 << lg; i++) if (refs[i] < -1 || refs[i] >= (1 << bd)) return "neighbour outside -1 .. maxv";
+  return nullptr;
+}
+// element (row r, column c) of stage st on the n x n block a with the parameters p
+B200_HD inline int debug_transform_stage(int st, const int32_t* p, const int* a, int r, int c) {
+  const int lg = p[DT_LOG2N], bd = p[DT_BD], qp = p[DT_QP];
+  const bool dst4 = p[DT_DST4] != 0;
+  switch (st) {
+    case 0: return fwd_col(a, dst4, lg, r, c, bd);
+    case 1: return fwd_row(a, dst4, lg, r, c);
+    case 2: return quant_level(a[(r << lg) + c], qp, lg, bd);
+    case 3: return dequant(a[(r << lg) + c], p[DT_M], qp, lg, bd);
+    case 4: return inv_col(a, dst4, lg, r, c);
+    default: return inv_row(a, dst4, lg, r, c, bd);
+  }
+}
+
 }  // namespace enc
 }  // namespace b200

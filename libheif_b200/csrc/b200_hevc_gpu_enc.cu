@@ -640,6 +640,38 @@ __global__ void pack_kernel(const uint8_t* ss, size_t cap, const unsigned* len, 
   for (unsigned i = threadIdx.x; i < len[row]; i += blockDim.x) d[i] = s[i];
 }
 
+// test-only (b200_debug_enc_transform_device): CTA (block i, stage st), one thread per output element
+__global__ void debug_transform_kernel(const int* prm, const int* in, int* out) {
+  const int i = blockIdx.x, st = blockIdx.y;
+  const int* p = prm + i * enc::DT_FIELDS;
+  const int lg = p[enc::DT_LOG2N], n = 1 << lg;
+  for (int e = threadIdx.x; e < n * n; e += blockDim.x)
+    out[((size_t)i * enc::DT_STAGES + st) * 1024 + e] = enc::debug_transform_stage(st, p, in + (size_t)i * 1024, e >> lg, e & (n - 1));
+}
+
+// test-only (b200_debug_enc_predict_device): one CTA per block; thread 0 substitutes and filters the neighbours, every
+// thread predicts samples of all 35 modes
+__global__ void debug_predict_kernel(const int* prm, const int16_t* refs, int16_t* rf, int* pred) {
+  __shared__ int16_t r[129], f[129];
+  __shared__ int dc;
+  const int i = blockIdx.x;
+  const int* p = prm + i * enc::DP_FIELDS;
+  const int lg = p[enc::DP_LOG2N], bd = p[enc::DP_BD], n = 1 << lg;
+  if (threadIdx.x == 0) {
+    for (int k = 0; k < 129; k++) r[k] = refs[(size_t)i * 129 + k];
+    enc::substitute_refs(r, n, bd);
+    enc::filter_refs(r, f, lg, p[enc::DP_STRONG] != 0, bd);
+    dc = enc::dc_value(r, lg);
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < 129; k += blockDim.x) { rf[(size_t)i * 258 + k] = r[k]; rf[(size_t)i * 258 + 129 + k] = f[k]; }
+  for (int e = threadIdx.x; e < 35 * n * n; e += blockDim.x) {
+    const int mode = e >> (2 * lg), s = e & (n * n - 1);
+    const bool filt = enc::refs_filtered(p[enc::DP_PLANE] != 0, mode, lg);
+    pred[((size_t)i * 35 + mode) * 1024 + s] = enc::pred_sample(filt ? f : r, dc, lg, mode, s & (n - 1), s >> lg, p[enc::DP_LUMA] != 0, (1 << bd) - 1);
+  }
+}
+
 }  // namespace genc
 }  // namespace b200
 
@@ -1061,6 +1093,43 @@ int b200_gpu_encoder_get_stats(b200_gpu_encoder* enc, b200_gpu_encode_stats* out
   using namespace b200;
   if (!enc || !out) return set_error(B200_E_INVALID, "null argument");
   *out = enc->stats;
+  return B200_OK;
+}
+
+// Test-only entry points (declared by the tests, not in include/b200_heif.h): b200_debug_enc_transform_host and
+// b200_debug_enc_predict_host (b200_hevc_enc.cc) with the same arguments, run by the device code of the GPU encoder
+int b200_debug_enc_transform_device(int n, const int32_t* prm, const int32_t* in, int32_t* out) {
+  using namespace b200;
+  if (n < 1 || n > 65536 || !prm || !in || !out) return set_error(B200_E_INVALID, "enc_transform: %d blocks, null argument", n);
+  for (int i = 0; i < n; i++)
+    if (const char* why = enc::debug_transform_args(prm + (size_t)i * enc::DT_FIELDS, in + (size_t)i * 1024)) return set_error(B200_E_INVALID, "enc_transform: block %d: %s", i, why);
+  DevBuf<int> d_prm, d_in, d_out;
+  int rc = 0;
+  if ((rc = d_prm.reserve((size_t)n * enc::DT_FIELDS, false)) || (rc = d_in.reserve((size_t)n * 1024, false)) ||
+      (rc = d_out.reserve((size_t)n * enc::DT_STAGES * 1024, false))) return rc;
+  B200_CUDA_CHECK(cudaMemcpy(d_prm.d, prm, (size_t)n * enc::DT_FIELDS * 4, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_in.d, in, (size_t)n * 1024 * 4, cudaMemcpyHostToDevice));
+  genc::debug_transform_kernel<<<dim3((unsigned)n, enc::DT_STAGES), 256>>>(d_prm.d, d_in.d, d_out.d);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpy(out, d_out.d, (size_t)n * enc::DT_STAGES * 1024 * 4, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
+
+int b200_debug_enc_predict_device(int n, const int32_t* prm, const int16_t* refs, int16_t* rf, int32_t* pred) {
+  using namespace b200;
+  if (n < 1 || n > 65536 || !prm || !refs || !rf || !pred) return set_error(B200_E_INVALID, "enc_predict: %d blocks, null argument", n);
+  for (int i = 0; i < n; i++)
+    if (const char* why = enc::debug_predict_args(prm + (size_t)i * enc::DP_FIELDS, refs + (size_t)i * 129)) return set_error(B200_E_INVALID, "enc_predict: block %d: %s", i, why);
+  DevBuf<int> d_prm, d_pred; DevBuf<int16_t> d_refs, d_rf;
+  int rc = 0;
+  if ((rc = d_prm.reserve((size_t)n * enc::DP_FIELDS, false)) || (rc = d_refs.reserve((size_t)n * 129, false)) ||
+      (rc = d_rf.reserve((size_t)n * 258, false)) || (rc = d_pred.reserve((size_t)n * 35 * 1024, false))) return rc;
+  B200_CUDA_CHECK(cudaMemcpy(d_prm.d, prm, (size_t)n * enc::DP_FIELDS * 4, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_refs.d, refs, (size_t)n * 129 * 2, cudaMemcpyHostToDevice));
+  genc::debug_predict_kernel<<<n, 256>>>(d_prm.d, d_refs.d, d_rf.d, d_pred.d);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpy(rf, d_rf.d, (size_t)n * 258 * 2, cudaMemcpyDeviceToHost));
+  B200_CUDA_CHECK(cudaMemcpy(pred, d_pred.d, (size_t)n * 35 * 1024 * 4, cudaMemcpyDeviceToHost));
   return B200_OK;
 }
 

@@ -23,6 +23,7 @@
 // The finished CTB leaves shared memory with one cp.async.bulk (TMA) row copy per lane; the halo (row above incl.
 // above-right, column to the left) is kept in shared memory next to the tile.  Integer work: no tensor cores.
 #include "b200_hevc.h"
+#include "b200_staging.h"
 
 namespace b200 {
 
@@ -196,7 +197,9 @@ __device__ __forceinline__ void residual4_lane(int16_t* scr, int lane, const Coe
 }
 
 // ---- phase A, 8x8 .. 32x32 blocks: the whole warp, in place in the block's residual slot (coefficients -> residuals).
-template <bool LIVE>
+// COPY: the same code in an out-of-line function of its own for the test harness (k1_residual_kernel): a second caller of K1's
+// copy changes how ptxas allocates K1's registers around the call.
+template <bool LIVE, int COPY = 0>
 __device__ __noinline__ void residual_big(int16_t* rs, int16_t* tmp, const int8_t* __restrict__ mat, const CoefEntry* __restrict__ ce, int nnz, int lg, int qp, int bd, int lane,
                                           const uint8_t* __restrict__ sf, int sf_dc, bool raw) {   // sf: 8x8 raster scaling factors of (component, size) or nullptr; sf_dc: factor of position (0, 0) for 16x16 / 32x32
   const int n = 1 << lg;
@@ -246,9 +249,24 @@ __device__ __noinline__ void residual_big(int16_t* rs, int16_t* tmp, const int8_
     int e = 0;
 #pragma unroll 2
     for (int q = 0; q < kq2; q++) { const int bq = mq[q]; e = __dp2a_lo(u[2 * q], bq, e); e = __dp2a_hi(u[2 * q + 1], bq, e); }
-    rs[p] = (int16_t)((e + rnd) >> bs2);
+    // the residual itself is unbounded (8.6.4.2) and reaches 61312 at 12 bits / 8x8 and 59584 at 10 bits / 32x32; any value
+    // past 16 bits is beyond maxv, so saturating it leaves Clip1(pred + r) of 8.6.7 exact
+    rs[p] = (int16_t)clip3i(-32768, 32767, (e + rnd) >> bs2);
   }
   __syncwarp();
+}
+
+// The transposed DCT matrices of the CTA (MT32_OFF, MT16_OFF, MT8_OFF), built by threads tid = 0, stride, 2 * stride, ...;
+// the caller synchronises before reading them
+__device__ void build_dct_matrices(int8_t* mat, int tid, int stride) {
+  for (int i = tid; i < 1024 + 256 + 64; i += stride) {
+    const int lg = i < 1024 ? 5 : (i < 1280 ? 4 : 3), j0 = i < 1024 ? i : (i < 1280 ? i - 1024 : i - 1280);
+    const int n = 1 << lg, y = j0 >> lg, kn = j0 & (n - 1), k = kn << (5 - lg);     // row kn of the n-point matrix = row kn << (5 - log2 n) of the 32-point one
+    int v;
+    if (k == 0) v = 64;
+    else { int j = (k * (2 * y + 1)) & 127, sgn = 1; if (j > 64) j = 128 - j; if (j > 32) { j = 64 - j; sgn = -1; } v = sgn * c_dct[j]; }
+    mat[(lg == 5 ? MT32_OFF : (lg == 4 ? MT16_OFF : MT8_OFF)) + y * (n + 4) + kn] = (int8_t)v;
+  }
 }
 
 // ---- phase B: one transform block (of one component, or of Cb and Cr on the two half-warps).
@@ -371,14 +389,7 @@ template <typename P, bool LIVE>
 __global__ void __launch_bounds__(WARPS * 32, B200_RECON_MIN_BLOCKS) hevc_recon_kernel(const DeviceBatch b) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   int8_t* mat = reinterpret_cast<int8_t*>(smem_raw);                       // the transposed DCT matrices, shared by the CTA
-  for (int i = threadIdx.x; i < 1024 + 256 + 64; i += blockDim.x) {
-    const int lg = i < 1024 ? 5 : (i < 1280 ? 4 : 3), j0 = i < 1024 ? i : (i < 1280 ? i - 1024 : i - 1280);
-    const int n = 1 << lg, y = j0 >> lg, kn = j0 & (n - 1), k = kn << (5 - lg);     // row kn of the n-point matrix = row kn << (5 - log2 n) of the 32-point one
-    int v;
-    if (k == 0) v = 64;
-    else { int j = (k * (2 * y + 1)) & 127, sgn = 1; if (j > 64) j = 128 - j; if (j > 32) { j = 64 - j; sgn = -1; } v = sgn * c_dct[j]; }
-    mat[(lg == 5 ? MT32_OFF : (lg == 4 ? MT16_OFF : MT8_OFF)) + y * (n + 4) + kn] = (int8_t)v;
-  }
+  build_dct_matrices(mat, threadIdx.x, blockDim.x);
   __syncthreads();
   const int lane = threadIdx.x & 31;
   const WarpLayout L = warp_layout(b.max_log2_ctb, (int)sizeof(P));
@@ -599,4 +610,108 @@ int launch_recon(const DeviceBatch& b, cudaStream_t s) {
   return B200_OK;
 }
 
+// ---- test-only: the scaling and inverse transform of phase A on single blocks (b200_debug_k1_residual)
+enum { K1B_LOG2N, K1B_BD, K1B_QP, K1B_DST, K1B_TSKIP, K1B_RAW, K1B_SF, K1B_NNZ, K1B_FIELDS };
+constexpr int K1H_RES = (MAT_BYTES + 15) & ~15, K1H_TMP = K1H_RES + 32 * 32 * 2, K1H_SMEM = K1H_TMP + 32 * 34 * 2;   // K1's 16-byte aligned res / tmp
+
+// One warp (CTA) per block: K1's residual4_lane (on lane 0, as a 4x4 block's owner lane) or residual_big, then the residual
+// in raster order to out[block][0 .. n * n)
+__global__ void __launch_bounds__(32) k1_residual_kernel(const int* __restrict__ prm, const uint8_t* __restrict__ sf, const CoefEntry* __restrict__ coefs,
+                                                         const int* __restrict__ coef_off, int16_t* __restrict__ out) {
+  __shared__ __align__(16) unsigned char sm[K1H_SMEM];
+  int8_t* mat = reinterpret_cast<int8_t*>(sm);
+  int16_t* rs = reinterpret_cast<int16_t*>(sm + K1H_RES);
+  int16_t* tmp = reinterpret_cast<int16_t*>(sm + K1H_TMP);
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const int* p = prm + b * K1B_FIELDS;
+  const int lg = p[K1B_LOG2N], n = 1 << lg;
+  const uint8_t* f = p[K1B_SF] ? sf + (size_t)b * 65 : nullptr;
+  const CoefEntry* ce = coefs + coef_off[b];
+  build_dct_matrices(mat, lane, 32);
+  __syncwarp();
+  if (lg == 2) {
+    if (lane == 0) residual4_lane<false>(tmp, 0, ce, p[K1B_NNZ], p[K1B_QP], p[K1B_BD], p[K1B_DST] != 0, p[K1B_TSKIP] != 0, p[K1B_RAW] != 0, rs, f);
+  } else {
+    residual_big<false, 1>(rs, tmp, mat, ce, p[K1B_NNZ], lg, p[K1B_QP], p[K1B_BD], lane, f, f ? (int)f[64] : 16, p[K1B_RAW] != 0);
+  }
+  __syncwarp();
+  for (int i = lane; i < n * n; i += 32) out[(size_t)b * 1024 + i] = rs[i];
+}
+
+__global__ void chroma_qp_kernel(const int* __restrict__ q, int n, int* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = chroma_qp(q[4 * i], q[4 * i + 1], q[4 * i + 2], q[4 * i + 3]);
+}
+
 }  // namespace b200
+
+// Test-only entry points (declared by the tests, not in include/b200_heif.h).  Every argument is checked here, on the host:
+// a call the checks refuse never reaches the device.
+//
+// b200_debug_k1_residual: K1's dequantisation and inverse transform of `n` blocks.  blocks[i * 8 ..]: log2 size (2..5), bit
+// depth (8..12), qp (Qp'Y or Qp'C as K1 passes it: 0 .. 51 + 6 * (bd - 8)), DST (4x4 only), transform skip (4x4 only), raw
+// (cu_transquant_bypass / PCM: the levels are the residuals), use scaling factors, nnz.  factors[i * 65 ..]: the block's
+// factors in sl::Factors layout (8x8 raster, or 4x4 raster in the first 16 entries) and the DC factor of 16x16 / 32x32; read
+// only for blocks that use them.  coefs: the blocks' CoefEntry lists back to back (pos = y * n + x, distinct within a block).
+// out[i * 1024 ..]: the int16 residual in raster order.
+extern "C" int b200_debug_k1_residual(int n, const int32_t* blocks, const uint8_t* factors, const uint32_t* coefs, int16_t* out) {
+  using namespace b200;
+  if (n < 1 || n > 65536 || !blocks || !out) return set_error(B200_E_INVALID, "k1_residual: %d blocks, null argument", n);
+  std::vector<int> off((size_t)n + 1, 0);
+  bool any_sf = false;
+  for (int i = 0; i < n; i++) {
+    const int32_t* p = blocks + (size_t)i * K1B_FIELDS;
+    const int lg = p[K1B_LOG2N], bd = p[K1B_BD], nn = 1 << (lg >= 2 && lg <= 5 ? lg : 2);
+    if (lg < 2 || lg > 5) return set_error(B200_E_INVALID, "k1_residual: block %d: log2 size %d", i, lg);
+    if (bd < 8 || bd > 12) return set_error(B200_E_INVALID, "k1_residual: block %d: bit depth %d", i, bd);
+    if (p[K1B_QP] < 0 || p[K1B_QP] > 51 + 6 * (bd - 8)) return set_error(B200_E_INVALID, "k1_residual: block %d: qp %d", i, p[K1B_QP]);
+    for (int f = K1B_DST; f <= K1B_SF; f++)
+      if (p[f] != 0 && p[f] != 1) return set_error(B200_E_INVALID, "k1_residual: block %d: flag %d = %d", i, f, p[f]);
+    if (lg > 2 && (p[K1B_DST] || p[K1B_TSKIP])) return set_error(B200_E_INVALID, "k1_residual: block %d: DST / transform skip on %dx%d", i, nn, nn);
+    if (p[K1B_TSKIP] && p[K1B_RAW]) return set_error(B200_E_INVALID, "k1_residual: block %d: transform skip and raw", i);
+    if (p[K1B_NNZ] < 0 || p[K1B_NNZ] > nn * nn) return set_error(B200_E_INVALID, "k1_residual: block %d: nnz %d", i, p[K1B_NNZ]);
+    if (p[K1B_NNZ] && !coefs) return set_error(B200_E_INVALID, "k1_residual: null coefficients");
+    any_sf |= p[K1B_SF] != 0;
+    uint32_t seen[32] = {};
+    for (int k = 0; k < p[K1B_NNZ]; k++) {
+      const unsigned pos = coefs[off[i] + k] & 0xffffu;
+      if (pos >= (unsigned)(nn * nn)) return set_error(B200_E_INVALID, "k1_residual: block %d: position %u", i, pos);
+      if (seen[pos >> 5] & (1u << (pos & 31))) return set_error(B200_E_INVALID, "k1_residual: block %d: position %u twice", i, pos);
+      seen[pos >> 5] |= 1u << (pos & 31);
+    }
+    off[(size_t)i + 1] = off[i] + p[K1B_NNZ];
+  }
+  if (any_sf && !factors) return set_error(B200_E_INVALID, "k1_residual: null factors");
+  DevBuf<int> d_prm, d_off; DevBuf<uint8_t> d_sf; DevBuf<uint32_t> d_ce; DevBuf<int16_t> d_out;
+  const size_t nsf = any_sf ? (size_t)n * 65 : 1, nce = off[n] ? (size_t)off[n] : 1;
+  int rc = 0;
+  if ((rc = d_prm.reserve((size_t)n * K1B_FIELDS, false)) || (rc = d_off.reserve(off.size(), false)) || (rc = d_sf.reserve(nsf, false)) ||
+      (rc = d_ce.reserve(nce, false)) || (rc = d_out.reserve((size_t)n * 1024, false))) return rc;
+  B200_CUDA_CHECK(cudaMemcpy(d_prm.d, blocks, (size_t)n * K1B_FIELDS * 4, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_off.d, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+  if (any_sf) B200_CUDA_CHECK(cudaMemcpy(d_sf.d, factors, nsf, cudaMemcpyHostToDevice));
+  if (off[n]) B200_CUDA_CHECK(cudaMemcpy(d_ce.d, coefs, nce * 4, cudaMemcpyHostToDevice));
+  k1_residual_kernel<<<n, 32>>>(d_prm.d, d_sf.d, reinterpret_cast<const CoefEntry*>(d_ce.d), d_off.d, d_out.d);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpy(out, d_out.d, (size_t)n * 1024 * 2, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
+
+// b200_debug_chroma_qp: K1's Qp'C (8.6.1) for n queries q[i * 4 ..] = (QpY, qp offset, bit depth, ChromaArrayType)
+extern "C" int b200_debug_chroma_qp(int n, const int32_t* q, int32_t* out) {
+  using namespace b200;
+  if (n < 1 || n > (1 << 20) || !q || !out) return set_error(B200_E_INVALID, "chroma_qp: %d queries, null argument", n);
+  for (int i = 0; i < n; i++) {
+    const int qpy = q[4 * i], off = q[4 * i + 1], bd = q[4 * i + 2], cat = q[4 * i + 3];
+    if (bd < 8 || bd > 12 || cat < 1 || cat > 3 || qpy < -6 * (bd - 8) || qpy > 51 || off < -12 || off > 12)
+      return set_error(B200_E_INVALID, "chroma_qp: query %d: QpY %d offset %d bit depth %d ChromaArrayType %d", i, qpy, off, bd, cat);
+  }
+  DevBuf<int> d_q, d_out;
+  int rc = 0;
+  if ((rc = d_q.reserve((size_t)n * 4, false)) || (rc = d_out.reserve((size_t)n, false))) return rc;
+  B200_CUDA_CHECK(cudaMemcpy(d_q.d, q, (size_t)n * 16, cudaMemcpyHostToDevice));
+  chroma_qp_kernel<<<(n + 127) / 128, 128>>>(d_q.d, n, d_out.d);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpy(out, d_out.d, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
