@@ -867,6 +867,45 @@ extern "C" int b200_debug_parse(const uint8_t* au, size_t size, int8_t* qp8, uin
   return B200_OK;
 }
 
+// Host-only: what the in-loop filters read of an access unit beyond b200_debug_parse's qp8 / edge8, in the record layouts of
+// b200_debug_loop_filters.  hdr[13]: coded width, height, log2 CTB size, bit depth, chroma_format_idc, pps Cb / Cr QP offsets,
+// sample_adaptive_offset_enabled_flag, number of regions, conformance window (crop_x, crop_y, out_w, out_h in luma samples).
+// ctbs[k * 19 ..] (raster order, room for `max_ctbs`): region index and the three SaoComp (type, band position / EO class,
+// four offsets).  regions[k * 6 ..] (room for `max_regions`): beta offset, tc offset, slice_loop_filter_across_slices_enabled_flag,
+// slice index, TileId, loop_filter_across_tiles_enabled_flag.  With ctbs / regions NULL only hdr is filled.
+extern "C" int b200_debug_parse_filters(const uint8_t* au, size_t size, int32_t* hdr, int32_t* ctbs, int max_ctbs, int32_t* regions, int max_regions) {
+  if (!au || !hdr) return set_error(B200_E_INVALID, "parse_filters: null argument");
+  ParsedPicture pp; ParseLimits lim;
+  int rc = parse_access_unit(au, size, lim, pp);
+  if (rc) return rc;
+  const PicDesc& p = pp.desc;
+  const int32_t h[13] = {p.width, p.height, p.log2_ctb, p.bit_depth, p.chroma, p.pps_cb_qp_offset, p.pps_cr_qp_offset, p.sao_enabled, (int32_t)pp.slices.size(),
+                         p.crop_x, p.crop_y, p.out_w, p.out_h};
+  memcpy(hdr, h, sizeof h);
+  const size_t nctb = (size_t)p.wctb * p.hctb;
+  if (ctbs) {
+    if (max_ctbs < 0 || (size_t)max_ctbs < nctb) return set_error(B200_E_INVALID, "parse_filters: room for %d CTBs, %zu needed", max_ctbs, nctb);
+    for (size_t k = 0; k < nctb; k++) {
+      const CtuInfo& ci = pp.ctus[k];
+      int32_t* o = ctbs + k * 19;
+      o[0] = ci.slice_idx;
+      for (int c = 0; c < 3; c++) {
+        o[1 + 6 * c] = ci.sao[c].type; o[2 + 6 * c] = ci.sao[c].band_or_class;
+        for (int j = 0; j < 4; j++) o[3 + 6 * c + j] = ci.sao[c].offset[j];
+      }
+    }
+  }
+  if (regions) {
+    if (max_regions < 0 || (size_t)max_regions < pp.slices.size()) return set_error(B200_E_INVALID, "parse_filters: room for %d regions, %zu needed", max_regions, pp.slices.size());
+    for (size_t k = 0; k < pp.slices.size(); k++) {
+      const SliceInfo& s = pp.slices[k];
+      int32_t* o = regions + k * 6;
+      o[0] = s.beta_offset; o[1] = s.tc_offset; o[2] = s.lf_across_slices; o[3] = s.slice_id; o[4] = s.tile_id; o[5] = s.lf_across_tiles;
+    }
+  }
+  return B200_OK;
+}
+
 // Host-only: parse n access units with `threads` parser threads (the decoder's front-end stage in isolation).
 // Returns the wall-clock milliseconds of the parallel parse in *ms_out.  Used by tests and for tuning on CPU-only hosts.
 extern "C" int b200_debug_parse_many(const uint8_t* const* au, const size_t* au_size, int n, int threads, int repeat, double* ms_out) {

@@ -7,8 +7,10 @@
 // edges of one direction are independent because they are 8 samples apart and touch at most 3 samples per side).
 // SAO reads the deblocked planes and writes the final samples straight into the destination (conformance window
 // applied, destination pointer already offset to the tile's paste position: K5 folded into K4's store).
+#include <algorithm>
 #include <cstdlib>
 #include "b200_hevc.h"
+#include "b200_staging.h"
 
 namespace b200 {
 
@@ -451,3 +453,169 @@ int launch_sao(const DeviceBatch& b, const PicDesc* hp, cudaStream_t s, int* lau
 }
 
 }  // namespace b200
+
+// ---- test-only: K3 and K4 on pictures the caller describes (b200_debug_loop_filters)
+namespace {
+enum { LFP_W, LFP_H, LFP_LOG2_CTB, LFP_BD, LFP_CHROMA, LFP_CB_OFF, LFP_CR_OFF, LFP_SAO, LFP_NSLICES, LFP_CROP_X, LFP_CROP_Y, LFP_OUT_W, LFP_OUT_H,
+       LFP_DST_W, LFP_DST_H, LFP_DST_PITCH, LFP_DST_CPITCH, LFP_PASTE_X, LFP_PASTE_Y, LFP_FIELDS };
+enum { LFC_SLICE, LFC_SAO, LFC_FIELDS = LFC_SAO + 3 * 6 };
+enum { LFS_BETA, LFS_TC, LFS_ACROSS_SLICES, LFS_SLICE_ID, LFS_TILE_ID, LFS_ACROSS_TILES, LFS_FIELDS };
+}  // namespace
+
+// b200_debug_loop_filters: the decoder's own launch_deblock (stages bit 0) and launch_sao (bit 1) on a batch of `npics`
+// pictures.  Per picture, in batch order:
+//   pics[i * 19 ..]: coded width, height (multiples of 8, at most 4096), log2 CTB size (4..6), bit depth (8..12),
+//     chroma_format_idc (0..3), pps Cb / Cr QP offsets (-12..12), sample_adaptive_offset_enabled_flag, number of regions,
+//     conformance window (crop_x, crop_y, out_w, out_h: luma samples, crop_x / crop_y multiples of SubWidthC / SubHeightC),
+//     destination (width, height, luma and chroma pitch in samples) and the paste position of the window in it (multiples
+//     of SubWidthC / SubHeightC; the window must fit);
+//   qp8 / edge8: the w8 x h8 maps (QpY from -6 * (bit depth - 8) to 51; filterEdgeFlags in bits 0..2 only);
+//   ctbs[k * 19 ..]: region index, then type (0..2), band position (0..31) or EO class (0..3) and the four SaoOffsetVal of
+//     Y, Cb, Cr (|offset| <= (1 << (Min(bit depth, 10) - 5)) - 1, shifted by bit depth - 10 above 10 bits);
+//   regions[k * 6 ..]: beta offset, tc offset (even, -12..12), slice_loop_filter_across_slices_enabled_flag, slice index in
+//     decoding order, TileId, loop_filter_across_tiles_enabled_flag (a PPS flag: the same in every region of a picture);
+//   planes_in / rec_out: the Y, Cb, Cr planes of the coded size, rows back to back (1 byte per sample at 8 bits, else 2);
+//   dst_out: the destination planes, pitch x rows (read only with bit 1).
+// The reconstruction planes are laid out as the decoder lays them out (stride (w + 63) & ~63 samples, 256-byte aligned
+// planes): K4's vector loads rely on it.  The destination is filled with `sentinel` bytes before K4 runs and returned whole.
+// rec_out receives the reconstruction planes after the run (deblocked with bit 0).
+extern "C" int b200_debug_loop_filters(int stages, int npics, const int32_t* pics, const int8_t* qp8, const uint8_t* edge8, const int32_t* ctbs,
+                                       const int32_t* regions, const void* planes_in, void* rec_out, void* dst_out, int sentinel) {
+  using namespace b200;
+  if (stages < 1 || stages > 3 || npics < 1 || npics > 256 || !pics || !qp8 || !edge8 || !ctbs || !regions || !planes_in || !rec_out || ((stages & 2) && !dst_out) ||
+      sentinel < 0 || sentinel > 255)
+    return set_error(B200_E_INVALID, "loop_filters: stages %d, %d pictures, null argument or sentinel %d", stages, npics, sentinel);
+  std::vector<PicDesc> hp((size_t)npics);
+  std::vector<CtuInfo> ctu;
+  std::vector<SliceInfo> sli;
+  size_t nmap = 0, in_bytes = 0, rec_bytes = 0, dst_bytes = 0;
+  std::vector<size_t> rec_off((size_t)npics * 3), dst_off((size_t)npics * 3);
+  bool any8 = false, any16 = false;
+  for (int i = 0; i < npics; i++) {
+    const int32_t* f = pics + (size_t)i * LFP_FIELDS;
+    PicDesc& p = hp[(size_t)i];
+    memset(&p, 0, sizeof p);
+    const int W = f[LFP_W], H = f[LFP_H], lg = f[LFP_LOG2_CTB], bd = f[LFP_BD], ch = f[LFP_CHROMA];
+    if (W < 8 || H < 8 || W > 4096 || H > 4096 || (W & 7) || (H & 7)) return set_error(B200_E_INVALID, "loop_filters: picture %d: size %dx%d", i, W, H);
+    if (lg < 4 || lg > 6 || bd < 8 || bd > 12 || ch < 0 || ch > 3) return set_error(B200_E_INVALID, "loop_filters: picture %d: log2 CTB %d, bit depth %d, chroma %d", i, lg, bd, ch);
+    if (f[LFP_CB_OFF] < -12 || f[LFP_CB_OFF] > 12 || f[LFP_CR_OFF] < -12 || f[LFP_CR_OFF] > 12 || (f[LFP_SAO] != 0 && f[LFP_SAO] != 1))
+      return set_error(B200_E_INVALID, "loop_filters: picture %d: qp offsets %d %d, sao %d", i, f[LFP_CB_OFF], f[LFP_CR_OFF], f[LFP_SAO]);
+    const int sx = (ch == 1 || ch == 2) ? 1 : 0, sy = ch == 1 ? 1 : 0;
+    const int cx = f[LFP_CROP_X], cy = f[LFP_CROP_Y], ow = f[LFP_OUT_W], oh = f[LFP_OUT_H];
+    if (cx < 0 || cy < 0 || ow < 1 || oh < 1 || (cx & sx) || (cy & sy) || (int64_t)cx + ow > W || (int64_t)cy + oh > H)
+      return set_error(B200_E_INVALID, "loop_filters: picture %d: conformance window %d,%d %dx%d in %dx%d", i, cx, cy, ow, oh, W, H);
+    const int dw = f[LFP_DST_W], dh = f[LFP_DST_H], dp = f[LFP_DST_PITCH], dcp = f[LFP_DST_CPITCH], px = f[LFP_PASTE_X], py = f[LFP_PASTE_Y];
+    const int dcw = ch ? (dw + sx) >> sx : 0, dch = ch ? (dh + sy) >> sy : 0;
+    if (dw < 1 || dh < 1 || dw > 8192 || dh > 8192 || dp < dw || dp > 8192 || (ch && (dcp < dcw || dcp > 8192)) || px < 0 || py < 0 || (px & sx) || (py & sy) ||
+        (int64_t)px + ow > dw || (int64_t)py + oh > dh)
+      return set_error(B200_E_INVALID, "loop_filters: picture %d: destination %dx%d pitch %d / %d, paste at %d,%d", i, dw, dh, dp, dcp, px, py);
+    const int ns = f[LFP_NSLICES];
+    if (ns < 1 || ns > 4096) return set_error(B200_E_INVALID, "loop_filters: picture %d: %d regions", i, ns);
+    (bd > 8 ? any16 : any8) = true;
+    p.width = W; p.height = H; p.log2_ctb = lg; p.wctb = (W + (1 << lg) - 1) >> lg; p.hctb = (H + (1 << lg) - 1) >> lg;
+    p.bit_depth = bd; p.chroma = ch; p.crop_x = cx; p.crop_y = cy; p.out_w = ow; p.out_h = oh;
+    p.pps_cb_qp_offset = f[LFP_CB_OFF]; p.pps_cr_qp_offset = f[LFP_CR_OFF]; p.sao_enabled = f[LFP_SAO]; p.nslices = ns;
+    p.w8 = W >> 3; p.h8 = H >> 3; p.scaling_idx = -1;
+    p.map8_base = (uint32_t)nmap; p.ctu_base = (uint32_t)ctu.size(); p.slice_base = (uint32_t)sli.size();
+    const int minqp = -6 * (bd - 8);
+    for (size_t k = 0; k < (size_t)p.w8 * p.h8; k++) {
+      if (qp8[nmap + k] < minqp || qp8[nmap + k] > 51) return set_error(B200_E_INVALID, "loop_filters: picture %d: QpY %d", i, qp8[nmap + k]);
+      if (edge8[nmap + k] & ~7) return set_error(B200_E_INVALID, "loop_filters: picture %d: edge flags %#x", i, edge8[nmap + k]);
+    }
+    nmap += (size_t)p.w8 * p.h8;
+    const int cmax = ((1 << (std::min(bd, 10) - 5)) - 1) << std::max(0, bd - 10);
+    for (int k = 0; k < p.wctb * p.hctb; k++) {
+      const int32_t* c = ctbs + (ctu.size()) * LFC_FIELDS;
+      CtuInfo ci; memset(&ci, 0, sizeof ci);
+      if (c[LFC_SLICE] < 0 || c[LFC_SLICE] >= ns) return set_error(B200_E_INVALID, "loop_filters: picture %d: CTB %d: region %d", i, k, c[LFC_SLICE]);
+      ci.slice_idx = (uint16_t)c[LFC_SLICE];
+      for (int comp = 0; comp < 3; comp++) {
+        const int32_t* s = c + LFC_SAO + 6 * comp;
+        if (s[0] < 0 || s[0] > 2 || s[1] < 0 || s[1] > (s[0] == 2 ? 3 : 31)) return set_error(B200_E_INVALID, "loop_filters: picture %d: CTB %d: SAO type %d / %d", i, k, s[0], s[1]);
+        ci.sao[comp].type = (uint8_t)s[0]; ci.sao[comp].band_or_class = (uint8_t)s[1];
+        for (int o = 0; o < 4; o++) {
+          if (s[2 + o] < -cmax || s[2 + o] > cmax) return set_error(B200_E_INVALID, "loop_filters: picture %d: CTB %d: SAO offset %d", i, k, s[2 + o]);
+          ci.sao[comp].offset[o] = (int8_t)s[2 + o];
+        }
+      }
+      ctu.push_back(ci);
+    }
+    for (int k = 0; k < ns; k++) {
+      const int32_t* r = regions + sli.size() * LFS_FIELDS;
+      if (r[LFS_BETA] < -12 || r[LFS_BETA] > 12 || (r[LFS_BETA] & 1) || r[LFS_TC] < -12 || r[LFS_TC] > 12 || (r[LFS_TC] & 1) || (r[LFS_ACROSS_SLICES] & ~1) ||
+          r[LFS_SLICE_ID] < 0 || r[LFS_SLICE_ID] > 65535 || r[LFS_TILE_ID] < 0 || r[LFS_TILE_ID] > 65535 || (r[LFS_ACROSS_TILES] & ~1))
+        return set_error(B200_E_INVALID, "loop_filters: picture %d: region %d", i, k);
+      if (r[LFS_ACROSS_TILES] != regions[(size_t)p.slice_base * LFS_FIELDS + LFS_ACROSS_TILES])   // a PPS flag: one value per picture
+        return set_error(B200_E_INVALID, "loop_filters: picture %d: region %d: loop_filter_across_tiles_enabled_flag differs", i, k);
+      SliceInfo si; memset(&si, 0, sizeof si);
+      si.beta_offset = (int8_t)r[LFS_BETA]; si.tc_offset = (int8_t)r[LFS_TC]; si.lf_across_slices = (uint8_t)r[LFS_ACROSS_SLICES];
+      si.slice_id = (uint16_t)r[LFS_SLICE_ID]; si.tile_id = (uint16_t)r[LFS_TILE_ID]; si.lf_across_tiles = (uint8_t)r[LFS_ACROSS_TILES];
+      sli.push_back(si);
+    }
+    const int bps = bd > 8 ? 2 : 1, maxv = (1 << bd) - 1;
+    for (int c = 0; c < (ch ? 3 : 1); c++) {
+      const int w = c ? W >> sx : W, h = c ? H >> sy : H, st = (w + 63) & ~63;
+      if (bps == 2) {
+        const uint16_t* s = reinterpret_cast<const uint16_t*>(static_cast<const uint8_t*>(planes_in) + in_bytes);
+        for (size_t k = 0; k < (size_t)w * h; k++) if (s[k] > maxv) return set_error(B200_E_INVALID, "loop_filters: picture %d: sample %u above %d", i, s[k], maxv);
+      }
+      in_bytes += (size_t)w * h * bps;
+      p.rec_stride[c] = st; rec_off[(size_t)i * 3 + c] = rec_bytes;
+      rec_bytes = (rec_bytes + (size_t)st * h * bps + 255) & ~(size_t)255;
+      const int rows = c ? dch : dh, pitch = c ? dcp : dp;
+      dst_off[(size_t)i * 3 + c] = dst_bytes;
+      p.dst_stride[c] = pitch;
+      dst_bytes += (size_t)pitch * rows * bps;
+    }
+  }
+  if (any8 && any16 && !(stages & 1)) return set_error(B200_E_UNSUPPORTED, "a batch must not mix 8-bit and >8-bit pictures");
+  DevBuf<PicDesc> d_pics; DevBuf<CtuInfo> d_ctu; DevBuf<SliceInfo> d_sli; DevBuf<int8_t> d_qp; DevBuf<uint8_t> d_edge, d_rec, d_dst;
+  int rc = 0;
+  if ((rc = d_pics.reserve((size_t)npics, false)) || (rc = d_ctu.reserve(ctu.size(), false)) || (rc = d_sli.reserve(sli.size(), false)) || (rc = d_qp.reserve(nmap, false)) ||
+      (rc = d_edge.reserve(nmap, false)) || (rc = d_rec.reserve(rec_bytes, false)) || (rc = d_dst.reserve(dst_bytes + 1, false)))
+    return rc;
+  for (int i = 0; i < npics; i++) {
+    PicDesc& p = hp[(size_t)i];
+    const int sx = (p.chroma == 1 || p.chroma == 2) ? 1 : 0, sy = p.chroma == 1 ? 1 : 0, bps = p.bit_depth > 8 ? 2 : 1;
+    const int32_t* f = pics + (size_t)i * LFP_FIELDS;
+    for (int c = 0; c < (p.chroma ? 3 : 1); c++) {
+      p.rec[c] = d_rec.d + rec_off[(size_t)i * 3 + c];
+      const int px = c ? f[LFP_PASTE_X] >> sx : f[LFP_PASTE_X], py = c ? f[LFP_PASTE_Y] >> sy : f[LFP_PASTE_Y];
+      p.dst[c] = d_dst.d + dst_off[(size_t)i * 3 + c] + ((size_t)py * p.dst_stride[c] + px) * bps;
+    }
+  }
+  size_t in_pos = 0;
+  for (int i = 0; i < npics; i++) {
+    const PicDesc& p = hp[(size_t)i];
+    const int sx = (p.chroma == 1 || p.chroma == 2) ? 1 : 0, sy = p.chroma == 1 ? 1 : 0, bps = p.bit_depth > 8 ? 2 : 1;
+    for (int c = 0; c < (p.chroma ? 3 : 1); c++) {
+      const int w = c ? p.width >> sx : p.width, h = c ? p.height >> sy : p.height;
+      B200_CUDA_CHECK(cudaMemcpy2D(p.rec[c], (size_t)p.rec_stride[c] * bps, static_cast<const uint8_t*>(planes_in) + in_pos, (size_t)w * bps, (size_t)w * bps, h, cudaMemcpyHostToDevice));
+      in_pos += (size_t)w * h * bps;
+    }
+  }
+  B200_CUDA_CHECK(cudaMemcpy(d_pics.d, hp.data(), hp.size() * sizeof(PicDesc), cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_ctu.d, ctu.data(), ctu.size() * sizeof(CtuInfo), cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_sli.d, sli.data(), sli.size() * sizeof(SliceInfo), cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_qp.d, qp8, nmap, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_edge.d, edge8, nmap, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemset(d_dst.d, sentinel, dst_bytes + 1));
+  DeviceBatch b{};
+  b.pics = d_pics.d; b.npics = npics; b.ctus = d_ctu.d; b.slices = d_sli.d; b.qp8 = d_qp.d; b.edge8 = d_edge.d;
+  b.wide_samples = any16 ? 1 : 0;
+  if ((stages & 1) && (rc = launch_deblock(b, hp.data(), nullptr))) return rc;
+  if ((stages & 2) && (rc = launch_sao(b, hp.data(), nullptr))) return rc;
+  B200_CUDA_CHECK(cudaDeviceSynchronize());
+  size_t out_pos = 0;
+  for (int i = 0; i < npics; i++) {
+    const PicDesc& p = hp[(size_t)i];
+    const int sx = (p.chroma == 1 || p.chroma == 2) ? 1 : 0, sy = p.chroma == 1 ? 1 : 0, bps = p.bit_depth > 8 ? 2 : 1;
+    for (int c = 0; c < (p.chroma ? 3 : 1); c++) {
+      const int w = c ? p.width >> sx : p.width, h = c ? p.height >> sy : p.height;
+      B200_CUDA_CHECK(cudaMemcpy2D(static_cast<uint8_t*>(rec_out) + out_pos, (size_t)w * bps, p.rec[c], (size_t)p.rec_stride[c] * bps, (size_t)w * bps, h, cudaMemcpyDeviceToHost));
+      out_pos += (size_t)w * h * bps;
+    }
+  }
+  if (stages & 2) B200_CUDA_CHECK(cudaMemcpy(dst_out, d_dst.d, dst_bytes, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
