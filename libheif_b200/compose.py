@@ -9,11 +9,11 @@ from ._lib import lib, check
 
 def _stream():
     import torch   # deferred: the package must stay importable in processes that only use the host-side C ABI
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
 
 
 def _planes(ts, n):
-    ptrs = (C.c_void_p * n)(*[C.c_void_p(t.data_ptr()) if t is not None else None for t in ts])
+    ptrs = (C.c_void_p * n)(*[t.data_ptr() if t is not None else None for t in ts])
     strides = (C.c_size_t * n)(*[t.stride(0) * t.element_size() if t is not None else 0 for t in ts])
     return ptrs, strides
 
@@ -35,7 +35,7 @@ def overlay(canvas, child_rgb, dx, dy, child_alpha=None):
     cp, cs = _planes([canvas[0], canvas[1], canvas[2]], 3)
     op, os_ = _planes([child_rgb[0], child_rgb[1], child_rgb[2], child_alpha], 4)
     check(lib().b200_overlay_device(cp, cs, canvas.shape[2], canvas.shape[1], op, os_, child_rgb.shape[2], child_rgb.shape[1],
-                                    C.c_int32(dx), C.c_int32(dy), _stream()))
+                                    dx, dy, _stream()))
     return canvas
 
 
@@ -45,7 +45,6 @@ def scale_nearest_plane(plane, out_w, out_h, image_in, image_out, components=1):
     assert plane.is_cuda and plane.dim() == 2
     out = torch.empty((out_h, out_w * components), dtype=plane.dtype, device=plane.device)
     bpp = components * plane.element_size()
-    check(lib().b200_scale_nearest_device(C.c_void_p(plane.data_ptr()), C.c_size_t(plane.stride(0) * plane.element_size()), C.c_void_p(out.data_ptr()),
-                                          C.c_size_t(out.stride(0) * out.element_size()), C.c_uint32(out_w), C.c_uint32(out_h), C.c_uint32(image_in[0]),
-                                          C.c_uint32(image_in[1]), C.c_uint32(image_out[0]), C.c_uint32(image_out[1]), bpp, _stream()))
+    check(lib().b200_scale_nearest_device(plane.data_ptr(), plane.stride(0) * plane.element_size(), out.data_ptr(), out.stride(0) * out.element_size(),
+                                          out_w, out_h, image_in[0], image_in[1], image_out[0], image_out[1], bpp, _stream()))
     return out

@@ -11,41 +11,8 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .color import Geometry, YCbCrImage, convert_colorspace
-
-
-class ImageInfo(C.Structure):
-    _fields_ = [(n, C.c_int) for n in ("width", "height", "tile_width", "tile_height", "chroma", "bit_depth", "colour_primaries",
-                                       "transfer_characteristics", "matrix_coefficients", "full_range")]
-
-
-class DecodeStats(C.Structure):
-    _fields_ = [(n, C.c_double) for n in ("parse_ms", "pack_ms", "h2d_ms", "gpu_ms", "total_ms", "entropy_ms", "recon_ms", "deblock_ms", "sao_ms")] + \
-               [(n, C.c_uint64) for n in ("bitstream_bytes", "command_bytes", "coefficient_entries", "transform_units", "ctus", "h2d_bytes", "pixels")] + \
-               [("kernel_launches", C.c_int), ("front_end", C.c_int), ("bands", C.c_int)]
-
-
-def _bind(l):
-    if getattr(l, "_dec_bound", False):
-        return
-    l.b200_decoder_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
-    l.b200_decoder_destroy.argtypes = [C.c_void_p]
-    l.b200_decoder_destroy.restype = None
-    l.b200_decoder_decode_grid.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_uint64,
-                                           C.c_int, C.c_int, C.POINTER(ImageInfo), C.c_void_p]
-    l.b200_decoder_get_planes.argtypes = [C.c_void_p, C.POINTER(_lib.Planes)]
-    l.b200_decoder_read_planes.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    l.b200_decoder_debug_read_tile.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    l.b200_decoder_set_debug_stage.argtypes = [C.c_void_p, C.c_int]
-    l.b200_decoder_set_front_end.argtypes = [C.c_void_p, C.c_int]
-    l.b200_decoder_get_stats.argtypes = [C.c_void_p, C.POINTER(DecodeStats)]
-    l.b200_decoder_rerun_device.argtypes = [C.c_void_p, C.c_void_p]
-    l.b200_decode_grid_to_rgb_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_uint64,
-                                               C.c_int, C.c_int, C.POINTER(_lib.Geometry), C.POINTER(_lib.ColorOptions), C.c_void_p,
-                                               C.c_size_t, C.POINTER(ImageInfo)]
-    l.b200_decode_grid_to_rgb_host_async.argtypes = l.b200_decode_grid_to_rgb_host.argtypes
-    l.b200_decoder_wait.argtypes = [C.c_void_p]
-    l._dec_bound = True
+from ._lib import DecodeStats, ImageInfo
+from .color import _BYTES_PER_PIXEL, Geometry, YCbCrImage, convert_colorspace
 
 
 class Decoder:
@@ -53,7 +20,6 @@ class Decoder:
 
     def __init__(self, host_threads: int = 0):
         self.l = _lib.lib()
-        _bind(self.l)
         self.h = C.c_void_p()
         _lib.check(self.l.b200_decoder_create(C.byref(self.h), host_threads))
         self.info = None
@@ -142,7 +108,7 @@ class Decoder:
         p = self.planes_device()
         geom = geometry or Geometry(p.width, p.height)
         ow, oh = geom.size
-        bpp = {10: 3, 11: 4, 12: 6, 13: 8, 14: 6, 15: 8}[out_chroma]
+        bpp = _BYTES_PER_PIXEL[out_chroma]
         if out is None:
             out = torch.empty((oh, ow * bpp), dtype=torch.uint8, device="cuda")
         opt = _lib.ColorOptions(out_chroma, 0, 0)
@@ -156,7 +122,7 @@ class Decoder:
         """heif_decode_image() equivalent on the fused path: HEVC tiles in host memory -> interleaved RGB in host memory."""
         arr, sizes = self._aus(aus)
         info = ImageInfo()
-        bpp = {10: 3, 11: 4, 12: 6, 13: 8, 14: 6, 15: 8}[out_chroma]
+        bpp = _BYTES_PER_PIXEL[out_chroma]
         opt = _lib.ColorOptions(out_chroma, 0, 0)
         if out is None:
             # size is known only after parsing: decode once into a maximal buffer is wasteful, so require the caller

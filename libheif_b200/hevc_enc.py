@@ -5,20 +5,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-
-
-class EncParams(C.Structure):
-    _fields_ = [(n, C.c_int) for n in (
-        "width", "height", "bit_depth", "chroma_format_idc", "log2_ctb_size", "qp", "init_qp",
-        "max_transform_hierarchy_depth_intra", "sao", "sign_data_hiding", "transform_skip", "strong_intra_smoothing",
-        "cu_qp_delta", "diff_cu_qp_delta_depth", "dqp_range", "cb_qp_offset", "cr_qp_offset", "slice_chroma_qp_offsets",
-        "slice_cb_qp_offset", "slice_cr_qp_offset", "wpp", "slice_ctb_rows", "dependent_slice_segments",
-        "loop_filter_across_slices", "slice_loop_filter_across_slices", "deblocking_disabled", "beta_offset_div2",
-        "tc_offset_div2", "slice_deblocking_override", "slice_deblocking_disabled", "slice_beta_offset_div2",
-        "slice_tc_offset_div2", "mode_decision", "split_threshold", "still_picture", "vui_present",
-        "colour_description_present", "colour_primaries", "transfer_characteristics", "matrix_coefficients", "full_range")] + \
-        [("seed", C.c_uint32), ("scaling_lists", C.c_int), ("pcm", C.c_int), ("transquant_bypass", C.c_int), ("tile_cols", C.c_int), ("tile_rows", C.c_int), ("tiles_uniform", C.c_int),
-         ("loop_filter_across_tiles", C.c_int), ("slice_per_tile", C.c_int), ("speed", C.c_int)]
+from ._lib import EncParams, GpuEncodeStats, GridEncodeInfo
 
 
 def default_params(**kw) -> EncParams:
@@ -49,21 +36,12 @@ def encode_intra(y, cb=None, cr=None, **kw) -> bytes:
     p = default_params(width=w, height=h, chroma_format_idc=cfmt, **kw)
     out = C.POINTER(C.c_uint8)()
     n = C.c_size_t()
-    l.b200_hevc_encode_intra.argtypes = [C.POINTER(EncParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t,
-                                         C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)]
-    l.b200_free.argtypes = [C.c_void_p]
     _lib.check(l.b200_hevc_encode_intra(C.byref(p), y.ctypes.data, cb.ctypes.data if chroma else None,
                                         cr.ctypes.data if chroma else None, y.strides[0], cb.strides[0] if chroma else 0,
                                         C.byref(out), C.byref(n)))
     data = bytes(C.cast(out, C.POINTER(C.c_uint8 * n.value)).contents)
     l.b200_free(out)
     return data
-
-
-class GpuEncodeStats(C.Structure):
-    _fields_ = [("analyse_ms", C.c_double), ("entropy_ms", C.c_double), ("framing_ms", C.c_double), ("total_ms", C.c_double),
-                ("bytes", C.c_uint64), ("ctus", C.c_uint64), ("pictures", C.c_uint64),
-                ("mode_evaluations", C.c_uint64), ("cu_evaluations", C.c_uint64)]
 
 
 # What the GPU encoder codes (b200_heif.h): no SAO, sign hiding or cu_qp_delta, one WPP sub-stream per CTB row.
@@ -76,15 +54,7 @@ def gpu_params(width, height, chroma, **kw) -> EncParams:
 
 
 def substream_capacity(width, log2_ctb_size, chroma=True) -> int:
-    l = _lib.lib()
-    l.b200_gpu_encoder_substream_capacity.restype = C.c_size_t
-    l.b200_gpu_encoder_substream_capacity.argtypes = [C.c_int, C.c_int, C.c_int]
-    return int(l.b200_gpu_encoder_substream_capacity(width, log2_ctb_size, 1 if chroma else 0))
-
-
-class GridEncodeInfo(C.Structure):
-    _fields_ = [(n, C.c_int) for n in ("cols", "rows", "tile_w", "tile_h", "width", "height", "has_alpha", "pipeline")] + \
-        [("colour_ms", C.c_double), ("upload_ms", C.c_double)]
+    return int(_lib.lib().b200_gpu_encoder_substream_capacity(width, log2_ctb_size, 1 if chroma else 0))
 
 
 def _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferred, bit_depth, endianness, alpha_bit_depth, params):
@@ -107,24 +77,14 @@ def _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferr
     return d, p, opt, device
 
 
-def _bind_grid(l):
-    l.b200_gpu_encode_rgb_grid_check.argtypes = [C.POINTER(_lib.RgbImage), C.c_int, C.c_int, C.POINTER(EncParams), C.POINTER(_lib.RgbToYCbCrOptions)]
-    l.b200_gpu_encode_rgb_grid_device.argtypes = [C.c_void_p, C.POINTER(_lib.RgbImage), C.c_int, C.c_int, C.POINTER(EncParams),
-                                                  C.POINTER(_lib.RgbToYCbCrOptions), C.c_void_p, C.POINTER(GridEncodeInfo)]
-    l.b200_gpu_encode_rgb_grid_host.argtypes = [C.c_void_p, C.POINTER(_lib.RgbImage), C.c_int, C.c_int, C.POINTER(EncParams),
-                                                C.POINTER(_lib.RgbToYCbCrOptions), C.POINTER(GridEncodeInfo)]
-
-
 def grid_encode_check(rgb, tile_w, tile_h, alpha=None, chroma_downsampling=2, only_use_preferred=False, input_bit_depth=None, endianness=None,
                       alpha_bit_depth=None, **params):
     """Host only, no CUDA (b200_gpu_encode_rgb_grid_check): raises B200Error with the code and message
     GpuEncoder.encode_rgb_grid would fail with for these arguments (numpy input; no pixel is read).  input_bit_depth /
     endianness / alpha_bit_depth describe uint16 inputs as rgb_to_ycbcr_ex's bit_depth / endianness / alpha_bit_depth do."""
-    l = _lib.lib()
-    _bind_grid(l)
     d, p, opt, _ = _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferred, input_bit_depth, endianness, alpha_bit_depth,
                               params)
-    _lib.check(l.b200_gpu_encode_rgb_grid_check(C.byref(d), tile_w, tile_h, C.byref(p), C.byref(opt)))
+    _lib.check(_lib.lib().b200_gpu_encode_rgb_grid_check(C.byref(d), tile_w, tile_h, C.byref(p), C.byref(opt)))
 
 
 class GpuEncoder:
@@ -135,18 +95,9 @@ class GpuEncoder:
     2 selects the mode decision (b200_heif.h): 1 searches at most 18 of the 35 luma modes per PU, 2 also decides open loop."""
 
     def __init__(self):
-        l = self._l = _lib.lib()
-        l.b200_gpu_encoder_create.argtypes = [C.POINTER(C.c_void_p)]
-        l.b200_gpu_encoder_destroy.argtypes = [C.c_void_p]
-        l.b200_gpu_encoder_destroy.restype = None
-        for f in (l.b200_gpu_encode_intra_device, l.b200_gpu_encode_intra_host):
-            f.argtypes = [C.c_void_p, C.POINTER(EncParams), C.c_int, C.POINTER(_lib.Planes)] + ([C.c_void_p] if f is l.b200_gpu_encode_intra_device else [])
-        l.b200_gpu_encoder_output.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t)]
-        l.b200_gpu_encoder_read_recon.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t]
-        l.b200_gpu_encoder_get_stats.argtypes = [C.c_void_p, C.POINTER(GpuEncodeStats)]
-        l.b200_gpu_encoder_e1_warps_per_sm.argtypes = [C.c_int, C.POINTER(C.c_int)]
+        self._l = _lib.lib()
         self._h = C.c_void_p()
-        _lib.check(l.b200_gpu_encoder_create(C.byref(self._h)))
+        _lib.check(self._l.b200_gpu_encoder_create(C.byref(self._h)))
         self._shape = None
 
     def close(self):
@@ -206,7 +157,6 @@ class GpuEncoder:
         the conversion target as well.  Returns dict(tiles=[bytes] in raster order, alpha=[bytes] or None, cols, rows, width,
         height, pipeline (B200_YCC_PIPE_* mask), colour_ms, upload_ms)."""
         d, p, opt, device = _grid_args(rgb, tile_w, tile_h, alpha, chroma_downsampling, only_use_preferred, None, None, None, params)
-        _bind_grid(self._l)
         info = GridEncodeInfo()
         if device:
             import torch

@@ -71,8 +71,8 @@ def main():
         h = rh.load()
         stats = None
         if gpu:
-            b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-            b200.b200_get_decoder_plugin.restype = C.c_void_p
+            from libheif_b200 import _lib
+            b200 = _lib.lib()
             if b200.b200_plugin_bind_libheif(None) != 0:
                 raise RuntimeError("the plugin could not resolve the libheif C API")
             rh.check(h.heif_register_decoder_plugin(C.c_void_p(b200.b200_get_decoder_plugin())), "register decoder plugin")

@@ -80,6 +80,9 @@ def load():
         h.heif_register_encoder_plugin.argtypes = [C.c_void_p]
         h.heif_decoding_options_alloc.restype = C.POINTER(DecodingOptionsHead)
         h.heif_decoding_options_free.argtypes = [C.POINTER(DecodingOptionsHead)]
+        h.heif_image_handle_has_alpha_channel.argtypes = [C.c_void_p]
+        h.heif_encoder_get_name.restype = C.c_char_p
+        h.heif_encoder_get_name.argtypes = [C.c_void_p]
         _h = h
     return _h
 
@@ -121,6 +124,19 @@ def make_ycbcr_image(y, cb, cr, bit_depth=8, nclx=None):
     if nclx is not None:
         n = Nclx(1, nclx[0], nclx[1], nclx[2], nclx[3])
         check(h.heif_image_set_nclx_color_profile(img, C.byref(n)))
+    return img
+
+
+def rgb_image(rgb):
+    """heif_image of an interleaved 8-bit RGB / RGBA array [H, W, 3|4]."""
+    h = load()
+    hh, ww, ch = rgb.shape
+    img = C.c_void_p()
+    check(h.heif_image_create(ww, hh, COLORSPACE_RGB, CHROMA_INTERLEAVED_RGBA if ch == 4 else CHROMA_INTERLEAVED_RGB, C.byref(img)))
+    check(h.heif_image_add_plane(img, CHANNEL_INTERLEAVED, ww, hh, 8))
+    st = C.c_int()
+    p = h.heif_image_get_plane(img, CHANNEL_INTERLEAVED, C.byref(st))
+    np.ctypeslib.as_array(p, shape=(hh, st.value))[:, :ww * ch] = rgb.reshape(hh, ww * ch)
     return img
 
 

@@ -55,10 +55,10 @@ def rgb_picture(size, block):
 
 def child(npy, tile, qp):
     """heif_context_encode_grid of the reference libheif with the "b200-gpu" plugin (never imports torch)."""
+    from libheif_b200 import _lib
     from oracle import refheif as rh
     h = rh.load()
-    b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-    b200.b200_get_gpu_encoder_plugin.restype = C.c_void_p
+    b200 = _lib.lib()
     assert b200.b200_plugin_bind_libheif(None) == 0
     rh.check(h.heif_register_encoder_plugin(b200.b200_get_gpu_encoder_plugin()), "register GPU encoder plugin")
     px = np.load(npy)

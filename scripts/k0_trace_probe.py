@@ -49,9 +49,7 @@ def child(side, reps):
     k0_ms = dec.stats().entropy_ms
     n = side * side * (1024 // 32)                 # one sub-stream per CTB row of every tile (CTB 32, WPP)
     buf = (C.c_ulonglong * (3 * n))()
-    lib = lb._lib.lib()
-    lib.b200_debug_entropy_trace.argtypes = [C.c_void_p, C.c_int]
-    lb._lib.check(lib.b200_debug_entropy_trace(buf, n))
+    lb._lib.check(lb._lib.lib().b200_debug_entropy_trace(buf, n))
     print(json.dumps({"k0_ms": k0_ms, "ctbs_per_sub": 1024 // 32, "trace": list(buf)}))
 
 

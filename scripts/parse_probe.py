@@ -6,7 +6,6 @@ from libheif_b200 import _lib
 n = 64
 tiles = bench.make_tiles(range(n))
 l = _lib.lib()
-l.b200_debug_parse_many.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double)]
 arr = (C.c_char_p * n)(*tiles); sizes = (C.c_size_t * n)(*[len(t) for t in tiles])
 res = {}
 for th in (1, 4, 8, 16, 32, 64, 128):

@@ -43,11 +43,10 @@ def arm(kind, size, frames, quality, batch, path, repeats):
     import numpy as np
     from oracle import refheif as rh
     import refheif_seq as rs
+    from libheif_b200 import _lib
     from libheif_b200.hevc_enc import synthetic_image
     h = rs.load()
-    b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-    for f in ("b200_get_decoder_plugin", "b200_get_encoder_plugin", "b200_get_gpu_encoder_plugin"):
-        getattr(b200, f).restype = C.c_void_p
+    b200 = _lib.lib()
     assert b200.b200_plugin_bind_libheif(None) == 0
     out = {}
     if kind.startswith("encode"):

@@ -14,30 +14,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 from oracle import refheif as rh  # noqa: E402
+from libheif_b200 import _lib  # noqa: E402
 from libheif_b200.hevc_enc import synthetic_image  # noqa: E402  (pure numpy helper)
 
 h = rh.load()
-b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-b200.b200_get_decoder_plugin.restype = C.c_void_p
-b200.b200_get_gpu_encoder_plugin.restype = C.c_void_p
+b200 = _lib.lib()
 assert b200.b200_plugin_bind_libheif(None) == 0, "plugin could not resolve the libheif C API"
 rh.check(h.heif_register_encoder_plugin(b200.b200_get_gpu_encoder_plugin()), "register GPU encoder plugin")
 rh.check(h.heif_register_decoder_plugin(b200.b200_get_decoder_plugin()), "register decoder plugin")
 rh.register_cpu_decoder()
-h.heif_encoder_get_name.restype = C.c_char_p
-h.heif_encoder_get_name.argtypes = [C.c_void_p]
-h.heif_image_handle_has_alpha_channel.argtypes = [C.c_void_p]
-
-
-def rgb_image(rgb):
-    hh, ww, ch = rgb.shape
-    img = C.c_void_p()
-    rh.check(h.heif_image_create(ww, hh, rh.COLORSPACE_RGB, rh.CHROMA_INTERLEAVED_RGBA if ch == 4 else rh.CHROMA_INTERLEAVED_RGB, C.byref(img)))
-    rh.check(h.heif_image_add_plane(img, rh.CHANNEL_INTERLEAVED, ww, hh, 8))
-    st = C.c_int()
-    p = h.heif_image_get_plane(img, rh.CHANNEL_INTERLEAVED, C.byref(st))
-    np.ctypeslib.as_array(p, shape=(hh, st.value))[:, :ww * ch] = rgb.reshape(hh, ww * ch)
-    return img
 
 
 def has_alpha(path):
@@ -77,7 +62,7 @@ res["encoder_ids"] = ["b200-gpu" if "GPU" in res["encoder_ids"][0] else res["enc
 planes = [synthetic_image(10 + c, 200, 136, 8, False)[0] for c in range(3)]
 rgb = np.stack(planes, axis=2)
 f = os.path.join(tmp, "rgb.heic")
-rh.encode_file(f, [rgb_image(rgb)], quality=70)
+rh.encode_file(f, [rh.rgb_image(rgb)], quality=70)
 cpu, res["rgb"] = decoded(f, rh.CHROMA_INTERLEAVED_RGB)
 res["rgb"]["psnr"] = psnr(cpu.reshape(136, 200, 3), rgb)
 
@@ -85,7 +70,7 @@ res["rgb"]["psnr"] = psnr(cpu.reshape(136, 200, 3), rgb)
 alpha = synthetic_image(20, 200, 136, 8, False)[0]
 rgba = np.concatenate([rgb, alpha[:, :, None]], axis=2)
 f = os.path.join(tmp, "rgba.heic")
-rh.encode_file(f, [rgb_image(rgba)], quality=70)
+rh.encode_file(f, [rh.rgb_image(rgba)], quality=70)
 cpu, res["rgba"] = decoded(f, rh.CHROMA_INTERLEAVED_RGBA)
 cpu = cpu.reshape(136, 200, 4)
 res["rgba"]["psnr"] = psnr(cpu[:, :, :3], rgb)
@@ -96,7 +81,7 @@ tiles, srcs = [], []
 for k in range(6):
     t = np.stack([synthetic_image(100 + 3 * k + c, 128, 128, 8, False)[0] for c in range(3)], axis=2)
     srcs.append(t)
-    tiles.append(rgb_image(t))
+    tiles.append(rh.rgb_image(t))
 f = os.path.join(tmp, "grid.heic")
 rh.encode_file(f, tiles, columns=3, rows=2, quality=70, params={"log2-ctb-size": 6})
 cpu, res["grid"] = decoded(f, rh.CHROMA_INTERLEAVED_RGB)

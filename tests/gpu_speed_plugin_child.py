@@ -2,7 +2,6 @@
 The "b200-gpu" encoder plugin's "speed" parameter inside the unmodified reference libheif: RGB, RGBA and a 3x2 grid at
 speed 2, each file decoded with the FFmpeg-backed CPU plugin and with this library's decoder plugin; a file written with
 speed 0 against one written without setting it; a speed-2 image sequence at sequence-batch 1 and 0 (automatic)."""
-import ctypes as C
 import hashlib
 import json
 import os
@@ -15,27 +14,15 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np  # noqa: E402
 from oracle import refheif as rh  # noqa: E402
 import refheif_seq as rs  # noqa: E402
+from libheif_b200 import _lib  # noqa: E402
 from libheif_b200.hevc_enc import synthetic_image  # noqa: E402  (pure numpy helper)
 
 h = rs.load()
-b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-b200.b200_get_decoder_plugin.restype = C.c_void_p
-b200.b200_get_gpu_encoder_plugin.restype = C.c_void_p
+b200 = _lib.lib()
 assert b200.b200_plugin_bind_libheif(None) == 0, "plugin could not resolve the libheif C API"
 rh.check(h.heif_register_encoder_plugin(b200.b200_get_gpu_encoder_plugin()), "register GPU encoder plugin")
 rh.check(h.heif_register_decoder_plugin(b200.b200_get_decoder_plugin()), "register decoder plugin")
 rh.register_cpu_decoder()
-
-
-def rgb_image(rgb):
-    hh, ww, ch = rgb.shape
-    img = C.c_void_p()
-    rh.check(h.heif_image_create(ww, hh, rh.COLORSPACE_RGB, rh.CHROMA_INTERLEAVED_RGBA if ch == 4 else rh.CHROMA_INTERLEAVED_RGB, C.byref(img)))
-    rh.check(h.heif_image_add_plane(img, rh.CHANNEL_INTERLEAVED, ww, hh, 8))
-    st = C.c_int()
-    p = h.heif_image_get_plane(img, rh.CHANNEL_INTERLEAVED, C.byref(st))
-    np.ctypeslib.as_array(p, shape=(hh, st.value))[:, :ww * ch] = rgb.reshape(hh, ww * ch)
-    return img
 
 
 def psnr(a, b):
@@ -60,18 +47,18 @@ SPEED2 = {"speed": 2}
 
 rgb = np.stack([synthetic_image(10 + c, 200, 136, 8, False)[0] for c in range(3)], axis=2)
 f = os.path.join(tmp, "rgb.heic")
-rh.encode_file(f, [rgb_image(rgb)], quality=70, params=SPEED2)
+rh.encode_file(f, [rh.rgb_image(rgb)], quality=70, params=SPEED2)
 res["rgb"] = decoded(f, rh.CHROMA_INTERLEAVED_RGB, rgb, (136, 200, 3))
 
 alpha = synthetic_image(20, 200, 136, 8, False)[0]
 rgba = np.concatenate([rgb, alpha[:, :, None]], axis=2)
 f = os.path.join(tmp, "rgba.heic")
-rh.encode_file(f, [rgb_image(rgba)], quality=70, params=SPEED2)
+rh.encode_file(f, [rh.rgb_image(rgba)], quality=70, params=SPEED2)
 res["rgba"] = decoded(f, rh.CHROMA_INTERLEAVED_RGBA, rgba, (136, 200, 4))
 
 srcs = [np.stack([synthetic_image(100 + 3 * k + c, 128, 128, 8, False)[0] for c in range(3)], axis=2) for k in range(6)]
 f = os.path.join(tmp, "grid.heic")
-rh.encode_file(f, [rgb_image(t) for t in srcs], columns=3, rows=2, quality=70, params={"log2-ctb-size": 6, **SPEED2})
+rh.encode_file(f, [rh.rgb_image(t) for t in srcs], columns=3, rows=2, quality=70, params={"log2-ctb-size": 6, **SPEED2})
 want = np.concatenate([np.concatenate(srcs[r * 3:(r + 1) * 3], axis=1) for r in range(2)], axis=0)
 res["grid"] = decoded(f, rh.CHROMA_INTERLEAVED_RGB, want, (256, 384, 3))
 
@@ -79,7 +66,7 @@ res["grid"] = decoded(f, rh.CHROMA_INTERLEAVED_RGB, want, (256, 384, 3))
 files = {}
 for name, params in (("unset", None), ("speed0", {"speed": 0}), ("speed2", SPEED2)):
     files[name] = os.path.join(tmp, name + ".heic")
-    rh.encode_file(files[name], [rgb_image(rgb)], quality=70, params=params)
+    rh.encode_file(files[name], [rh.rgb_image(rgb)], quality=70, params=params)
 res["default"] = {k: md5_file(v) for k, v in files.items()}
 
 # a speed-2 sequence, frame by frame and in automatically sized batches

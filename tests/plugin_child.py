@@ -12,6 +12,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 from oracle import bindings as ob  # noqa: E402
 from oracle import refheif as rh  # noqa: E402
+from libheif_b200 import _lib  # noqa: E402
 
 mode = sys.argv[1]
 if mode == "plugin-path-gpu":
@@ -21,9 +22,7 @@ if mode == "plugin-path-gpu":
     os.symlink(os.path.join(ROOT, "libheif_b200", "libb200heif.so"), os.path.join(plugdir, "libb200heif.so"))
     os.environ["LIBHEIF_PLUGIN_PATH"] = plugdir
 h = rh.load()
-b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-b200.b200_get_decoder_plugin.restype = C.c_void_p
-b200.b200_get_encoder_plugin.restype = C.c_void_p
+b200 = _lib.lib()
 assert b200.b200_plugin_bind_libheif(None) == 0, "plugin could not resolve the libheif C API"
 rh.check(h.heif_register_encoder_plugin(b200.b200_get_encoder_plugin()), "register encoder plugin")
 rh.register_cpu_decoder()

@@ -22,13 +22,12 @@ import numpy as np  # noqa: E402
 from oracle import bindings as ob  # noqa: E402
 from oracle import refheif as rh  # noqa: E402
 import refheif_seq as rs  # noqa: E402
+from libheif_b200 import _lib  # noqa: E402
 from libheif_b200.hevc_enc import encode_intra, synthetic_image  # noqa: E402  (host encoder, numpy helper)
 
 mode = sys.argv[1]
 h = rs.load()
-b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-for f in ("b200_get_decoder_plugin", "b200_get_encoder_plugin", "b200_get_gpu_encoder_plugin"):
-    getattr(b200, f).restype = C.c_void_p
+b200 = _lib.lib()
 assert b200.b200_plugin_bind_libheif(None) == 0, "plugin could not resolve the libheif C API"
 if mode in ("cpu", "memlimit"):
     rh.check(h.heif_register_encoder_plugin(b200.b200_get_encoder_plugin()), "register host encoder plugin")
@@ -37,7 +36,6 @@ else:
 if mode != "cpu":
     rh.check(h.heif_register_decoder_plugin(b200.b200_get_decoder_plugin()), "register decoder plugin")
 rh.register_cpu_decoder()
-h.heif_image_handle_has_alpha_channel.argtypes = [C.c_void_p]
 
 QUALITY = 70
 QP = 51 - (QUALITY * 45 + 50) // 100           # the plugins' quality -> QP mapping
@@ -52,17 +50,6 @@ def md5(b):
 def psnr(a, b):
     mse = np.mean((a.astype(np.float64) - b.astype(np.float64)) ** 2)
     return 99.0 if mse == 0 else float(10 * np.log10(255.0 ** 2 / mse))
-
-
-def rgb_image(rgb):
-    hh, ww, ch = rgb.shape
-    img = C.c_void_p()
-    rh.check(h.heif_image_create(ww, hh, rh.COLORSPACE_RGB, rh.CHROMA_INTERLEAVED_RGBA if ch == 4 else rh.CHROMA_INTERLEAVED_RGB, C.byref(img)))
-    rh.check(h.heif_image_add_plane(img, rh.CHANNEL_INTERLEAVED, ww, hh, 8))
-    st = C.c_int()
-    p = h.heif_image_get_plane(img, rh.CHANNEL_INTERLEAVED, C.byref(st))
-    np.ctypeslib.as_array(p, shape=(hh, st.value))[:, :ww * ch] = rgb.reshape(hh, ww * ch)
-    return img
 
 
 def release(imgs):
@@ -179,7 +166,7 @@ if mode == "cpu":
     W, H, N = 200, 136, 9
     rgbs = rgb_frames(N, W, H, 0x5E0)
     f = os.path.join(tmp, "rgb.heif")
-    imgs = [rgb_image(x) for x in rgbs]
+    imgs = [rh.rgb_image(x) for x in rgbs]
     rs.write_sequence(f, imgs, quality=QUALITY, timescale=30000, durations=[1001 + k for k in range(N)])
     release(imgs)
     res["rgb"], _ = sample_report(f)
@@ -305,7 +292,7 @@ else:
     W2, H2, N2 = 200, 136, 9
     rgbas = rgb_frames(N2, W2, H2, 0x700, alpha=True)
     f3 = os.path.join(tmp, "rgba.heif")
-    imgs = [rgb_image(x) for x in rgbas]
+    imgs = [rh.rgb_image(x) for x in rgbas]
     rs.write_sequence(f3, imgs, quality=QUALITY, params=params, timescale=1000, durations=[40] * N2)
     release(imgs)
     res["rgba"], _ = sample_report(f3)
@@ -377,10 +364,10 @@ else:
     # still image and grid through heif_decode_image, unchanged: this decoder plugin == the CPU plugin
     planes = [synthetic_image(10 + c, 200, 136, 8, False)[0] for c in range(3)]
     fs = os.path.join(tmp, "still.heic")
-    img = rgb_image(np.stack(planes, axis=2))
+    img = rh.rgb_image(np.stack(planes, axis=2))
     rh.encode_file(fs, [img], quality=QUALITY)
     release([img])
-    tiles = [rgb_image(np.stack([synthetic_image(100 + 3 * k + c, 128, 128, 8, False)[0] for c in range(3)], axis=2)) for k in range(4)]
+    tiles = [rh.rgb_image(np.stack([synthetic_image(100 + 3 * k + c, 128, 128, 8, False)[0] for c in range(3)], axis=2)) for k in range(4)]
     fg = os.path.join(tmp, "grid.heic")
     rh.encode_file(fg, tiles, columns=2, rows=2, quality=QUALITY)
     release(tiles)

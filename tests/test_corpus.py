@@ -30,9 +30,7 @@ def test_host_front_end_on_corpus(path):
     n8 = 4096 * 4096 // 64
     qp8 = np.zeros(n8, np.int8); edge8 = np.zeros(n8, np.uint8); lm = np.zeros(n8 * 4, np.uint8); cm = np.zeros(n8 * 4, np.uint8)
     out5 = (C.c_ulonglong * 5)()
-    l.b200_debug_parse.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_ulonglong)]
-    info = (C.c_int * 10)()
-    l.b200_probe_access_unit.argtypes = [C.c_char_p, C.c_size_t, C.c_uint64, C.c_void_p]
+    info = _lib.ImageInfo()
     if l.b200_probe_access_unit(au, len(au), 4096 * 4096, info) != 0:
         return                                            # rejected by the header parser: fine
     rc = l.b200_debug_parse(au, len(au), qp8.ctypes.data, edge8.ctypes.data, lm.ctypes.data, cm.ctypes.data, out5)

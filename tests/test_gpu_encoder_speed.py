@@ -49,8 +49,6 @@ def test_check_refuses_speed(speed):
 
 
 def _plugin_params(getter):
-    lib = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-
     class Integer(C.Structure):
         _fields_ = [("default_value", C.c_int), ("have_minmax", C.c_uint8), ("minimum", C.c_int), ("maximum", C.c_int),
                     ("valid_values", C.c_void_p), ("num_valid_values", C.c_int)]
@@ -58,9 +56,7 @@ def _plugin_params(getter):
     class Param(C.Structure):         # b200h_encoder_parameter == heif_encoder_parameter (heif_plugin.h)
         _fields_ = [("version", C.c_int), ("name", C.c_char_p), ("type", C.c_int), ("integer", Integer), ("has_default", C.c_int)]
 
-    f = getattr(lib, getter)
-    f.restype = C.c_void_p
-    words = (C.c_void_p * 33).from_address(f())        # b200h_encoder_plugin as pointer-sized words (x86-64 layout)
+    words = (C.c_void_p * 33).from_address(getattr(_lib.lib(), getter)())        # b200h_encoder_plugin as pointer-sized words (x86-64 layout)
     lst = C.CFUNCTYPE(C.POINTER(C.POINTER(Param)), C.c_void_p)(words[15])(None)
     out = []
     for i in range(16):

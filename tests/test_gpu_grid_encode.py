@@ -81,10 +81,8 @@ def two_step(enc, rgb, alpha_plane, w, h, tw, th, params, convert=None):
 
 # ------------------------------------------------------------------------------------------------ CPU: the host-only check
 def _check_raw(rgb_image, tw, th, p, opt=None):
-    l = _lib.lib()
-    l.b200_gpu_encode_rgb_grid_check.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
-    return l.b200_gpu_encode_rgb_grid_check(C.byref(rgb_image) if rgb_image is not None else None, tw, th,
-                                            C.byref(p) if p is not None else None, C.byref(opt) if opt is not None else None)
+    return _lib.lib().b200_gpu_encode_rgb_grid_check(C.byref(rgb_image) if rgb_image is not None else None, tw, th,
+                                                     C.byref(p) if p is not None else None, C.byref(opt) if opt is not None else None)
 
 
 def _refusal(code, fn, *a, **kw):
@@ -146,8 +144,6 @@ def test_check_refuses_null_pointers():
     q.width, q.height, q.chroma, q.bit_depth = 64, 64, lb.CHROMA_444, 8
     assert _check_raw(q, 32, 32, p) == -1
     l = _lib.lib()
-    l.b200_gpu_encode_rgb_grid_host.argtypes = [C.c_void_p] * 2 + [C.c_int] * 2 + [C.c_void_p] * 3
-    l.b200_gpu_encode_rgb_grid_device.argtypes = [C.c_void_p] * 2 + [C.c_int] * 2 + [C.c_void_p] * 4
     d.rgb = rgb.ctypes.data                             # a NULL encoder is refused before any CUDA call
     assert l.b200_gpu_encode_rgb_grid_host(None, C.byref(d), 32, 32, C.byref(p), None, None) == -1
     assert l.b200_gpu_encode_rgb_grid_device(None, C.byref(d), 32, 32, C.byref(p), None, None, None) == -1
@@ -323,14 +319,10 @@ def test_same_picture_as_libheif_encode_grid(enc, tmp_path):
 def _child(ours):
     from oracle import refheif as rh
     h = rh.load()
-    b200 = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
-    b200.b200_get_decoder_plugin.restype = C.c_void_p
-    b200.b200_get_gpu_encoder_plugin.restype = C.c_void_p
+    b200 = _lib.lib()
     assert b200.b200_plugin_bind_libheif(None) == 0, "plugin could not resolve the libheif C API"
     rh.check(h.heif_register_encoder_plugin(b200.b200_get_gpu_encoder_plugin()), "register GPU encoder plugin")
     rh.register_cpu_decoder()
-    h.heif_encoder_get_name.restype = C.c_char_p
-    h.heif_encoder_get_name.argtypes = [C.c_void_p]
     ctx = h.heif_context_alloc()
     e = C.c_void_p()
     rh.check(h.heif_context_get_encoder_for_format(ctx, rh.COMPRESSION_HEVC, C.byref(e)), "get_encoder_for_format")

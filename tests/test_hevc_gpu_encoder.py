@@ -8,7 +8,7 @@ import pytest
 
 import libheif_b200 as lb
 from libheif_b200 import _lib
-from libheif_b200.hevc_enc import EncParams, GpuEncoder, gpu_params, substream_capacity, synthetic_image
+from libheif_b200.hevc_enc import GpuEncoder, gpu_params, substream_capacity, synthetic_image
 from oracle import bindings as ob
 
 
@@ -46,9 +46,7 @@ def psnr(a, b):
 # ------------------------------------------------------------------------------------------------ CPU: refusals, bound
 def _call_device(p, n, planes):
     # b200_gpu_encode_check: the argument check the encode calls run before touching CUDA, without encoding
-    l = _lib.lib()
-    l.b200_gpu_encode_check.argtypes = [C.POINTER(EncParams), C.c_int, C.c_void_p]
-    return l.b200_gpu_encode_check(C.byref(p) if p is not None else None, n, planes)
+    return _lib.lib().b200_gpu_encode_check(C.byref(p) if p is not None else None, n, planes)
 
 
 def _planes(n, w=64, h=64, chroma=1):

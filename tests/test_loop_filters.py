@@ -12,7 +12,6 @@ which branch every edge segment and every sample takes, so that the tests can as
   filters' reads near the right and bottom edges are compared too;
 - conformance windows with left and top offsets, written into real streams by an SPS rewriter, decode to the window of the
   window-free decode."""
-import ctypes as C
 import os
 from collections import Counter, defaultdict
 
@@ -351,14 +350,6 @@ def crop_paste(pic, planes, cov):
 
 
 # ------------------------------------------------------------------------------------------ the exports
-def _l():
-    l = _lib.lib()
-    l.b200_debug_loop_filters.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 8 + [C.c_int]
-    l.b200_debug_parse_filters.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-    l.b200_debug_parse.argtypes = [C.c_char_p, C.c_size_t] + [C.c_void_p] * 5
-    return l
-
-
 def _records(pics):
     rec = np.array([[p.w, p.h, p.lg, p.bd, p.chroma, p.cb_off, p.cr_off, p.sao_enabled, len(p.regions), *p.window, *p.dst] for p in pics], np.int32)
     qp8 = np.concatenate([p.qp8.reshape(-1) for p in pics]).astype(np.int8)
@@ -376,8 +367,8 @@ def run_filters(pics, stages):
     rout = np.zeros_like(pin)
     dsz = sum(rows * pitch * (1 if p.bd == 8 else 2) for p in pics for rows, pitch in p.dst_shapes())
     dout = np.zeros(max(dsz, 1), np.uint8)
-    rc = _l().b200_debug_loop_filters(stages, len(pics), rec.ctypes.data, qp8.ctypes.data, edge8.ctypes.data, ctbs.ctypes.data, regs.ctypes.data,
-                                      pin.ctypes.data, rout.ctypes.data, dout.ctypes.data, SENTINEL)
+    rc = _lib.lib().b200_debug_loop_filters(stages, len(pics), rec.ctypes.data, qp8.ctypes.data, edge8.ctypes.data, ctbs.ctypes.data, regs.ctypes.data,
+                                            pin.ctypes.data, rout.ctypes.data, dout.ctypes.data, SENTINEL)
     if rc:
         return rc, None, None
     recs, dsts, a, b = [], [], 0, 0
@@ -398,7 +389,7 @@ def run_filters(pics, stages):
 
 def parse_filters(au):
     """b200_debug_parse_filters + b200_debug_parse: the Pic (without planes) the host front-end parses from `au`"""
-    l = _l()
+    l = _lib.lib()
     hdr = np.zeros(13, np.int32)
     _lib.check(l.b200_debug_parse_filters(au, len(au), hdr.ctypes.data, None, 0, None, 0))
     w, h, lg, bd, chroma, cb, cr, sao_en, ns, cx, cy, ow, oh = hdr.tolist()
@@ -945,8 +936,8 @@ def test_loop_filters_refuses_bad_arguments(what):
         rec[0, 8] = args["nslices"]
     pin = np.frombuffer(planes, np.uint8).copy()
     out = np.zeros(1 << 16, np.uint8)
-    rc = _l().b200_debug_loop_filters(args["stages"], args["npics"], rec.ctypes.data, qp8.ctypes.data, edge8.ctypes.data, ctbs.ctypes.data, regs.ctypes.data,
-                                      pin.ctypes.data, out.ctypes.data, out.ctypes.data if args["dst"] else None, args["sentinel"])
+    rc = _lib.lib().b200_debug_loop_filters(args["stages"], args["npics"], rec.ctypes.data, qp8.ctypes.data, edge8.ctypes.data, ctbs.ctypes.data, regs.ctypes.data,
+                                            pin.ctypes.data, out.ctypes.data, out.ctypes.data if args["dst"] else None, args["sentinel"])
     assert (rc != E_INVALID) if what == "none" else (rc == E_INVALID)
 
 
@@ -1090,7 +1081,7 @@ def test_cropped_stream_on_the_cpu(name, kind, win):
 def test_too_large_window_is_refused():
     base = windowless(synth_stream("ctb32"))
     _, w, h, _ = sps_window(base)
-    l = _l()
+    l = _lib.lib()
     hdr = np.zeros(13, np.int32)
     for win in [(w // 4, w // 4, 0, 0), (0, 0, h // 2, 0), (w // 2, 0, 0, 0)]:
         au = set_conformance_window(base, *win)
@@ -1121,7 +1112,7 @@ def test_too_large_window_fails_to_decode(cuda, front_end):
 
 def test_parse_filters_refuses_bad_arguments():
     au = synth_stream("ctb32")
-    l = _l()
+    l = _lib.lib()
     hdr = np.zeros(13, np.int32)
     small = np.zeros(19, np.int32)
     assert l.b200_debug_parse_filters(None, 0, hdr.ctypes.data, None, 0, None, 0) == E_INVALID

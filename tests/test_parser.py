@@ -17,7 +17,6 @@ def product_digest(au):
     n8 = 2048 * 2048 // 64
     qp8 = np.zeros(n8, np.int8); edge8 = np.zeros(n8, np.uint8); lm = np.zeros(n8 * 4, np.uint8); cm = np.zeros(n8 * 4, np.uint8)
     out5 = (C.c_ulonglong * 5)()
-    l.b200_debug_parse.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_ulonglong)]
     _lib.check(l.b200_debug_parse(au, len(au), qp8.ctypes.data, edge8.ctypes.data, lm.ctypes.data, cm.ctypes.data, out5))
     w, h = out5[3], out5[4]
     return dict(hash=out5[0], ncoef=out5[1], ntu=out5[2], w=w, h=h, qp8=qp8[:w * h // 64].copy(), edge8=edge8[:w * h // 64].copy(),
@@ -69,7 +68,6 @@ def test_mutated_streams_never_crash_the_front_end():
     n8 = 2048 * 2048 // 64
     qp8 = np.zeros(n8, np.int8); edge8 = np.zeros(n8, np.uint8); lm = np.zeros(n8 * 4, np.uint8); cm = np.zeros(n8 * 4, np.uint8)
     out5 = (C.c_ulonglong * 5)()
-    l.b200_debug_parse.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_ulonglong)]
     streams = [a for _, a in all_streams() + cpu_extra_streams() if len(a) < 100000]
     rng = random.Random(0xB200)
     decoded = 0
@@ -217,7 +215,6 @@ def test_extreme_exp_golomb_values_in_every_header_field(which):
     qp8 = np.zeros(n8, np.int8); edge8 = np.zeros(n8, np.uint8); lm = np.zeros(n8 * 4, np.uint8); cm = np.zeros(n8 * 4, np.uint8)
     guard = [a.copy() for a in (qp8, edge8, lm, cm)]
     out5 = (C.c_ulonglong * 5)()
-    l.b200_debug_parse.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_ulonglong)]
     streams = dict(all_streams() + cpu_extra_streams())
     base = [streams[k] for k in sorted(streams) if len(streams[k]) < 60000][:6]
     ran = rejected = 0
@@ -249,7 +246,6 @@ def test_advice_r1_reproducer_min_cb_wraps():
     nals[i] = out[:2] + _escape(out[2:])
     m = _join_nals(nals)
     buf = np.zeros(1 << 20, np.uint8); out5 = (C.c_ulonglong * 5)()
-    l.b200_debug_parse.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_ulonglong)]
     assert l.b200_debug_parse(m, len(m), buf.ctypes.data, buf.ctypes.data, buf.ctypes.data, buf.ctypes.data, out5) != 0
 
 
@@ -260,8 +256,6 @@ def test_emulation_prevention_removal_matches_the_byte_serial_rule():
     import ctypes as C
     from libheif_b200 import _lib
     l = _lib.lib()
-    l.b200_debug_unescape.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
-    l.b200_debug_unescape.restype = C.c_int
     rng = np.random.default_rng(7)
 
     def serial(b):

@@ -1,6 +1,5 @@
 """Drop-in boundary tests: libb200heif.so's heif_encoder_plugin / heif_decoder_plugin inside the UNMODIFIED reference
 libheif (oracle/_ref/libheif_ref.so).  Runs in a child process (see oracle/refheif.py for why)."""
-import ctypes as C
 import json
 import os
 import subprocess
@@ -24,7 +23,8 @@ def child(mode):
 def test_library_exports_every_declared_symbol():
     """The C-ABI library loads and exports every symbol of include/b200_heif.h and include/b200_heif_plugin_abi.h."""
     import re
-    lib = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
+    from libheif_b200 import _lib
+    lib = _lib.lib()
     names = set()
     for hdr in ("b200_heif.h", "b200_heif_plugin_abi.h"):
         src = open(os.path.join(ROOT, "include", hdr)).read()

@@ -27,7 +27,8 @@ def test_encoder_tables_declare_sequence_members():
     """Both encoder tables are v4 tables with the sequence members set and does_indicate_keyframes = 1; the GPU table lists
     the "sequence-batch" parameter (default 0 = automatic)."""
     import ctypes as C
-    lib = C.CDLL(os.path.join(ROOT, "libheif_b200", "libb200heif.so"))
+    from libheif_b200 import _lib
+    lib = _lib.lib()
 
     class Integer(C.Structure):
         _fields_ = [("default_value", C.c_int), ("have_minmax", C.c_uint8), ("minimum", C.c_int), ("maximum", C.c_int),
@@ -38,9 +39,7 @@ def test_encoder_tables_declare_sequence_members():
 
     names = {}
     for getter in ("b200_get_encoder_plugin", "b200_get_gpu_encoder_plugin"):
-        f = getattr(lib, getter)
-        f.restype = C.c_void_p
-        p = f()
+        p = getattr(lib, getter)()
         words = (C.c_void_p * 33).from_address(p)       # b200h_encoder_plugin as pointer-sized words (x86-64 layout)
         assert C.c_int.from_address(p).value == 4
         # the v4 members after minimum_required_libheif_version: start / frame / end / get_compressed_data2, does_indicate_keyframes

@@ -141,22 +141,7 @@ def test_worst_case_residuals(lg, dst, want):
         assert max_abs_residual(lg, 12, dst, -32768) <= 32767
 
 
-# ------------------------------------------------------------------------------------------ bindings
-def _l():
-    l = _lib.lib()
-    l.b200_debug_k1_residual.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    l.b200_debug_chroma_qp.argtypes = [C.c_int, C.c_void_p, C.c_void_p]
-    for f in (l.b200_debug_enc_transform_host, l.b200_debug_enc_transform_device):
-        f.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
-    for f in (l.b200_debug_enc_predict_host, l.b200_debug_enc_predict_device):
-        f.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    l.b200_debug_hevc_encode_forced_levels.argtypes = [C.POINTER(hevc_enc.EncParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t,
-                                                       C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(C.c_size_t),
-                                                       C.c_void_p, C.c_void_p, C.c_void_p]
-    l.b200_free.argtypes = [C.c_void_p]
-    return l
-
-
+# ------------------------------------------------------------------------------------------ K1 harness
 class Block:
     """One block of the K1 harness: parameters, optional scaling factors, (pos, level) list."""
 
@@ -187,7 +172,7 @@ def k1_pack(blocks):
 def k1_run(blocks):
     prm, fac, co = k1_pack(blocks)
     out = np.zeros((len(blocks), 1024), I16)
-    _lib.check(_l().b200_debug_k1_residual(len(blocks), prm.ctypes.data, fac.ctypes.data, co.ctypes.data, out.ctypes.data))
+    _lib.check(_lib.lib().b200_debug_k1_residual(len(blocks), prm.ctypes.data, fac.ctypes.data, co.ctypes.data, out.ctypes.data))
     return [out[i, :1 << (2 * b.lg)].reshape(1 << b.lg, 1 << b.lg).astype(np.int64) for i, b in enumerate(blocks)]
 
 
@@ -292,7 +277,7 @@ def test_chroma_qp(cuda):
     assert {-6 * (bd - 8) for bd in range(8, 13)} <= {max(a + b, -6 * (c - 8)) for a, b, c, _ in q.tolist()}
     assert (q[:, 0] + q[:, 1]).max() > 57
     out = np.zeros(len(q), I32)
-    _lib.check(_l().b200_debug_chroma_qp(len(q), q.ctypes.data, out.ctypes.data))
+    _lib.check(_lib.lib().b200_debug_chroma_qp(len(q), q.ctypes.data, out.ctypes.data))
     want = np.array([chroma_qp_ref(*r) for r in q.tolist()], I32)
     assert np.array_equal(out, want)
 
@@ -345,7 +330,7 @@ def enc_cases(bds):
 
 def enc_transform(side, prm, ins):
     out = np.zeros((len(prm), 6, 1024), I32)
-    f = _l().b200_debug_enc_transform_host if side == "host" else _l().b200_debug_enc_transform_device
+    f = _lib.lib().b200_debug_enc_transform_host if side == "host" else _lib.lib().b200_debug_enc_transform_device
     _lib.check(f(len(prm), prm.ctypes.data, ins.ctypes.data, out.ctypes.data))
     return out
 
@@ -525,7 +510,7 @@ def pred_cases(bds):
 def enc_predict(side, prm, refs):
     rf = np.zeros((len(prm), 258), I16)
     pred = np.zeros((len(prm), 35, 1024), I32)
-    f = _l().b200_debug_enc_predict_host if side == "host" else _l().b200_debug_enc_predict_device
+    f = _lib.lib().b200_debug_enc_predict_host if side == "host" else _lib.lib().b200_debug_enc_predict_device
     _lib.check(f(len(prm), prm.ctypes.data, refs.ctypes.data, rf.ctypes.data, pred.ctypes.data))
     return rf, pred
 
@@ -565,8 +550,8 @@ def _k1_call(blocks_prm, coefs, factors=None, n=None):
     prm = np.array(blocks_prm, I32).reshape(-1, 8)
     co = np.array(coefs or [0], np.uint32)
     out = np.zeros((max(len(prm), 1), 1024), I16)
-    return _l().b200_debug_k1_residual(len(prm) if n is None else n, prm.ctypes.data, None if factors is None else factors.ctypes.data,
-                                       co.ctypes.data, out.ctypes.data)
+    return _lib.lib().b200_debug_k1_residual(len(prm) if n is None else n, prm.ctypes.data, None if factors is None else factors.ctypes.data,
+                                             co.ctypes.data, out.ctypes.data)
 
 
 @pytest.mark.parametrize("prm,coefs,why", [
@@ -588,14 +573,14 @@ def test_k1_residual_refusals(prm, coefs, why):
 def test_k1_residual_refusals_counts():
     assert _k1_call([3, 8, 0, 0, 0, 0, 0, 0], [], n=0) == E_INVALID
     assert _k1_call([3, 8, 0, 0, 0, 0, 0, 0], [], n=-3) == E_INVALID
-    assert _l().b200_debug_k1_residual(1, None, None, None, None) == E_INVALID
+    assert _lib.lib().b200_debug_k1_residual(1, None, None, None, None) == E_INVALID
 
 
 @pytest.mark.parametrize("q", [(-1, 0, 8, 1), (52, 0, 8, 1), (-13, 0, 10, 1), (0, 13, 8, 1), (0, -13, 8, 1), (0, 0, 7, 1), (0, 0, 13, 1), (0, 0, 8, 0), (0, 0, 8, 4)])
 def test_chroma_qp_refusals(q):
     qq = np.array([(20, 0, 8, 1), q], I32)
     out = np.zeros(2, I32)
-    assert _l().b200_debug_chroma_qp(2, qq.ctypes.data, out.ctypes.data) == E_INVALID
+    assert _lib.lib().b200_debug_chroma_qp(2, qq.ctypes.data, out.ctypes.data) == E_INVALID
 
 
 @pytest.mark.parametrize("side", ["host", "device"])
@@ -608,7 +593,7 @@ def test_enc_transform_refusals(side, p, bad):
     if bad is not None:
         ins[0, 15] = bad
     out = np.zeros((1, 6, 1024), I32)
-    f = _l().b200_debug_enc_transform_host if side == "host" else _l().b200_debug_enc_transform_device
+    f = _lib.lib().b200_debug_enc_transform_host if side == "host" else _lib.lib().b200_debug_enc_transform_device
     assert f(1, prm.ctypes.data, ins.ctypes.data, out.ctypes.data) == E_INVALID
 
 
@@ -622,7 +607,7 @@ def test_enc_predict_refusals(side, p, bad):
         refs[0, 16] = bad
     rf = np.zeros((1, 258), I16)
     pred = np.zeros((1, 35, 1024), I32)
-    f = _l().b200_debug_enc_predict_host if side == "host" else _l().b200_debug_enc_predict_device
+    f = _lib.lib().b200_debug_enc_predict_host if side == "host" else _lib.lib().b200_debug_enc_predict_device
     assert f(1, prm.ctypes.data, refs.ctypes.data, rf.ctypes.data, pred.ctypes.data) == E_INVALID
 
 
@@ -636,7 +621,7 @@ def forced_encode(bd, cfmt, log2ctb, pattern, count=64, sdh=0, seed=0x7A11):
     rec = [np.zeros((h, w), U16), np.zeros((h >> sy, w >> sx), U16), np.zeros((h >> sy, w >> sx), U16)]
     pat = np.ascontiguousarray(pattern, I16)
     data, size = C.POINTER(C.c_uint8)(), C.c_size_t()
-    l = _l()
+    l = _lib.lib()
     rc = l.b200_debug_hevc_encode_forced_levels(C.byref(p), y.ctypes.data, cb.ctypes.data, cr.ctypes.data, y.strides[0], cb.strides[0],
                                                  pat.ctypes.data, count, C.byref(data), C.byref(size), rec[0].ctypes.data, rec[1].ctypes.data,
                                                  rec[2].ctypes.data)
