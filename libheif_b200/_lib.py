@@ -151,6 +151,8 @@ DEBUG_FUNCTIONS = {
     "b200_debug_unescape": (_int, [C.c_char_p, _sz, _vp, _vp, _sz, _P(_sz)]),
     "b200_debug_k1_residual": (_int, [_int, _vp, _vp, _vp, _vp]),
     "b200_debug_chroma_qp": (_int, [_int, _vp, _vp]),
+    "b200_debug_k1_predict": (_int, [_int] + [_vp] * 7),
+    "b200_debug_k1_descriptors": (_int, [C.c_char_p, _sz, _vp, _vp, _int, _vp, _int]),
     "b200_debug_loop_filters": (_int, [_int, _int] + [_vp] * 8 + [_int]),
     "b200_debug_enc_transform_host": (_int, [_int, _vp, _vp, _vp]),
     "b200_debug_enc_transform_device": (_int, [_int, _vp, _vp, _vp]),

@@ -61,8 +61,8 @@ __constant__ int16_t c_inv_angle[35] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, -4096, 
 __constant__ uint8_t c_qpc[14] = {29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37};
 __constant__ uint8_t c_level_scale[6] = {40, 45, 51, 57, 64, 72};
 
-__device__ __forceinline__ int clip3i(int lo, int hi, int v) { return min(max(v, lo), hi); }
-__device__ __forceinline__ unsigned morton4(unsigned x, unsigned y) {   // z-order index of a 4x4 block inside a CTB
+__host__ __device__ __forceinline__ int clip3i(int lo, int hi, int v) { return min(max(v, lo), hi); }
+__host__ __device__ __forceinline__ unsigned morton4(unsigned x, unsigned y) {   // z-order index of a 4x4 block inside a CTB
   unsigned sx = (x & 1) | ((x & 2) << 1) | ((x & 4) << 2) | ((x & 8) << 3);
   unsigned sy = (y & 1) | ((y & 2) << 1) | ((y & 4) << 2) | ((y & 8) << 3);
   return sx | (sy << 1);
@@ -92,7 +92,10 @@ template <bool LIVE> __device__ __forceinline__ CtuInfo ld_ctu(const CtuInfo* p)
   return c;
 }
 
-__device__ __forceinline__ int chroma_qp(int qpy, int off, int bd, int cfmt = 1) {       // 8.6.1: Table 8-10 when ChromaArrayType == 1, else Min(qPi, 51)
+__host__ __device__ __forceinline__ int chroma_qp(int qpy, int off, int bd, int cfmt = 1) {       // 8.6.1: Table 8-10 when ChromaArrayType == 1, else Min(qPi, 51)
+#ifndef __CUDA_ARCH__
+  static const uint8_t c_qpc[14] = {29, 30, 31, 32, 33, 33, 34, 34, 35, 35, 36, 36, 37, 37};   // the host's copy of the table
+#endif
   const int qbd = 6 * (bd - 8);
   const int qpi = clip3i(-qbd, 57, qpy + off);
   const int qpc = cfmt != 1 ? min(qpi, 51) : (qpi < 30 ? qpi : (qpi >= 43 ? qpi - 6 : c_qpc[qpi - 30]));
@@ -112,7 +115,7 @@ __device__ __forceinline__ int dequant(int level, int qp, int bd_shift, int m) {
 //  y: offset of the block's residuals inside the component's residual area (samples)
 // (tw, th: the component's CTB size; shx: its horizontal sub-sampling when the decoding order inside the CTB has to be judged in
 //  LUMA units -- the 4:2:2 chroma planes, whose blocks follow the z-order of the luma quadtree, not of their own coordinates)
-__device__ __forceinline__ unsigned make_desc(int bx, int by, int lg, int mode, int coded0, int coded1, int tw, int th, int shx, int cx0, int cy0, int cw, int ch,
+__host__ __device__ __forceinline__ unsigned make_desc(int bx, int by, int lg, int mode, int coded0, int coded1, int tw, int th, int shx, int cx0, int cy0, int cw, int ch,
                                               bool nbL, bool nbAL, bool nbA, bool nbAR) {
   const int n = 1 << lg;
   const bool fL = bx > 0 || nbL, fT = by > 0 || nbA;
@@ -130,6 +133,52 @@ __device__ __forceinline__ unsigned make_desc(int bx, int by, int lg, int mode, 
   return (unsigned)(bx >> 2) | ((unsigned)(by >> 2) << 4) | ((unsigned)(lg - 2) << 8) | ((unsigned)mode << 10) | ((unsigned)coded0 << 16) | ((unsigned)coded1 << 17) |
          ((unsigned)fL << 18) | ((unsigned)fC << 19) | ((unsigned)fT << 20) | ((unsigned)(blc >> 2) << 21) | ((unsigned)(trc >> 2) << 25);
 }
+
+// Phase A's derivation, shared by K1 and the host descriptor export (b200_debug_k1_descriptors), so that the export runs K1's own
+// code.  Macros rather than functions: every function form of this code, even a one-line inline helper, changed ptxas's register
+// allocation of K1 (more spills); the expansions are token for token the code K1 had inline.
+//
+// B200_K1_CTB_NEIGHBOURS(REGION): the CTB-level availability nbL / nbAL / nbA / nbAR -- the left / above-left / above / above-right
+// CTB holds the current CTB's region (one slice inside one tile, b200_hevc_types.h).  Expands where rx, ry, addr (raster address),
+// wctb and cur (the CTB's region index) are defined; REGION(a) is the region index of the CTB at raster address a.
+#define B200_K1_CTB_NEIGHBOURS(REGION)                                                  \
+  const bool nbL = rx > 0 && REGION(addr - 1) == cur;                                   \
+  const bool nbAL = rx > 0 && ry > 0 && REGION(addr - wctb - 1) == cur;                 \
+  const bool nbA = ry > 0 && REGION(addr - wctb) == cur;                                \
+  const bool nbAR = ry > 0 && rx + 1 < wctb && REGION(addr - wctb + 1) == cur;
+// B200_K1_TB_OF_CMD: one lane's TuCmd `cmd` (valid: the lane holds one) in component group g of the CTB at luma (x0, y0) -> has, the
+// block's position bx, by in the component's CTB, log2 size lg, mode, coded0 / coded1 (Cb / Cr in the pair), pcm, and what the
+// residual needs (qp0 / qp1, ts0 / ts1, ce / ce1, n0 / n1, raw).  Not paired: a luma block, or (4:2:2 / 4:4:4) the block of plane
+// `pl`, the commands of the other planes skipped; paired: the 4:2:0 Cb + Cr blocks (those of a 4x4 luma unit at the parent 8x8
+// origin).  A lane without a block gets an uncoded 4x4 block at (0, 0).  Expands where cmd, valid, paired, pl, shx, x0, y0, bd,
+// cfmt, sl (SliceInfo) and coefs are defined.
+#define B200_K1_TB_OF_CMD                                                                                                                  \
+  const int log2n = 2 + (int)((cmd.w0 >> 24) & 3);                                                                                         \
+  const int lx = (int)((cmd.w0 & 0xfff) << 2) - x0, ly = (int)(((cmd.w0 >> 12) & 0xfff) << 2) - y0;                                        \
+  const int qpy = (int)((cmd.w1 >> 12) & 0xff) - 64;                                                                                       \
+  const bool pcm = (cmd.w1 >> 21) & 1, raw = ((cmd.w1 >> 21) & 3) != 0;                                                                    \
+  const int nl = (int)(cmd.w3 & 0x7ff), ncb = (int)((cmd.w3 >> 11) & 0x3ff), ncr = (int)((cmd.w3 >> 21) & 0x3ff);                          \
+  const CoefEntry* ce = coefs + cmd.w2;                                                                                                    \
+  bool has; int bx, by, lg, mode, coded0, coded1, qp0, qp1 = 0, ts0, ts1 = 0, n0, n1 = 0; const CoefEntry* ce1 = ce;                       \
+  if (!paired) {                                                                                                                           \
+    has = valid && (int)((cmd.w1 >> 23) & 3) == pl;                                                                                        \
+    bx = lx >> shx; by = ly; lg = log2n; mode = (int)(cmd.w1 & 63); coded0 = (int)((cmd.w0 >> 26) & 1); coded1 = 0;                        \
+    qp0 = pl == 0 ? qpy + 6 * (bd - 8) : chroma_qp(qpy, pl == 1 ? sl.cb_qp_offset : sl.cr_qp_offset, bd, cfmt);                           \
+    ts0 = (int)((cmd.w0 >> 30) & 1); n0 = nl;                                                                                              \
+  } else {                                                                                                                                 \
+    has = valid && ((cmd.w0 >> 29) & 1);                                                                                                   \
+    if (log2n > 2) { bx = lx >> 1; by = ly >> 1; lg = log2n - 1; } else { bx = (lx - 4) >> 1; by = (ly - 4) >> 1; lg = 2; }               \
+    mode = (int)((cmd.w1 >> 6) & 63); coded0 = (int)((cmd.w0 >> 27) & 1); coded1 = (int)((cmd.w0 >> 28) & 1);                             \
+    qp0 = chroma_qp(qpy, sl.cb_qp_offset, bd); qp1 = chroma_qp(qpy, sl.cr_qp_offset, bd);                                                  \
+    ts0 = (int)((cmd.w0 >> 31) & 1); ts1 = (int)((cmd.w1 >> 20) & 1);                                                                      \
+    ce = ce + nl; n0 = ncb; ce1 = ce + ncb; n1 = ncr;                                                                                      \
+  }                                                                                                                                        \
+  if (!has) { coded0 = coded1 = 0; bx = by = 0; lg = 2; }                                                                                  \
+  coded0 = coded0 && n0 > 0; coded1 = coded1 && n1 > 0;
+// B200_K1_DESC: the descriptor word of that block (after B200_K1_TB_OF_CMD and B200_K1_CTB_NEIGHBOURS; tw, th, cx0, cy0, cw, ch: the
+// component's CTB size, CTB origin and plane size).  The 4:2:0 pair is judged in its own coordinates (shx 0), a 4:2:2 plane in luma
+// units.
+#define B200_K1_DESC (make_desc(bx, by, lg, mode, coded0, coded1, tw, th, paired ? 0 : shx, cx0, cy0, cw, ch, nbL, nbAL, nbA, nbAR) | ((unsigned)pcm << 29))
 
 // ---- phase A, 4x4 blocks: the calling lane owns the block.  scr: the warp's [16][32] int16 scratch (column = lane).
 template <bool LIVE>
@@ -457,10 +506,9 @@ __global__ void __launch_bounds__(WARPS * 32, B200_RECON_MIN_BLOCKS) hevc_recon_
       const int addr = ry * wctb + rx;
       const CtuInfo ci = ld_ctu<LIVE>(&ctus[addr]);
       const int cur = ci.slice_idx;
-      const bool nbL = rx > 0 && (int)ld_cmd<LIVE>(&ctus[addr - 1].slice_idx) == cur;
-      const bool nbAL = rx > 0 && ry > 0 && (int)ld_cmd<LIVE>(&ctus[addr - wctb - 1].slice_idx) == cur;
-      const bool nbA = ry > 0 && (int)ld_cmd<LIVE>(&ctus[addr - wctb].slice_idx) == cur;
-      const bool nbAR = ry > 0 && rx + 1 < wctb && (int)ld_cmd<LIVE>(&ctus[addr - wctb + 1].slice_idx) == cur;
+#define B200_K1_REGION(a) (int)ld_cmd<LIVE>(&ctus[a].slice_idx)
+      B200_K1_CTB_NEIGHBOURS(B200_K1_REGION)
+#undef B200_K1_REGION
       const SliceInfo sl = slices[cur];
       // ---- phase A: descriptors + residuals, lane-parallel over the CTB's transform units
       int ntb = 0;
@@ -469,33 +517,11 @@ __global__ void __launch_bounds__(WARPS * 32, B200_RECON_MIN_BLOCKS) hevc_recon_
         const bool valid = base + lane < ci.tu_count;
         TuCmd cmd{0, 0, 0, 0};
         if (valid) cmd = ld_tu<LIVE>(&tus[ci.tu_start + base + lane]);
-        const int log2n = 2 + (int)((cmd.w0 >> 24) & 3);
-        const int lx = (int)((cmd.w0 & 0xfff) << 2) - x0, ly = (int)(((cmd.w0 >> 12) & 0xfff) << 2) - y0;   // luma position inside the CTB
-        const int qpy = (int)((cmd.w1 >> 12) & 0xff) - 64;
-        const bool pcm = (cmd.w1 >> 21) & 1, raw = ((cmd.w1 >> 21) & 3) != 0;
-        const int nl = (int)(cmd.w3 & 0x7ff), ncb = (int)((cmd.w3 >> 11) & 0x3ff), ncr = (int)((cmd.w3 >> 21) & 0x3ff);
-        const CoefEntry* ce = coefs + cmd.w2;
-        bool has; int bx, by, lg, mode, coded0, coded1, qp0, qp1 = 0, ts0, ts1 = 0, n0, n1 = 0; const CoefEntry* ce1 = ce;
-        if (!paired) {
-          // a luma block, or (4:2:2 / 4:4:4) the block of plane `pl`: the commands of the other planes are skipped
-          has = valid && (int)((cmd.w1 >> 23) & 3) == pl;
-          bx = lx >> shx; by = ly; lg = log2n; mode = (int)(cmd.w1 & 63); coded0 = (int)((cmd.w0 >> 26) & 1); coded1 = 0;
-          qp0 = pl == 0 ? qpy + 6 * (bd - 8) : chroma_qp(qpy, pl == 1 ? sl.cb_qp_offset : sl.cr_qp_offset, bd, cfmt);
-          ts0 = (int)((cmd.w0 >> 30) & 1); n0 = nl;
-        } else {
-          has = valid && ((cmd.w0 >> 29) & 1);
-          if (log2n > 2) { bx = lx >> 1; by = ly >> 1; lg = log2n - 1; } else { bx = (lx - 4) >> 1; by = (ly - 4) >> 1; lg = 2; }
-          mode = (int)((cmd.w1 >> 6) & 63); coded0 = (int)((cmd.w0 >> 27) & 1); coded1 = (int)((cmd.w0 >> 28) & 1);
-          qp0 = chroma_qp(qpy, sl.cb_qp_offset, bd); qp1 = chroma_qp(qpy, sl.cr_qp_offset, bd);
-          ts0 = (int)((cmd.w0 >> 31) & 1); ts1 = (int)((cmd.w1 >> 20) & 1);
-          ce = ce + nl; n0 = ncb; ce1 = ce + ncb; n1 = ncr;
-        }
-        if (!has) { coded0 = coded1 = 0; bx = by = 0; lg = 2; }
-        coded0 = coded0 && n0 > 0; coded1 = coded1 && n1 > 0;
+        B200_K1_TB_OF_CMD
         const unsigned hb = __ballot_sync(0xffffffffu, has);
         const int idx = ntb + __popc(hb & lt_mask);
         const unsigned roff = morton4((unsigned)bx >> 2, (unsigned)by >> 2) * 16;
-        if (has) desc[idx] = make_uint2(make_desc(bx, by, lg, mode, coded0, coded1, tw, th, paired ? 0 : shx, cx0, cy0, cw, ch, nbL, nbAL, nbA, nbAR) | ((unsigned)pcm << 29), roff);
+        if (has) desc[idx] = make_uint2(B200_K1_DESC, roff);
         ntb += __popc(hb);
         // 4x4 blocks: one lane each, in registers
         if (lg == 2) {
@@ -643,6 +669,70 @@ __global__ void chroma_qp_kernel(const int* __restrict__ q, int n, int* __restri
   if (i < n) out[i] = chroma_qp(q[4 * i], q[4 * i + 1], q[4 * i + 2], q[4 * i + 3]);
 }
 
+// ---- test-only: K1's make_desc + predict_tb on one constructed block per warp (b200_debug_k1_predict)
+enum { K1P_KIND, K1P_LOG2CTB, K1P_BD, K1P_STRONG, K1P_BX, K1P_BY, K1P_LG, K1P_MODE, K1P_CODED0, K1P_CODED1, K1P_PCM, K1P_CX0, K1P_CY0, K1P_CW, K1P_CH,
+       K1P_NBL, K1P_NBAL, K1P_NBA, K1P_NBAR, K1P_FIELDS };
+enum { K1P_LUMA, K1P_PAIR420, K1P_PLANE422, K1P_PLANE444 };
+constexpr int K1P_TILE = 64 * (64 + PAD), K1P_TOP = 256, K1P_RES = 1024, K1P_REF = 129;   // per-component slots of the buffers
+constexpr int K1P_SENTINEL = -32768;                                                     // neighbour-array entries nobody wrote
+
+// One warp (CTA) per case in K1's configuration for the case's kind: the warp's shared-memory slice of warp_layout(log2ctb,
+// sizeof(P)) at K1's offset, the per-component tl / tp / rs / rf, and lpc / gmask / cidx / luma / smooth / strong_en as at K1's
+// predict_tb call (kind 0: g = 0; 1: g = 1; 2 / 3: g = 2 of a 4:2:2 / 4:4:4 picture).
+template <typename P>
+__global__ void __launch_bounds__(32) k1_predict_kernel(const int* __restrict__ prm, const uint16_t* __restrict__ tiles, const uint16_t* __restrict__ tops,
+                                                        const int16_t* __restrict__ res, uint32_t* __restrict__ desc_out, int16_t* __restrict__ ref_out,
+                                                        uint16_t* __restrict__ tile_out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const int* p = prm + (size_t)b * K1P_FIELDS;
+  const int kind = p[K1P_KIND], log2ctb = p[K1P_LOG2CTB], bd = p[K1P_BD];
+  const WarpLayout L = warp_layout(log2ctb, (int)sizeof(P));
+  unsigned char* wb = smem_raw + MAT_BYTES;
+  P* const tile0 = reinterpret_cast<P*>(wb + L.tile);
+  P* const top0 = reinterpret_cast<P*>(wb + L.top);
+  int16_t* const res0 = reinterpret_cast<int16_t*>(wb + L.res);
+  int16_t* const tmp = reinterpret_cast<int16_t*>(wb + L.tmp);
+  const bool paired = kind == K1P_PAIR420;
+  const int shx = kind == K1P_PAIR420 || kind == K1P_PLANE422 ? 1 : 0, shy = paired ? 1 : 0;
+  const int tw = (1 << log2ctb) >> shx, th = (1 << log2ctb) >> shy, S = tw + PAD, ntop = PAD + 2 * tw + 16;
+  const int ncomp = paired ? 2 : 1;
+  const int bx = p[K1P_BX], by = p[K1P_BY], lg = p[K1P_LG], n = 1 << lg;
+  const unsigned roff = morton4((unsigned)bx >> 2, (unsigned)by >> 2) * 16;
+  for (int c = 0; c < ncomp; c++) {
+    const size_t slot = (size_t)b * 2 + c;
+    for (int i = lane; i < th * S; i += 32) tile0[c * (th * S) + i] = (P)tiles[slot * K1P_TILE + i];
+    for (int i = lane; i < ntop; i += 32) top0[c * ntop + i] = (P)tops[slot * K1P_TOP + i];
+    for (int i = lane; i < tw * th; i += 32) res0[c * (tw * th) + i] = 0;
+  }
+  for (int i = lane; i < 2 * REF_STRIDE; i += 32) tmp[i] = (int16_t)K1P_SENTINEL;
+  __syncwarp();
+  for (int c = 0; c < ncomp; c++)
+    for (int i = lane; i < n * n; i += 32) res0[c * (tw * th) + roff + i] = res[((size_t)b * 2 + c) * K1P_RES + i];
+  __syncwarp();
+  // lane roles as in K1
+  const int lpc = paired ? 16 : 32, l = lane & (lpc - 1), cidx = paired ? lane >> 4 : 0;
+  const unsigned gmask = paired ? (0xffffu << (16 * cidx)) : 0xffffffffu;
+  P* const tl = tile0 + cidx * (th * S);
+  P* const tp = top0 + cidx * (PAD + 2 * tw + 16);
+  int16_t* const rs = res0 + cidx * (tw * th);
+  int16_t* const rf = tmp + cidx * REF_STRIDE;
+  const uint2 d = make_uint2(make_desc(bx, by, lg, p[K1P_MODE], p[K1P_CODED0], p[K1P_CODED1], tw, th, paired ? 0 : shx, p[K1P_CX0], p[K1P_CY0], p[K1P_CW], p[K1P_CH],
+                                       p[K1P_NBL] != 0, p[K1P_NBAL] != 0, p[K1P_NBA] != 0, p[K1P_NBAR] != 0) | ((unsigned)p[K1P_PCM] << 29), roff);
+  const bool luma = kind == K1P_LUMA, smooth = kind == K1P_LUMA || kind == K1P_PLANE444;
+  predict_tb<P>(d, tl, tp, rs, rf, S, l, lpc, gmask, cidx, luma, smooth, bd, luma ? p[K1P_STRONG] : 0);
+  __syncwarp();
+  if (lane == 0) desc_out[b] = d.x;
+  for (int c = 0; c < ncomp; c++) {
+    const size_t slot = (size_t)b * 2 + c;
+    for (int i = lane; i < th * S; i += 32) tile_out[slot * K1P_TILE + i] = (uint16_t)tile0[c * (th * S) + i];
+    for (int i = lane; i <= 4 * n; i += 32) {
+      ref_out[(slot * 2) * K1P_REF + i] = tmp[c * REF_STRIDE + i];
+      if (!paired) ref_out[(slot * 2 + 1) * K1P_REF + i] = tmp[REF_STRIDE + i];     // the filtered array (in the pair, Cr's rf is there)
+    }
+  }
+}
+
 }  // namespace b200
 
 // Test-only entry points (declared by the tests, not in include/b200_heif.h).  Every argument is checked here, on the host:
@@ -713,5 +803,127 @@ extern "C" int b200_debug_chroma_qp(int n, const int32_t* q, int32_t* out) {
   chroma_qp_kernel<<<(n + 127) / 128, 128>>>(d_q.d, n, d_out.d);
   B200_CUDA_CHECK(cudaGetLastError());
   B200_CUDA_CHECK(cudaMemcpy(out, d_out.d, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
+
+// b200_debug_k1_predict: K1's make_desc and predict_tb on n constructed blocks, one warp each.  cases[i * 19 ..]: kind (0: luma,
+// 1: 4:2:0 Cb + Cr pair on the two half-warps, 2: a 4:2:2 chroma plane, 3: a 4:4:4 chroma plane), log2 CTB size (4..6), bit depth
+// (8..12), strong_intra_smoothing_enabled_flag, then make_desc's inputs: bx, by (component samples inside the component's CTB),
+// log2 size, mode, coded (Cb / first component), coded (Cr, pair only), pcm, cx0, cy0 (the CTB's component origin), cw, ch (the
+// component plane's size), nbL, nbAL, nbA, nbAR.  Per case and component c (one, two for the pair), at slot s = i * 2 + c:
+// tiles[s * 5120 ..]: the component's tile as K1 keeps it in shared memory (th rows of tw + 16 samples; sample (x, y) at
+// [y * (tw + 16) + 16 + x], column 15 the left halo); tops[s * 256 ..]: its halo row (sample x at [16 + x]); res[s * 1024 ..]: the
+// block's residual (raster), for pcm the samples.  Outputs: desc[i], the descriptor word; refs[(s * 2) * 129 ..]: rf after
+// substitution, refs[(s * 2 + 1) * 129 ..]: the filtered array (-32768 where nothing was written; not for the pair);
+// tiles_out[s * 5120 ..]: the whole tile after the call.
+extern "C" int b200_debug_k1_predict(int n, const int32_t* cases, const uint16_t* tiles, const uint16_t* tops, const int16_t* res, uint32_t* desc,
+                                     int16_t* refs, uint16_t* tiles_out) {
+  using namespace b200;
+  if (n < 1 || n > 65536 || !cases || !tiles || !tops || !res || !desc || !refs || !tiles_out) return set_error(B200_E_INVALID, "k1_predict: %d cases, null argument", n);
+  bool wide = false, narrow = false;
+  for (int i = 0; i < n; i++) {
+    const int32_t* p = cases + (size_t)i * K1P_FIELDS;
+    const int kind = p[K1P_KIND], lc = p[K1P_LOG2CTB], bd = p[K1P_BD], lg = p[K1P_LG];
+    if (kind < 0 || kind > 3 || lc < 4 || lc > 6 || bd < 8 || bd > 12) return set_error(B200_E_INVALID, "k1_predict: case %d: kind %d log2 CTB %d bit depth %d", i, kind, lc, bd);
+    (bd > 8 ? wide : narrow) = true;
+    const int shx = kind == K1P_PAIR420 || kind == K1P_PLANE422 ? 1 : 0, shy = kind == K1P_PAIR420 ? 1 : 0;
+    const int tw = (1 << lc) >> shx, th = (1 << lc) >> shy, nmax = kind == K1P_LUMA || kind == K1P_PLANE444 ? 5 : 4;
+    if (lg < 2 || lg > nmax || (1 << lg) > tw || (1 << lg) > th) return set_error(B200_E_INVALID, "k1_predict: case %d: log2 size %d", i, lg);
+    const int nn = 1 << lg, bx = p[K1P_BX], by = p[K1P_BY];
+    if (bx < 0 || by < 0 || bx % nn || by % nn || bx + nn > tw || by + nn > th) return set_error(B200_E_INVALID, "k1_predict: case %d: block at (%d, %d)", i, bx, by);
+    if (p[K1P_MODE] < 0 || p[K1P_MODE] > 34) return set_error(B200_E_INVALID, "k1_predict: case %d: mode %d", i, p[K1P_MODE]);
+    for (int f : {K1P_STRONG, K1P_CODED0, K1P_CODED1, K1P_PCM, K1P_NBL, K1P_NBAL, K1P_NBA, K1P_NBAR})
+      if (p[f] != 0 && p[f] != 1) return set_error(B200_E_INVALID, "k1_predict: case %d: flag %d = %d", i, f, p[f]);
+    if (p[K1P_CODED1] && kind != K1P_PAIR420) return set_error(B200_E_INVALID, "k1_predict: case %d: second coded flag outside the pair", i);
+    const int cx0 = p[K1P_CX0], cy0 = p[K1P_CY0], cw = p[K1P_CW], ch = p[K1P_CH];
+    if (cw < 4 || ch < 4 || cw > 8192 || ch > 8192 || cw % 4 || ch % 4 || cx0 < 0 || cy0 < 0 || cx0 % tw || cy0 % th || cx0 + bx + nn > cw || cy0 + by + nn > ch)
+      return set_error(B200_E_INVALID, "k1_predict: case %d: CTB at (%d, %d) of a %dx%d plane", i, cx0, cy0, cw, ch);
+    if ((p[K1P_NBL] && cx0 == 0) || (p[K1P_NBAL] && (cx0 == 0 || cy0 == 0)) || (p[K1P_NBA] && cy0 == 0) || (p[K1P_NBAR] && (cy0 == 0 || cx0 + tw >= cw)))
+      return set_error(B200_E_INVALID, "k1_predict: case %d: a neighbouring CTB outside the picture is available", i);
+    const int maxv = (1 << bd) - 1, S = tw + PAD, ntop = PAD + 2 * tw + 16;
+    for (int c = 0; c < (kind == K1P_PAIR420 ? 2 : 1); c++) {
+      const size_t s = (size_t)i * 2 + c;
+      for (int k = 0; k < th * S; k++) if (tiles[s * K1P_TILE + k] > maxv) return set_error(B200_E_INVALID, "k1_predict: case %d: tile sample above %d", i, maxv);
+      for (int k = 0; k < ntop; k++) if (tops[s * K1P_TOP + k] > maxv) return set_error(B200_E_INVALID, "k1_predict: case %d: halo sample above %d", i, maxv);
+      if (p[K1P_PCM])
+        for (int k = 0; k < nn * nn; k++) if (res[s * K1P_RES + k] < 0 || res[s * K1P_RES + k] > maxv) return set_error(B200_E_INVALID, "k1_predict: case %d: pcm sample outside [0, %d]", i, maxv);
+    }
+  }
+  if (wide && narrow) return set_error(B200_E_INVALID, "k1_predict: 8-bit and deeper cases in one call");
+  DevBuf<int> d_prm; DevBuf<uint16_t> d_tiles, d_tops, d_tout; DevBuf<int16_t> d_res, d_refs; DevBuf<uint32_t> d_desc;
+  const size_t nt = (size_t)n * 2 * K1P_TILE;
+  int rc = 0;
+  if ((rc = d_prm.reserve((size_t)n * K1P_FIELDS, false)) || (rc = d_tiles.reserve(nt, false)) || (rc = d_tops.reserve((size_t)n * 2 * K1P_TOP, false)) ||
+      (rc = d_res.reserve((size_t)n * 2 * K1P_RES, false)) || (rc = d_desc.reserve((size_t)n, false)) || (rc = d_refs.reserve((size_t)n * 4 * K1P_REF, false)) ||
+      (rc = d_tout.reserve(nt, false))) return rc;
+  B200_CUDA_CHECK(cudaMemcpy(d_prm.d, cases, (size_t)n * K1P_FIELDS * 4, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_tiles.d, tiles, nt * 2, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_tops.d, tops, (size_t)n * 2 * K1P_TOP * 2, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemcpy(d_res.d, res, (size_t)n * 2 * K1P_RES * 2, cudaMemcpyHostToDevice));
+  B200_CUDA_CHECK(cudaMemset(d_refs.d, 0, (size_t)n * 4 * K1P_REF * 2));
+  B200_CUDA_CHECK(cudaMemset(d_tout.d, 0, nt * 2));
+  const int smem = MAT_BYTES + warp_layout(6, wide ? 2 : 1).total;
+  const void* kern = wide ? (const void*)k1_predict_kernel<uint16_t> : (const void*)k1_predict_kernel<uint8_t>;
+  B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  if (wide) k1_predict_kernel<uint16_t><<<n, 32, smem>>>(d_prm.d, d_tiles.d, d_tops.d, d_res.d, d_desc.d, d_refs.d, d_tout.d);
+  else k1_predict_kernel<uint8_t><<<n, 32, smem>>>(d_prm.d, d_tiles.d, d_tops.d, d_res.d, d_desc.d, d_refs.d, d_tout.d);
+  B200_CUDA_CHECK(cudaGetLastError());
+  B200_CUDA_CHECK(cudaMemcpy(desc, d_desc.d, (size_t)n * 4, cudaMemcpyDeviceToHost));
+  B200_CUDA_CHECK(cudaMemcpy(refs, d_refs.d, (size_t)n * 4 * K1P_REF * 2, cudaMemcpyDeviceToHost));
+  B200_CUDA_CHECK(cudaMemcpy(tiles_out, d_tout.d, nt * 2, cudaMemcpyDeviceToHost));
+  return B200_OK;
+}
+
+// Host-only: the descriptors phase A of K1 builds for one access unit parsed by the host front-end.  hdr[6]: coded width, height,
+// log2 CTB size, chroma_format_idc, number of component groups G (1 for 4:0:0; 2 for 4:2:0: luma, Cb + Cr; 3 otherwise: luma, Cb, Cr),
+// number of descriptors.  desc (room for max_desc): the descriptor words (make_desc's layout, pcm in bit 29) per CTB in raster order,
+// per group, in the order of the CTB's commands; counts[ctb * G + group] (room for max_counts): how many of them.  With desc / counts
+// NULL only hdr is filled.
+extern "C" int b200_debug_k1_descriptors(const uint8_t* au, size_t size, int32_t* hdr, uint32_t* desc, int max_desc, int32_t* counts, int max_counts) {
+  using namespace b200;
+  if (!au || !hdr) return set_error(B200_E_INVALID, "k1_descriptors: null argument");
+  ParsedPicture pp; ParseLimits lim;
+  int rc = parse_access_unit(au, size, lim, pp);
+  if (rc) return rc;
+  const PicDesc& p = pp.desc;
+  const int cfmt = p.chroma, ng = cfmt == 0 ? 1 : (cfmt == 1 ? 2 : 3), wctb = p.wctb, nctb = p.wctb * p.hctb;
+  std::vector<uint32_t> all;
+  std::vector<int32_t> cnt((size_t)nctb * ng, 0);
+  const int bd = p.bit_depth;
+  const CoefEntry* coefs = pp.coefs.data();
+  for (int addr = 0; addr < nctb; addr++) {
+    const int rx = addr % wctb, ry = addr / wctb;
+    const CtuInfo& ci = pp.ctus[(size_t)addr];
+    const int cur = ci.slice_idx;
+#define B200_HOST_REGION(a) (int)pp.ctus[(size_t)(a)].slice_idx
+    B200_K1_CTB_NEIGHBOURS(B200_HOST_REGION)
+#undef B200_HOST_REGION
+    const SliceInfo sl = pp.slices[(size_t)cur];
+    for (int gi = 0; gi < ng; gi++) {
+      // the work item's group as K1 sees it: 0 luma, 1 the 4:2:0 pair, 2 / 3 the Cb / Cr plane of 4:2:2 / 4:4:4
+      const int g = gi == 0 ? 0 : (cfmt == 1 ? 1 : gi + 1);
+      const int pl = g >= 2 ? g - 1 : 0;
+      const int shx = g == 0 ? 0 : (g == 1 ? 1 : (cfmt == 2 ? 1 : 0)), shy = g == 1 ? 1 : 0;
+      const bool paired = g == 1;
+      const int tw = (1 << p.log2_ctb) >> shx, th = (1 << p.log2_ctb) >> shy, cw = p.width >> shx, ch = p.height >> shy;
+      const int x0 = rx << p.log2_ctb, y0 = ry << p.log2_ctb, cx0 = x0 >> shx, cy0 = y0 >> shy;
+      for (unsigned k = 0; k < ci.tu_count; k++) {
+        const TuCmd cmd = pp.tus[ci.tu_start + k];
+        const bool valid = true;
+        B200_K1_TB_OF_CMD
+        if (has) { all.push_back(B200_K1_DESC); cnt[(size_t)addr * ng + gi]++; }
+      }
+    }
+  }
+  const int32_t h[6] = {p.width, p.height, p.log2_ctb, cfmt, ng, (int32_t)all.size()};
+  memcpy(hdr, h, sizeof h);
+  if (desc) {
+    if (max_desc < 0 || (size_t)max_desc < all.size()) return set_error(B200_E_INVALID, "k1_descriptors: room for %d descriptors, %zu needed", max_desc, all.size());
+    memcpy(desc, all.data(), all.size() * 4);
+  }
+  if (counts) {
+    if (max_counts < 0 || (size_t)max_counts < cnt.size()) return set_error(B200_E_INVALID, "k1_descriptors: room for %d counts, %zu needed", max_counts, cnt.size());
+    memcpy(counts, cnt.data(), cnt.size() * 4);
+  }
   return B200_OK;
 }

@@ -12,6 +12,7 @@ import pytest
 
 from libheif_b200 import _lib
 from libheif_b200 import hevc_enc
+from intra_ref import filtered, predict, substitute
 
 I32, I16, U8, U16 = np.int32, np.int16, np.uint8, np.uint16
 E_INVALID = -1
@@ -364,115 +365,6 @@ def test_enc_transform_device(cuda):
 
 
 # ------------------------------------------------------------------------------------------ intra prediction (8.4.4.2.2 - 8.4.4.2.6)
-ANGLE = [0, 0, 32, 26, 21, 17, 13, 9, 5, 2, 0, -2, -5, -9, -13, -17, -21, -26, -32, -26, -21, -17, -13, -9, -5, -2, 0, 2, 5, 9, 13, 17, 21, 26, 32]
-INV_ANGLE = {11: -4096, 12: -1638, 13: -910, 14: -630, 15: -482, 16: -390, 17: -315, 18: -256, 19: -315, 20: -390, 21: -482, 22: -630,
-             23: -910, 24: -1638, 25: -4096}
-
-
-def to_xy(r, n):
-    """r[0 .. 4n] (r[2n - 1 - y] = p[-1][y], r[2n] = p[-1][-1], r[2n + 1 + x] = p[x][-1]) -> (left[y], corner, top[x])."""
-    r = [int(v) for v in r]
-    return [r[2 * n - 1 - y] for y in range(2 * n)], r[2 * n], [r[2 * n + 1 + x] for x in range(2 * n)]
-
-
-def to_r(left, corner, top):
-    return list(reversed(left)) + [corner] + list(top)
-
-
-def substitute(r, n, bd):
-    """8.4.4.2.2, walking p[-1][2n - 1] up to p[-1][-1], then p[0][-1] .. p[2n - 1][-1]."""
-    seq = list(r)                     # already in that order
-    if all(v < 0 for v in seq):
-        return [1 << (bd - 1)] * len(seq)
-    if seq[0] < 0:
-        seq[0] = next(v for v in seq if v >= 0)
-    for i in range(1, len(seq)):
-        if seq[i] < 0:
-            seq[i] = seq[i - 1]
-    return seq
-
-
-def filtered(r, n, bd, strong):
-    """8.4.4.2.3 filtering process of the neighbours (both filters, regardless of filterFlag)."""
-    left, c, top = to_xy(r, n)
-    if strong and n == 32 and abs(c + top[2 * n - 1] - 2 * top[n - 1]) < (1 << (bd - 5)) and abs(c + left[2 * n - 1] - 2 * left[n - 1]) < (1 << (bd - 5)):
-        fl = [((63 - y) * c + (y + 1) * left[63] + 32) >> 6 for y in range(63)] + [left[63]]
-        ft = [((63 - x) * c + (x + 1) * top[63] + 32) >> 6 for x in range(63)] + [top[63]]
-        return to_r(fl, c, ft)
-    fc = (left[0] + 2 * c + top[0] + 2) >> 2
-    fl = [(left[y + 1] + 2 * left[y] + (left[y - 1] if y else c) + 2) >> 2 for y in range(2 * n - 1)] + [left[2 * n - 1]]
-    ft = [((top[x - 1] if x else c) + 2 * top[x] + top[x + 1] + 2) >> 2 for x in range(2 * n - 1)] + [top[2 * n - 1]]
-    return to_r(fl, fc, ft)
-
-
-def filter_flag(plane, mode, n):
-    if not plane or mode == 1 or n == 4:
-        return False
-    return min(abs(mode - 26), abs(mode - 10)) > {8: 7, 16: 1, 32: 0}[n]
-
-
-def predict(r, f, n, mode, luma, plane, bd):
-    """8.4.4.2.4 - 8.4.4.2.6: the n x n prediction [y][x] from the substituted neighbours r (f: filtered)."""
-    lg = n.bit_length() - 1
-    left, c, top = to_xy(f if filter_flag(plane, mode, n) else r, n)
-    P = lambda x, y: c if x < 0 and y < 0 else (left[y] if x < 0 else top[x])   # noqa: E731
-    maxv = (1 << bd) - 1
-    out = np.zeros((n, n), np.int64)
-    if mode == 0:
-        for y in range(n):
-            for x in range(n):
-                out[y, x] = ((n - 1 - x) * P(-1, y) + (x + 1) * P(n, -1) + (n - 1 - y) * P(x, -1) + (y + 1) * P(-1, n) + n) >> (lg + 1)
-        return out
-    if mode == 1:
-        dc = (sum(P(x, -1) for x in range(n)) + sum(P(-1, y) for y in range(n)) + n) >> (lg + 1)
-        out[:] = dc
-        if luma and n < 32:
-            out[0, 0] = (P(-1, 0) + 2 * dc + P(0, -1) + 2) >> 2
-            for x in range(1, n):
-                out[0, x] = (P(x, -1) + 3 * dc + 2) >> 2
-            for y in range(1, n):
-                out[y, 0] = (P(-1, y) + 3 * dc + 2) >> 2
-        return out
-    ang = ANGLE[mode]
-    ref = {}
-    if mode >= 18:
-        for x in range(n + 1):
-            ref[x] = P(-1 + x, -1)
-        if ang < 0:
-            if (n * ang) >> 5 < -1:
-                for x in range((n * ang) >> 5, 0):
-                    ref[x] = P(-1, -1 + ((x * INV_ANGLE[mode] + 128) >> 8))
-        else:
-            for x in range(n + 1, 2 * n + 1):
-                ref[x] = P(-1 + x, -1)
-        for y in range(n):
-            idx, fact = ((y + 1) * ang) >> 5, ((y + 1) * ang) & 31
-            for x in range(n):
-                out[y, x] = ((32 - fact) * ref[x + idx + 1] + fact * ref[x + idx + 2] + 16) >> 5 if fact else ref[x + idx + 1]
-        if mode == 26 and luma and n < 32:
-            for y in range(n):
-                out[y, 0] = min(max(P(0, -1) + ((P(-1, y) - P(-1, -1)) >> 1), 0), maxv)
-    else:
-        for x in range(n + 1):
-            ref[x] = P(-1, -1 + x)
-        if ang < 0:
-            if (n * ang) >> 5 < -1:
-                for x in range((n * ang) >> 5, 0):
-                    ref[x] = P(-1 + ((x * INV_ANGLE[mode] + 128) >> 8), -1)
-        else:
-            for x in range(n + 1, 2 * n + 1):
-                ref[x] = P(-1, -1 + x)
-        for x in range(n):
-            idx, fact = ((x + 1) * ang) >> 5, ((x + 1) * ang) & 31
-            for y in range(n):
-                out[y, x] = ((32 - fact) * ref[y + idx + 1] + fact * ref[y + idx + 2] + 16) >> 5 if fact else ref[y + idx + 1]
-        if mode == 10 and luma and n < 32:
-            for x in range(n):
-                out[0, x] = min(max(P(-1, 0) + ((P(x, -1) - P(-1, -1)) >> 1), 0), maxv)
-    return out
-
-
-
 def pred_cases(bds):
     """(log2n, bd, luma, plane filtered, strong) x neighbours: random, all 0, all maxv, a smooth ramp (strong smoothing),
     and partly unavailable (-1) runs."""
