@@ -99,6 +99,19 @@ typedef struct b200_color_options {
 int b200_color_convert_device(const b200_planes* in, const b200_geometry* geom, const b200_color_options* opt,
                               void* out, void* out_g, void* out_b, size_t out_stride, void* stream, int* pipeline);
 
+/* Device -> device: b200_color_convert_device followed by HeifPixelImage::scale_nearest_neighbor
+   (libheif/image/pixelimage.cc:1783-1972, what heif_image_scale_image runs) to scale_w x scale_h, without the full-size
+   RGB picture: only the pixels the scaler keeps are converted.  Result pixel (x, y) = pixel (x * out_w / scale_w,
+   y * out_h / scale_h) (64-bit integer arithmetic) of the b200_color_convert_device picture, all components together (the
+   planes of planar RGB with the same indices); up- and down-scaling, any scale_w, scale_h >= 1.  out / out_g / out_b /
+   out_stride describe the scale_w x scale_h result.  The 4:4:4 conversion point and bilinear upsampling keep their full-size
+   4:4:4 intermediates; only the last conversion is scaled.  *pipeline as for the unscaled call.  B200_E_INVALID (before any
+   CUDA call, message naming the argument) for scale_w or scale_h < 1 or a NULL in / geom / opt / out; everything else as
+   b200_color_convert_device. */
+int b200_color_convert_scaled_device(const b200_planes* in, const b200_geometry* geom, const b200_color_options* opt,
+                                     int scale_w, int scale_h, void* out, void* out_g, void* out_b, size_t out_stride,
+                                     void* stream, int* pipeline);
+
 /* Host -> host form with H2D / D2H inside (what a libheif ColorConversionOperation calls: integration/b200_color_op.cc).
    Pageable operands move through a page-locked bounce buffer in bands (host threads fill / drain band k while the DMA
    engine moves band k - 1); the device buffers, the bounce buffer and the stream are kept per GPU for the life of the
@@ -407,6 +420,18 @@ int b200_probe_access_unit(const uint8_t* au, size_t au_size, uint64_t max_image
 int b200_decode_grid_to_rgb_host(b200_decoder* dec, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
                                  uint64_t max_image_size_pixels, int canvas_w, int canvas_h, const b200_geometry* geom /* NULL = identity */,
                                  const b200_color_options* opt, void* out, size_t out_stride, b200_image_info* info);
+
+/* Fused: b200_decode_grid_to_rgb_host whose result is scaled to scale_w x scale_h -- heif_decode_image followed by
+   heif_image_scale_image (HeifPixelImage::scale_nearest_neighbor, libheif/image/pixelimage.cc:1783-1972), as
+   heif-thumbnailer does (examples/heif_thumbnailer.cc:148-207).  One scaled colour conversion of the finished canvas
+   (b200_color_convert_scaled_device), so the full-size RGB picture is never written and only the scale_w x scale_h result is
+   copied to `out` (pageable: through the decoder's bounce buffer; page-locked: directly).  Interleaved targets, as there.
+   B200_E_INVALID (before any CUDA call, message naming the argument) for scale_w or scale_h < 1 or a NULL dec / au / au_size /
+   opt / out; everything else as b200_decode_grid_to_rgb_host. */
+int b200_decode_grid_to_rgb_scaled_host(b200_decoder* dec, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
+                                        uint64_t max_image_size_pixels, int canvas_w, int canvas_h, const b200_geometry* geom,
+                                        const b200_color_options* opt, int scale_w, int scale_h, void* out, size_t out_stride,
+                                        b200_image_info* info);
 
 /* Throughput form: returns when the work is queued; the D2H of this picture overlaps the kernels of the next call (two device
    RGB buffers, a second stream).  `out` must be page-locked.  b200_decoder_wait() blocks until everything submitted has

@@ -13,3 +13,4 @@ from .color import (Geometry, YCbCrImage, convert_colorspace, convert_colorspace
 from .decoder import Decoder, ImageInfo, DecodeStats  # noqa: F401,E402
 from . import hevc_enc  # noqa: F401,E402
 from . import compose  # noqa: F401,E402
+from .compose import thumbnail_size  # noqa: F401,E402

@@ -90,6 +90,7 @@ FUNCTIONS = {
     "b200_geometry_mirror": (_int, [_P(Geometry), _int]),
     "b200_geometry_crop": (_int, [_P(Geometry), _int, _int, _int, _int]),
     "b200_color_convert_device": (_int, [_P(Planes), _P(Geometry), _P(ColorOptions), _vp, _vp, _vp, _sz, _vp, _P(_int)]),
+    "b200_color_convert_scaled_device": (_int, [_P(Planes), _P(Geometry), _P(ColorOptions), _int, _int, _vp, _vp, _vp, _sz, _vp, _P(_int)]),
     "b200_color_convert_host": (_int, [_P(Planes), _P(Geometry), _P(ColorOptions), _vp, _vp, _vp, _sz, _P(_int)]),
     "b200_rgb_to_ycbcr_device": (_int, [_vp, _sz, _int, _P(Planes), _vp]),
     "b200_rgb_to_ycbcr_host": (_int, [_vp, _sz, _int, _P(Planes)]),
@@ -129,6 +130,7 @@ FUNCTIONS = {
     "b200_probe_access_unit": (_int, [C.c_char_p, _sz, C.c_uint64, _P(ImageInfo)]),
     "b200_decode_grid_to_rgb_host": _decode_to_rgb,
     "b200_decode_grid_to_rgb_host_async": _decode_to_rgb,
+    "b200_decode_grid_to_rgb_scaled_host": (_int, _decode_to_rgb[1][:10] + [_int, _int] + _decode_to_rgb[1][10:]),
     "b200_decoder_wait": (_int, [_vp]),
     "b200_host_alloc": (_int, [_sz, _P(_vp)]),
     "b200_host_free": (None, [_vp]),

@@ -142,27 +142,35 @@ def _out_shape(out_chroma, w, h, bit_depth):
     return (h, w * _BYTES_PER_PIXEL[out_chroma]), False
 
 
-def _convert(mem, img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry], out=None, bilinear: bool = False):
+def _convert(mem, img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry], out=None, bilinear: bool = False, scale=None):
     h, w = img.y.shape
     geom = geometry or Geometry(w, h)
     if out is None:
-        shape, wide = _out_shape(out_chroma, *geom.size, img.bit_depth)
+        shape, wide = _out_shape(out_chroma, *(scale or geom.size), img.bit_depth)
         out = mem.empty(shape, mem.rgb16 if wide else mem.u8)
     if out_chroma == CHROMA_444:
         o, og, ob = mem.ptr(out[0]), mem.ptr(out[1]), mem.ptr(out[2])
     else:
         o, og, ob = mem.ptr(out), None, None
     opt = _lib.ColorOptions(out_chroma, 0, 1 if bilinear else 0)
-    pipe = mem.call("b200_color_convert", C.byref(_fill_planes(img, mem)), C.byref(geom.g), C.byref(opt), o, og, ob,
-                    mem.stride(out[0] if out_chroma == CHROMA_444 else out))
+    head = (C.byref(_fill_planes(img, mem)), C.byref(geom.g), C.byref(opt))
+    stride = mem.stride(out[0] if out_chroma == CHROMA_444 else out)
+    if scale is None:
+        pipe = mem.call("b200_color_convert", *head, o, og, ob, stride)
+    else:
+        pipe = mem.call("b200_color_convert_scaled", *head, int(scale[0]), int(scale[1]), o, og, ob, stride)
     return out, pipe
 
 
-def convert_colorspace(img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry] = None, out=None, stream=None, bilinear: bool = False):
+def convert_colorspace(img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry] = None, out=None, stream=None, bilinear: bool = False,
+                       scale=None):
     """Device -> device. `img` planes are CUDA torch tensors (uint8, or int16/uint16 for >8 bit).
 
-    Returns a CUDA uint8 tensor [H, W*bytes_per_pixel] (interleaved) or [3, H, W] (planar RGB 4:4:4)."""
-    return _convert(_Cuda(img.y.device, stream), img, out_chroma, geometry, out, bilinear)[0]
+    scale=(w, h): the result scaled to w x h as heif_image_scale_image (HeifPixelImage::scale_nearest_neighbor) would scale
+    the unscaled one, converting only the pixels it keeps (b200_color_convert_scaled_device).
+    Returns a CUDA uint8 tensor [H, W*bytes_per_pixel] (interleaved) or [3, H, W] (planar RGB 4:4:4), H x W = the scaled size
+    when scale is given."""
+    return _convert(_Cuda(img.y.device, stream), img, out_chroma, geometry, out, bilinear, scale)[0]
 
 
 def convert_colorspace_host(img: YCbCrImage, out_chroma: int, geometry: Optional[Geometry] = None):

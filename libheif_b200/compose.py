@@ -48,3 +48,18 @@ def scale_nearest_plane(plane, out_w, out_h, image_in, image_out, components=1):
     check(lib().b200_scale_nearest_device(plane.data_ptr(), plane.stride(0) * plane.element_size(), out.data_ptr(), out.stride(0) * out.element_size(),
                                           out_w, out_h, image_in[0], image_in[1], image_out[0], image_out[1], bpp, _stream()))
     return out
+
+
+def thumbnail_size(width, height, size):
+    """(w, h) heif-thumbnailer scales a width x height picture to for a thumbnail of `size` (examples/heif_thumbnailer.cc:169-191):
+    the long side becomes `size`, the other side other * size // long; a picture that fits is left as it is.  Raises
+    ValueError where the reference gives up with "Zero thumbnail output size"."""
+    if width <= size and height <= size:
+        return width, height
+    if width > height:
+        w, h = size, height * size // width
+    else:
+        w, h = width * size // height, size
+    if w == 0 or h == 0:
+        raise ValueError(f"{width} x {height} at size {size}: zero thumbnail output size")
+    return w, h

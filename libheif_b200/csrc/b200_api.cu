@@ -87,6 +87,16 @@ int b200_color_convert_device(const b200_planes* in, const b200_geometry* geom, 
   return launch_color(in, geom, opt, out, out_g, out_b, out_stride, (cudaStream_t)stream, pipeline);
 }
 
+int b200_color_convert_scaled_device(const b200_planes* in, const b200_geometry* geom, const b200_color_options* opt, int scale_w, int scale_h,
+                                     void* out, void* out_g, void* out_b, size_t out_stride, void* stream, int* pipeline) {
+  if (scale_w < 1) return set_error(B200_E_INVALID, "scale_w %d: the scaled picture needs at least one column", scale_w);
+  if (scale_h < 1) return set_error(B200_E_INVALID, "scale_h %d: the scaled picture needs at least one row", scale_h);
+  const void* const args[] = {in, geom, opt, out};
+  const char* const names[] = {"in", "geom", "opt", "out"};
+  for (int i = 0; i < 4; i++) if (!args[i]) return set_error(B200_E_INVALID, "%s is NULL", names[i]);
+  return launch_color(in, geom, opt, out, out_g, out_b, out_stride, (cudaStream_t)stream, pipeline, scale_w, scale_h);
+}
+
 static size_t out_row_bytes(int fmt, int w, int bit_depth_in) {
   switch (fmt) {
     case B200_CHROMA_INTERLEAVED_RGB: return (size_t)w * 3;

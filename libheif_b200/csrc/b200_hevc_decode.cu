@@ -668,10 +668,11 @@ struct DeviceRgb {                  // where decode_to_rgb_device left the RGB o
 // Common part of the fused entry points: decode -> colour conversion into one of the two device RGB buffers.  `direct_out`:
 // the page-locked destination the bands may be copied into as they are finished (nullptr: none).  The synchronous entry point
 // takes bands whenever the plan gives them; the asynchronous one, whose D2H already overlaps the next call's kernels, only
-// when B200_CHUNKS asks for them.
+// when B200_CHUNKS asks for them.  scale_w x scale_h > 0: the RGB scaled with HeifPixelImage::scale_nearest_neighbor, converted
+// from the finished canvas in one launch (no bands: the copy of a scaled result is small).
 static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size, uint64_t max_pixels, int canvas_w,
-                                int canvas_h, const b200_geometry* geom, const b200_color_options* opt, b200_image_info* info, int slot,
-                                void* direct_out, size_t direct_stride, bool async, DeviceRgb* res) {
+                                int canvas_h, const b200_geometry* geom, const b200_color_options* opt, int scale_w, int scale_h, b200_image_info* info,
+                                int slot, void* direct_out, size_t direct_stride, bool async, DeviceRgb* res) {
   const Overrides env = Overrides::read();
   cudaStream_t s = d->own;
   // the page-locked staging of the previous call must have left for the device before the host overwrites it
@@ -689,7 +690,8 @@ static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8
   // whole-picture one for the reference's default planner choice (nearest-neighbour chroma, per-sample arithmetic) without
   // rotate / mirror / crop; every other request converts the finished canvas in one go, below.
   bool banded = false; int hook_rc = B200_OK;
-  if (!geom && opt->chroma_upsampling == 0 && direct_out && (!async || env.bands == Overrides::ON)) {
+  const bool scaled = scale_w > 0 && scale_h > 0;
+  if (!scaled && !geom && opt->chroma_upsampling == 0 && direct_out && (!async || env.bands == Overrides::ON)) {
     d->band_hook = [&, slot, bpp](int c, cudaStream_t side) -> int {
       const b200_image_info& I = d->info;
       const int th = I.tile_height, y0 = std::min(I.height, (d->band_pic[c] / d->shape.cols) * th);
@@ -728,26 +730,26 @@ static int decode_to_rgb_device(b200_decoder* d, int cols, int rows, const uint8
   B200_CUDA_CHECK(cudaMemcpyAsync(&d->err_host.h[slot], d->sync.d + ScratchLayout::error_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, s));   // this step's error flag (the next step clears the device copy)
   b200_planes pl; if ((rc = b200_decoder_get_planes(d, &pl))) return rc;
   b200_geometry g; if (geom) g = *geom; else b200_geometry_identity(inf.width, inf.height, &g);
-  const size_t rowb = (size_t)g.out_w * bpp, pitch = (rowb + 255) & ~(size_t)255;
+  const int ow = scaled ? scale_w : g.out_w, oh = scaled ? scale_h : g.out_h;
+  const size_t rowb = (size_t)ow * bpp, pitch = (rowb + 255) & ~(size_t)255;
   if (!banded) {
-    if ((rc = d->rgb2[slot].reserve(pitch * g.out_h, false))) return rc;
+    if ((rc = d->rgb2[slot].reserve(pitch * oh, false))) return rc;
     B200_CUDA_CHECK(cudaStreamWaitEvent(s, d->ev_d2h[slot], 0));           // the copy that last read this buffer has finished
-    if ((rc = b200_color_convert_device(&pl, &g, opt, d->rgb2[slot].d, nullptr, nullptr, pitch, s, nullptr))) return rc;
+    if ((rc = b200_color_convert_scaled_device(&pl, &g, opt, ow, oh, d->rgb2[slot].d, nullptr, nullptr, pitch, s, nullptr))) return rc;
   }
   B200_CUDA_CHECK(cudaEventRecord(d->ev_k6[slot], s));
-  res->rowb = rowb; res->pitch = pitch; res->height = g.out_h; res->bands_copied = banded;
+  res->rowb = rowb; res->pitch = pitch; res->height = oh; res->bands_copied = banded;
   return B200_OK;
 }
 
-extern "C" {
-
-int b200_decode_grid_to_rgb_host(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
-                                 uint64_t max_pixels, int canvas_w, int canvas_h, const b200_geometry* geom,
-                                 const b200_color_options* opt, void* out, size_t out_stride, b200_image_info* info) {
-  if (!d || !opt || !out) return set_error(B200_E_INVALID, "null argument");
+// The synchronous fused entry points (scale_w x scale_h: 0 x 0 = unscaled)
+static int decode_to_rgb_host(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size, uint64_t max_pixels, int canvas_w,
+                              int canvas_h, const b200_geometry* geom, const b200_color_options* opt, int scale_w, int scale_h, void* out,
+                              size_t out_stride, b200_image_info* info) {
   const bool pinned = is_page_locked(out);
   DeviceRgb r;
-  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, info, 0, pinned ? out : nullptr, out_stride, false, &r);
+  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, scale_w, scale_h, info, 0, pinned ? out : nullptr,
+                                out_stride, false, &r);
   if (rc) return rc;
   cudaStream_t s = d->own;
   if (r.bands_copied) {                                 // the bands left through the copy stream as they were finished
@@ -763,6 +765,28 @@ int b200_decode_grid_to_rgb_host(b200_decoder* d, int cols, int rows, const uint
   return B200_OK;
 }
 
+extern "C" {
+
+int b200_decode_grid_to_rgb_host(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
+                                 uint64_t max_pixels, int canvas_w, int canvas_h, const b200_geometry* geom,
+                                 const b200_color_options* opt, void* out, size_t out_stride, b200_image_info* info) {
+  if (!d || !opt || !out) return set_error(B200_E_INVALID, "null argument");
+  return decode_to_rgb_host(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, 0, 0, out, out_stride, info);
+}
+
+// heif_decode_image + heif_image_scale_image (heif-thumbnailer) in one call: the scaled result is all that is converted and copied
+int b200_decode_grid_to_rgb_scaled_host(b200_decoder* d, int cols, int rows, const uint8_t* const* au, const size_t* au_size,
+                                        uint64_t max_pixels, int canvas_w, int canvas_h, const b200_geometry* geom,
+                                        const b200_color_options* opt, int scale_w, int scale_h, void* out, size_t out_stride,
+                                        b200_image_info* info) {
+  if (scale_w < 1) return set_error(B200_E_INVALID, "scale_w %d: the scaled picture needs at least one column", scale_w);
+  if (scale_h < 1) return set_error(B200_E_INVALID, "scale_h %d: the scaled picture needs at least one row", scale_h);
+  const void* const args[] = {d, au, au_size, opt, out};
+  const char* const names[] = {"dec", "au", "au_size", "opt", "out"};
+  for (int i = 0; i < 5; i++) if (!args[i]) return set_error(B200_E_INVALID, "%s is NULL", names[i]);
+  return decode_to_rgb_host(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, scale_w, scale_h, out, out_stride, info);
+}
+
 // Throughput form of the fused entry point: returns once the work is queued (the host part -- header parsing, packing -- is
 // done); the RGB reaches `out` (page-locked memory, see b200_host_alloc) through a second stream, so the D2H of picture i
 // overlaps the kernels of picture i + 1 (two device RGB buffers).  b200_decoder_wait() blocks until everything submitted
@@ -775,7 +799,7 @@ int b200_decode_grid_to_rgb_host_async(b200_decoder* d, int cols, int rows, cons
   const int slot = d->async_slot; d->async_slot ^= 1;
   if (d->err_host.h[slot]) d->async_error = true;                 // the step that used this slot two calls ago failed
   DeviceRgb r;
-  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, info, slot, out, out_stride, true, &r);
+  int rc = decode_to_rgb_device(d, cols, rows, au, au_size, max_pixels, canvas_w, canvas_h, geom, opt, 0, 0, info, slot, out, out_stride, true, &r);
   if (rc) return rc;
   if (!r.bands_copied) {
     B200_CUDA_CHECK(cudaStreamWaitEvent(d->copy, d->ev_k6[slot], 0));

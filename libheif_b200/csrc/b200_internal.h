@@ -38,8 +38,9 @@ inline bool is_identity(const int m[6], int w, int h, int w_in, int h_in) {
 }
 
 void ycbcr_to_rgb_coefficients(int matrix, int primaries, float out[4]);
+// scale_w x scale_h > 0: the result scaled with HeifPixelImage::scale_nearest_neighbor (0 x 0: the geometry's size)
 int launch_color(const b200_planes* in, const b200_geometry* g, const b200_color_options* opt, void* out, void* out_g,
-                 void* out_b, size_t out_stride, cudaStream_t stream, int* pipeline);
+                 void* out_b, size_t out_stride, cudaStream_t stream, int* pipeline, int scale_w = 0, int scale_h = 0);
 int launch_rgb_to_ycbcr(const void* rgb, size_t rgb_stride, int has_alpha, const b200_planes* out, cudaStream_t stream);
 int plan_rgb_to_ycbcr(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, int* pipeline);
 int launch_rgb_to_ycbcr_ex(const b200_rgb_image* in, const b200_planes* out, const b200_rgb_to_ycbcr_options* opt, cudaStream_t stream, int* pipeline);

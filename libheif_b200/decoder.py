@@ -102,24 +102,31 @@ class Decoder:
         _lib.check(self.l.b200_decoder_get_stats(self.h, C.byref(st)))
         return st
 
-    def to_rgb_device(self, out_chroma: int, geometry: Optional[Geometry] = None, out=None, stream=None):
-        """Colour post-stage on the canvas, device -> device (torch tensor result)."""
+    def to_rgb_device(self, out_chroma: int, geometry: Optional[Geometry] = None, out=None, stream=None, scale=None):
+        """Colour post-stage on the canvas, device -> device (torch tensor result).  scale=(w, h): the result scaled to w x h
+        with the reference's nearest-neighbour scaler, only the kept pixels converted (b200_color_convert_scaled_device)."""
         import torch
         p = self.planes_device()
         geom = geometry or Geometry(p.width, p.height)
-        ow, oh = geom.size
+        ow, oh = scale or geom.size
         bpp = _BYTES_PER_PIXEL[out_chroma]
         if out is None:
             out = torch.empty((oh, ow * bpp), dtype=torch.uint8, device="cuda")
         opt = _lib.ColorOptions(out_chroma, 0, 0)
         s = C.c_void_p(stream.cuda_stream) if stream is not None else C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _lib.check(self.l.b200_color_convert_device(C.byref(p), C.byref(geom.g), C.byref(opt), out.data_ptr(), None, None,
-                                                    out.stride(0), s, None))
+        if scale is None:
+            _lib.check(self.l.b200_color_convert_device(C.byref(p), C.byref(geom.g), C.byref(opt), out.data_ptr(), None, None,
+                                                        out.stride(0), s, None))
+        else:
+            _lib.check(self.l.b200_color_convert_scaled_device(C.byref(p), C.byref(geom.g), C.byref(opt), int(ow), int(oh), out.data_ptr(),
+                                                               None, None, out.stride(0), s, None))
         return out
 
     def decode_grid_to_rgb_host(self, aus: Sequence[bytes], cols: int, rows: int, out_chroma: int, canvas=(0, 0), geometry: Optional[Geometry] = None,
-                                out: Optional[np.ndarray] = None, max_image_size_pixels: int = 0):
-        """heif_decode_image() equivalent on the fused path: HEVC tiles in host memory -> interleaved RGB in host memory."""
+                                out: Optional[np.ndarray] = None, max_image_size_pixels: int = 0, scale=None):
+        """heif_decode_image() equivalent on the fused path: HEVC tiles in host memory -> interleaved RGB in host memory.
+        scale=(w, h): heif_decode_image + heif_image_scale_image in one call (b200_decode_grid_to_rgb_scaled_host); `out` is
+        then [h, w*bytes_per_pixel] and only the scaled picture is converted and copied."""
         arr, sizes = self._aus(aus)
         info = ImageInfo()
         bpp = _BYTES_PER_PIXEL[out_chroma]
@@ -129,8 +136,13 @@ class Decoder:
             # to pass `out` for big images; small ones use a probe of tile size * grid
             raise ValueError("pass a preallocated `out` array [H, W*bytes_per_pixel] (uint8)")
         g = C.byref(geometry.g) if geometry is not None else None
-        _lib.check(self.l.b200_decode_grid_to_rgb_host(self.h, cols, rows, arr, sizes, max_image_size_pixels, canvas[0], canvas[1], g,
-                                                       C.byref(opt), out.ctypes.data, out.strides[0], C.byref(info)))
+        if scale is None:
+            _lib.check(self.l.b200_decode_grid_to_rgb_host(self.h, cols, rows, arr, sizes, max_image_size_pixels, canvas[0], canvas[1], g,
+                                                           C.byref(opt), out.ctypes.data, out.strides[0], C.byref(info)))
+        else:
+            _lib.check(self.l.b200_decode_grid_to_rgb_scaled_host(self.h, cols, rows, arr, sizes, max_image_size_pixels, canvas[0], canvas[1], g,
+                                                                  C.byref(opt), int(scale[0]), int(scale[1]), out.ctypes.data, out.strides[0],
+                                                                  C.byref(info)))
         self.info = info
         return out, info
 
